@@ -8,7 +8,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libhorizonnet_b200.so')
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 _lib = None
 _lock = threading.Lock()
@@ -45,6 +45,8 @@ SIGNATURES = {
                            + [ctypes.c_int] * 7 + [vp, vp, vp]),
     'hn_conv2d_wgrad_tc': (ctypes.c_int, [vp] + [ctypes.c_int] * 4 + [vp] + [ctypes.c_int] * 7 + [vp, vp]),
     'hn_wgrad_tc_plan': (ctypes.c_int, [ctypes.c_int] * 12 + [c_int_p]),
+    'hn_conv2d_dgrad_tc': (ctypes.c_int, [ctypes.c_int] * 4 + [vp, vp] + [ctypes.c_int] * 7 + [vp, vp]),
+    'hn_conv_tc_plan': (ctypes.c_int, [ctypes.c_int] * 16 + [c_int_p]),
     'hn_wgrad_tc_enabled': (ctypes.c_int, []),
     'hn_bn_forward_backward': (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp,
                                               ctypes.c_double, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp,

@@ -1078,13 +1078,9 @@ bool tc_prefetch_on() {
 }
 
 template <int BN>
-int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcArgs& a, cudaStream_t st) {
+int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcArgs& a, int grid, cudaStream_t st) {
     using S = Smem<BN>;
     HN_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    int dev = 0, sms = 0;
-    HN_CUDA_OK(cudaGetDevice(&dev));
-    HN_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const int grid = a.num_tiles < sms ? a.num_tiles : sms;
     HN_CUDA_OK(launch_tc(conv_tc_kernel<BN>, grid, S::TOTAL, st, tmA, tmB, a));
     HN_LAUNCH_OK();
     return 0;
@@ -1106,15 +1102,11 @@ bool conv_tc_supported(const ConvDesc& d, const Act& in, const Act& out) {
     return true;
 }
 
-// in / out / residual are split plane pairs in halo-NHWC geometry (hi plane, then lo plane).
-// wq: [2][Cout][K] weight planes, K = (dy*kw+dx)*Cin + c; tc_scale folds BN scale and the plane scales.
-int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_aux, const Act& in,
-                   const unsigned short* in_planes, const Act& out, unsigned short* out_planes, float* out_f32,
-                   const unsigned short* res_planes, cudaStream_t st) {
+int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32, bool has_residual, int sms, TcPlan* p) {
     HN_CHECK(conv_tc_supported(d, in, out), "conv_tc: unsupported shape");
-    const int K = d.kh * d.kw * d.Cin;
-    TcArgs a;
-    memset(&a, 0, sizeof(a));
+    HN_CHECK(!(out_f32 && has_residual), "conv_tc: residual with fp32 output is not supported");
+    HN_CHECK(sms >= 1, "conv_tc_plan: sms must be positive");
+    memset(p, 0, sizeof(*p));
     const bool gemm = (d.kh == 1 && d.kw == 1 && d.sh == 1 && d.sw == 1 && in.halo == out.halo);
     int BN = d.Cout >= 128 ? 128 : d.Cout;
     {   // layers with too few 128x128 tiles to fill the SMs (the tail of the height-reduction convs): halve the tile width
@@ -1122,6 +1114,68 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
         const long long tiles128 = ((rows + BM - 1) / BM) * (d.Cout / 128 > 0 ? d.Cout / 128 : 1);
         if (BN == 128 && tiles128 < 110) BN = 64;
     }
+    p->num_kc = d.kh * d.kw * (d.Cin / BKC);
+    p->seg = tc_segment_chunks();
+    p->box_rows = p->box_imgs = 1;
+    long long m_tiles;
+    // asynchronous-epilogue GEMM kernel: plane output, K <= 512, Cout a multiple of 64
+    static const bool gemm_kernel_on = [] { const char* e = getenv("HN_TC_GEMM"); return !(e && atoi(e) == 0); }();
+    if (gemm && gemm_kernel_on && !out_f32 && d.Cin <= 256 && d.Cout % GBN == 0 && d.Cout <= GSmem::MAX_COUT) {
+        const long long Mtot = (long long)in.B * in.H * in.Wp();
+        p->gemm_kernel = 1;
+        p->BN = GBN;
+        p->mode = 0;
+        p->M = (int)Mtot;
+        // L2 prefetch two tile rounds ahead for the K = 64 layers (one activation box per tile); the K = 256 layers
+        // already keep 8 boxes per tile in flight
+        p->pf = (tc_prefetch_on() && p->num_kc == 1) ? 2 : 0;
+        m_tiles = (Mtot + BM - 1) / BM;
+    } else if (gemm) {
+        p->BN = BN;
+        p->mode = 0;
+        p->M = (int)((long long)in.B * in.H * in.Wp());
+        m_tiles = ((long long)p->M + BM - 1) / BM;
+    } else {
+        p->BN = BN;
+        p->mode = 1;
+        p->M = out.B * out.H;
+        p->tw = out.W < 128 ? out.W : 128;
+        p->rows_per_tile = BM / p->tw;
+        p->wsegs = out.W / p->tw;
+        p->parity = (d.sw == 2);
+        // one box for all rows of a tile when they are consecutive input rows of one image (stride 1 along H)
+        static const bool rowbox_on = [] { const char* e = getenv("HN_TC_ROWBOX"); return !(e && atoi(e) == 0); }();
+        static const bool rowbox2_on = [] { const char* e = getenv("HN_TC_ROWBOX2"); return !(e && atoi(e) == 0); }();
+        // ... or whole images when an image has fewer output rows than a tile (the last height-reduction convs):
+        // the box then spans R / Ho consecutive images of the plane
+        if (rowbox_on && p->rows_per_tile > 1 && (d.sh == 1 || (d.sh == 2 && rowbox2_on))) {
+            if (out.H % p->rows_per_tile == 0) { p->rowbox = 1; p->box_rows = p->rows_per_tile; }
+            else if (p->rows_per_tile % out.H == 0) { p->rowbox = 1; p->box_rows = out.H; p->box_imgs = p->rows_per_tile / out.H; }
+        }
+        // dx reuse (HN_TC_DXR=0 disables)
+        static const int dxr_mode = [] { const char* e = getenv("HN_TC_DXR"); return e ? atoi(e) : 1; }();
+        p->dxr = (dxr_mode != 0 && !p->parity && d.kw == 3 && p->rows_per_tile == 1 && p->tw == BM &&
+                  (long long)p->wsegs * BM + (in.halo - d.pw) + 2 <= (long long)in.Wp()) ? 1 : 0;
+        m_tiles = (long long)((p->M + p->rows_per_tile - 1) / p->rows_per_tile) * p->wsegs;
+    }
+    p->n_tiles = d.Cout / p->BN;
+    HN_CHECK(m_tiles * p->n_tiles < (1ll << 31), "conv_tc: too many tiles");
+    p->num_tiles = (int)(m_tiles * p->n_tiles);
+    p->grid = p->num_tiles < sms ? p->num_tiles : sms;
+    return 0;
+}
+
+// in / out / residual are split plane pairs in halo-NHWC geometry (hi plane, then lo plane).
+// wq: [2][Cout][K] weight planes, K = (dy*kw+dx)*Cin + c; tc_scale folds BN scale and the plane scales.
+int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_aux, const Act& in,
+                   const unsigned short* in_planes, const Act& out, unsigned short* out_planes, float* out_f32,
+                   const unsigned short* res_planes, cudaStream_t st) {
+    TcPlan pl;
+    if (conv_tc_plan(d, in, out, out_f32 != nullptr, res_planes != nullptr, num_sms(), &pl)) return -1;
+    const int K = d.kh * d.kw * d.Cin;
+    const int BN = pl.BN;
+    TcArgs a;
+    memset(&a, 0, sizeof(a));
     const size_t in_plane = in.numel(), out_plane = out.numel();
     CUtensorMap tmA, tmB;
     {   // weights: {K, Cout, 2}
@@ -1131,29 +1185,22 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
         if (make_map(&tmB, wq, 3, dims, str, box)) return -1;
     }
     a.Cout = d.Cout;
-    a.n_tiles = d.Cout / BN;
+    a.n_tiles = pl.n_tiles;
+    a.num_tiles = pl.num_tiles;
     a.kw = d.kw;
     a.kc_per_tap = d.Cin / BKC;
-    a.num_kc = d.kh * d.kw * a.kc_per_tap;
-    HN_CHECK(!(out_f32 && res_planes), "conv_tc: residual with fp32 output is not supported");
+    a.num_kc = pl.num_kc;
     a.scale = out_f32 ? tc_aux : tc_aux + d.Cout;            // fp32 outputs in true units, planes in plane units
     a.shift = out_f32 ? d.shift : tc_aux + 2 * d.Cout;
     a.res = res_planes; a.out = out_planes; a.out_f32 = out_f32; a.out_plane = out_plane; a.relu = d.relu;
     a.Bimg = in.B;
-    a.seg = tc_segment_chunks();
+    a.seg = pl.seg;
     { static int dbg = [] { const char* e = getenv("HN_TC_DBG"); return e ? atoi(e) : 0; }(); a.dbg = dbg; }
-    long long m_tiles;
-    // asynchronous-epilogue GEMM kernel: plane output, K <= 512, Cout a multiple of 64
-    static const bool gemm_kernel_on = [] { const char* e = getenv("HN_TC_GEMM"); return !(e && atoi(e) == 0); }();
-    const bool use_gemm_kernel = gemm && gemm_kernel_on && !out_f32 && d.Cin <= 256 && d.Cout % GBN == 0 && d.Cout <= GSmem::MAX_COUT;
-    if (use_gemm_kernel) {
-        const long long Mtot = (long long)in.B * in.H * in.Wp();
-        a.mode = 0;
-        a.M = (int)Mtot;
-        a.n_tiles = d.Cout / GBN;
-        // L2 prefetch two tile rounds ahead for the K = 64 layers (one activation box per tile); the K = 256 layers
-        // already keep 8 boxes per tile in flight
-        a.pf = (tc_prefetch_on() && a.num_kc == 1) ? 2 : 0;
+    a.mode = pl.mode;
+    a.M = pl.M;
+    if (pl.gemm_kernel) {
+        const long long Mtot = pl.M;
+        a.pf = pl.pf;
         CUtensorMap tmR, tmO;
         {
             cuuint64_t dims[3] = {(cuuint64_t)d.Cin, (cuuint64_t)Mtot, 2};
@@ -1162,86 +1209,52 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
             if (make_map(&tmA, in_planes, 3, dims, str, box)) return -1;
         }
         {
-            cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)d.Cout, 2};
-            cuuint64_t str[2] = {(cuuint64_t)K * 2, (cuuint64_t)K * d.Cout * 2};
-            cuuint32_t box[3] = {BKC, GBN, 1};
-            if (make_map(&tmB, wq, 3, dims, str, box)) return -1;
-        }
-        {
             cuuint64_t dims[3] = {(cuuint64_t)d.Cout, (cuuint64_t)Mtot, 2};
             cuuint64_t str[2] = {(cuuint64_t)d.Cout * 2, (cuuint64_t)out_plane * 2};
             cuuint32_t box[3] = {GBN, BM, 1};
             if (make_map(&tmO, out_planes, 3, dims, str, box)) return -1;
             if (make_map(&tmR, res_planes ? res_planes : out_planes, 3, dims, str, box)) return -1;
         }
-        const long long mt = (Mtot + BM - 1) / BM;
-        HN_CHECK(mt * a.n_tiles < (1ll << 31), "conv_tc: too many tiles");
-        a.num_tiles = (int)(mt * a.n_tiles);
-        int dev = 0, sms = 0;
-        HN_CUDA_OK(cudaGetDevice(&dev));
-        HN_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         HN_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GSmem::TOTAL));
-        HN_CUDA_OK(launch_tc(gemm_tc_kernel, a.num_tiles < sms ? a.num_tiles : sms, GSmem::TOTAL, st, tmA, tmB, tmR, tmO, a));
+        HN_CUDA_OK(launch_tc(gemm_tc_kernel, pl.grid, GSmem::TOTAL, st, tmA, tmB, tmR, tmO, a));
         HN_LAUNCH_OK();
         return 0;
     }
-    if (gemm) {
-        const long long Mtot = (long long)in.B * in.H * in.Wp();
-        a.mode = 0;
-        a.M = (int)Mtot;
-        cuuint64_t dims[3] = {(cuuint64_t)d.Cin, (cuuint64_t)Mtot, 2};
+    if (pl.mode == 0) {
+        cuuint64_t dims[3] = {(cuuint64_t)d.Cin, (cuuint64_t)pl.M, 2};
         cuuint64_t str[2] = {(cuuint64_t)d.Cin * 2, (cuuint64_t)in_plane * 2};
         cuuint32_t box[3] = {BKC, BM, 1};
         if (make_map(&tmA, in_planes, 3, dims, str, box)) return -1;
-        m_tiles = (Mtot + BM - 1) / BM;
     } else {
-        a.mode = 1;
         a.Ho = out.H; a.Wo = out.W; a.Wop = out.Wp(); a.out_halo = out.halo;
-        a.M = out.B * out.H;
-        a.tw = out.W < 128 ? out.W : 128;
-        a.rows_per_tile = BM / a.tw;
-        a.wsegs = out.W / a.tw;
+        a.tw = pl.tw;
+        a.rows_per_tile = pl.rows_per_tile;
+        a.wsegs = pl.wsegs;
         a.sh = d.sh; a.ph = d.ph; a.woff = in.halo - d.pw;
-        a.parity = (d.sw == 2);
-        // one box for all rows of a tile when they are consecutive input rows of one image (stride 1 along H)
-        static const bool rowbox_on = [] { const char* e = getenv("HN_TC_ROWBOX"); return !(e && atoi(e) == 0); }();
-        static const bool rowbox2_on = [] { const char* e = getenv("HN_TC_ROWBOX2"); return !(e && atoi(e) == 0); }();
-        // ... or whole images when an image has fewer output rows than a tile (the last height-reduction convs):
-        // the box then spans R / Ho consecutive images of the plane
-        int box_rows = 1, box_imgs = 1;
-        a.rowbox = 0;
-        if (rowbox_on && a.rows_per_tile > 1 && (d.sh == 1 || (d.sh == 2 && rowbox2_on))) {
-            if (out.H % a.rows_per_tile == 0) { a.rowbox = 1; box_rows = a.rows_per_tile; }
-            else if (a.rows_per_tile % out.H == 0) { a.rowbox = 1; box_rows = out.H; box_imgs = a.rows_per_tile / out.H; }
-        }
+        a.parity = pl.parity;
+        a.rowbox = pl.rowbox;
+        a.dxr = pl.dxr;
         // stride 2 along H (height-reduction convs): the box spans 2*rows input rows and takes every second one
-        const cuuint32_t boxrows = a.rowbox ? (cuuint32_t)(box_rows * d.sh) : 1u;
+        const cuuint32_t boxrows = a.rowbox ? (cuuint32_t)(pl.box_rows * d.sh) : 1u;
         const int hs = (a.rowbox && d.sh == 2) ? 2 : 1;
         const cuuint64_t C2 = (cuuint64_t)d.Cin * 2, Wp = in.Wp();
-        // dx reuse (HN_TC_DXR=0 disables)
-        static const int dxr_mode = [] { const char* e = getenv("HN_TC_DXR"); return e ? atoi(e) : 1; }();
-        a.dxr = (dxr_mode != 0 && !a.parity && d.kw == 3 && a.rows_per_tile == 1 && a.tw == BM &&
-                 (long long)a.wsegs * BM + a.woff + 2 <= (long long)Wp) ? 1 : 0;
         if (!a.parity) {
             cuuint64_t dims[4] = {(cuuint64_t)d.Cin, Wp, (cuuint64_t)in.H, (cuuint64_t)2 * in.B};
             cuuint64_t str[3] = {C2, C2 * Wp, C2 * Wp * in.H};
-            cuuint32_t box[4] = {BKC, a.dxr ? 130u : (cuuint32_t)a.tw, boxrows, (cuuint32_t)box_imgs};
+            cuuint32_t box[4] = {BKC, a.dxr ? 130u : (cuuint32_t)a.tw, boxrows, (cuuint32_t)pl.box_imgs};
             if (make_map(&tmA, in_planes, 4, dims, str, box, hs == 2 ? 2 : -1, hs)) return -1;
         } else {
             cuuint64_t dims[5] = {(cuuint64_t)d.Cin, 2, Wp / 2, (cuuint64_t)in.H, (cuuint64_t)2 * in.B};
             cuuint64_t str[4] = {C2, 2 * C2, C2 * Wp, C2 * Wp * in.H};
-            cuuint32_t box[5] = {BKC, 1, (cuuint32_t)a.tw, boxrows, (cuuint32_t)box_imgs};
+            cuuint32_t box[5] = {BKC, 1, (cuuint32_t)a.tw, boxrows, (cuuint32_t)pl.box_imgs};
             if (make_map(&tmA, in_planes, 5, dims, str, box, hs == 2 ? 3 : -1, hs)) return -1;
         }
-        m_tiles = (long long)((a.M + a.rows_per_tile - 1) / a.rows_per_tile) * a.wsegs;
     }
-    HN_CHECK(m_tiles * a.n_tiles < (1ll << 31), "conv_tc: too many tiles");
-    a.num_tiles = (int)(m_tiles * a.n_tiles);
     if (a.num_tiles == 0) return 0;
     switch (BN) {
-        case 128: return launch<128>(tmA, tmB, a, st);
-        case 64: return launch<64>(tmA, tmB, a, st);
-        default: return launch<32>(tmA, tmB, a, st);
+        case 128: return launch<128>(tmA, tmB, a, pl.grid, st);
+        case 64: return launch<64>(tmA, tmB, a, pl.grid, st);
+        default: return launch<32>(tmA, tmB, a, pl.grid, st);
     }
 }
 
@@ -1483,24 +1496,30 @@ int tc_aux_update(const float* scale, const float* shift, const float* absmax, f
     return 0;
 }
 
-// Unit-test convenience: fp32 halo-NHWC in and out, planes built on the fly.
-int conv_tc(const ConvDesc& d, const Act& in, const Act& out, const float* residual, cudaStream_t st) {
+// Unit-test convenience: fp32 halo-NHWC in and out, planes built on the fly; out_f32: the kernel's fp32 epilogue writes
+// `out` directly (true-unit scale, d.shift) instead of planes that are merged afterwards.
+int conv_tc(const ConvDesc& d, const Act& in, const Act& out, const float* residual, bool out_f32, cudaStream_t st) {
     HN_CHECK(conv_tc_supported(d, in, out), "conv_tc: unsupported shape");
+    HN_CHECK(!(out_f32 && residual), "conv_tc: residual with fp32 output is not supported");
     const size_t K = (size_t)d.kh * d.kw * d.Cin;
     const size_t n_in = in.numel(), n_out = out.numel(), n_w = K * d.Cout;
     unsigned short *pin = nullptr, *pout = nullptr, *pres = nullptr, *pw = nullptr;
     float* aux = nullptr;          // [3*Cout] tc_aux + 1 scratch float
     HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&pin), n_in * 4, st));
-    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&pout), n_out * 4, st));
+    if (!out_f32) {   // all-ones fp16 = NaN: an output plane element the kernel leaves unwritten merges to NaN
+        HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&pout), n_out * 4, st));
+        HN_CUDA_OK(cudaMemsetAsync(pout, 0xff, n_out * 4, st));
+    }
     HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&pw), n_w * 4, st));
     HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&aux), (3 * d.Cout + 1) * sizeof(float), st));
     if (residual) HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&pres), n_out * 4, st));
     int rc = split_planes(in.p, pin, n_in, st);
     if (!rc && residual) rc = split_planes(residual, pres, n_out, st);
     if (!rc) rc = pack_weight_impl<false>(d.w, pw, d.scale, d.shift, aux, aux + 3 * d.Cout, d.Cout, d.Cin, d.kh, d.kw, st);
-    if (!rc) rc = conv_tc_planes(d, pw, aux, in, pin, out, pout, nullptr, pres, st);
-    if (!rc) rc = merge_planes(pout, out.p, n_out, st);
-    cudaFreeAsync(pin, st); cudaFreeAsync(pout, st); cudaFreeAsync(pw, st); cudaFreeAsync(aux, st);
+    if (!rc) rc = conv_tc_planes(d, pw, aux, in, pin, out, pout, out_f32 ? out.p : nullptr, pres, st);
+    if (!rc && !out_f32) rc = merge_planes(pout, out.p, n_out, st);
+    cudaFreeAsync(pin, st); cudaFreeAsync(pw, st); cudaFreeAsync(aux, st);
+    if (pout) cudaFreeAsync(pout, st);
     if (pres) cudaFreeAsync(pres, st);
     return rc;
 }

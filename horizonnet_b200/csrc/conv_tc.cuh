@@ -56,8 +56,25 @@ __device__ __forceinline__ float pow2_factor(float absmax) {
 }
 
 bool conv_tc_supported(const ConvDesc& d, const Act& in, const Act& out);
-// fp32 halo-NHWC in/out convenience wrapper (unit tests): splits, runs the plane kernel, merges.
-int conv_tc(const ConvDesc& d, const Act& in, const Act& out, const float* residual, cudaStream_t st);
+// Launch plan of conv_tc_planes for one shape (host only): which kernel, tile shape, operand boxes and grid.
+struct TcPlan {
+    int gemm_kernel;          // 1: gemm_tc_kernel (asynchronous epilogue), 0: conv_tc_kernel
+    int BN;                   // output channels per tile (128, 64 or 32)
+    int mode;                 // 0: GEMM rows over all halo-NHWC pixels, 1: conv rows
+    int M;                    // mode 0: pixel rows, mode 1: B * Ho output rows
+    int tw, rows_per_tile, wsegs;          // mode 1: tile columns, output rows per tile, tiles per output row
+    int rowbox, box_rows, box_imgs;        // one TMA box for all rows of a tile: rows of one image x images
+    int dxr, parity;                       // 3x3 dx reuse of one 130-pixel input row; stride 2 along W (parity view)
+    int num_kc, seg;                       // K chunks of 64; chunks per tensor-core accumulation segment
+    int pf;                                // gemm_tc_kernel: L2 prefetch distance in tile rounds, 0 = off
+    int n_tiles, num_tiles, grid;          // tiles along Cout, all tiles, CTAs (persistent, min(num_tiles, sms))
+};
+// Reads the HN_TC_* switches; -1 (with hn_last_error set) for a shape conv_tc_supported rejects or a residual with fp32
+// output.  conv_tc_planes launches exactly this plan.
+int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32, bool has_residual, int sms, TcPlan* p);
+// fp32 halo-NHWC in/out convenience wrapper (unit tests): splits, runs the plane kernel, merges the output planes, or with
+// out_f32 lets the kernel write fp32 directly (the epilogue of the LSTM projections and of the data gradient; no residual).
+int conv_tc(const ConvDesc& d, const Act& in, const Act& out, const float* residual, bool out_f32, cudaStream_t st);
 // The real thing: operands and result are split planes.  wq: [2][Cout][K] weight planes
 // (fp16 hi, fp16 lo of w * 2^t); tc_aux = 3*Cout floats written by pack_weight_tc:
 //   [0,C)  accumulator -> true units   (BN scale * 2^(4-t)),  used with d.shift for fp32 outputs

@@ -248,7 +248,7 @@ int conv_bn(hn_model* m, const ConvLayer& c, const Act& in, const Act& out, cons
 extern "C" {
 
 const char* hn_last_error(void) { return g_err.c_str(); }
-int hn_abi_version(void) { return 2; }
+int hn_abi_version(void) { return 3; }
 const char* hn_build_digest(void) { return HN_BUILD_DIGEST; }
 long long hn_kernel_launches(void) { return g_launches.load(); }
 
@@ -968,11 +968,31 @@ int hn_conv2d(const float* in, int B, int H, int W, int Cin, int in_halo, const 
     Act a = mk(const_cast<float*>(in), B, H, W, Cin, in_halo);
     const int Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
     Act o = mk(out, B, Ho, Wo, Cout, out_halo);
-    if (impl == 1) {
+    if (impl == 1 || impl == 2) {
         if (!conv_tc_supported(d, a, o)) return fail("hn_conv2d: shape not supported by the tensor-core kernel");
-        return conv_tc(d, a, o, residual, (cudaStream_t)stream);
+        if (impl == 2 && residual) return fail("hn_conv2d: the fp32-output tensor-core epilogue takes no residual");
+        return conv_tc(d, a, o, residual, impl == 2, (cudaStream_t)stream);
     }
+    HN_CHECK(impl == 0, "hn_conv2d: impl must be 0, 1 or 2");
     return conv_f32(d, a, o, residual, (cudaStream_t)stream);
+}
+
+// Launch plan of the tensor-core convolution for one shape (no GPU work): the one conv_tc_planes launches with.
+int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
+                    int out_halo, int out_f32, int has_residual, int sms, int plan[18]) {
+    HN_CHECK(plan, "hn_conv_tc_plan: NULL argument");
+    HN_CHECK(B >= 1 && H >= 1 && W >= 1 && kh >= 1 && kw >= 1 && sh >= 1 && sw >= 1 && in_halo >= 0 && out_halo >= 0,
+             "hn_conv_tc_plan: bad geometry");
+    ConvDesc d;
+    d.Cin = Cin; d.Cout = Cout; d.kh = kh; d.kw = kw; d.sh = sh; d.sw = sw; d.ph = ph; d.pw = pw;
+    const Act a = mk(nullptr, B, H, W, Cin, in_halo);
+    const Act o = mk(nullptr, B, (H + 2 * ph - kh) / sh + 1, (W + 2 * pw - kw) / sw + 1, Cout, out_halo);
+    TcPlan p;
+    if (conv_tc_plan(d, a, o, out_f32 != 0, has_residual != 0, sms, &p)) return -1;
+    const int v[18] = {p.gemm_kernel, p.BN, p.mode, p.M, p.tw, p.rows_per_tile, p.wsegs, p.rowbox, p.box_rows, p.box_imgs,
+                       p.dxr, p.parity, p.num_kc, p.seg, p.pf, p.n_tiles, p.num_tiles, p.grid};
+    memcpy(plan, v, sizeof(v));
+    return 0;
 }
 
 int hn_lstm_layer(const float* xproj, const float* whf, const float* whb, float* out, int T, int B, void* stream) {

@@ -287,6 +287,56 @@ Act grad_of(const TrainState* ts, const Act& y) {
     return g;
 }
 
+// ---- data gradient on the tensor cores: the transposed convolution as a stride-1 convolution of dz (zero-dilated for a
+// strided conv) with the flipped weights, fp32 result added to din
+struct DgradTc {
+    ConvDesc t;               // the transposed convolution: Cin <-> Cout, padding kh-1-ph, kw-1-pw
+    Act src;                  // its input: dz, or the dilated copy in din's geometry with Cout channels
+    Act landing;              // its fp32 output, din's geometry
+};
+
+DgradTc dgrad_tc_geometry(const ConvDesc& d, const Act& dz, const Act& din, float* dil, float* landing) {
+    DgradTc g;
+    g.t.Cin = d.Cout; g.t.Cout = d.Cin; g.t.kh = d.kh; g.t.kw = d.kw;
+    g.t.ph = d.kh - 1 - d.ph; g.t.pw = d.kw - 1 - d.pw;
+    g.src = dz;
+    if (d.sh != 1 || d.sw != 1) { g.src = din; g.src.C = d.Cout; g.src.p = dil; }
+    g.landing = din; g.landing.p = landing;
+    return g;
+}
+
+bool dgrad_tc_supported(const ConvDesc& d, const Act& dz, const Act& din) {
+    const DgradTc g = dgrad_tc_geometry(d, dz, din, nullptr, nullptr);
+    return conv_tc_supported(g.t, g.src, g.landing);
+}
+
+struct DgradScratch {
+    float* dil;               // strided convs: din's pixels x Cout
+    float* landing;           // din.numel()
+    unsigned short* sp;       // planes of the (dilated) dz: 2 x its numel
+    float* wflip;             // Cout*Cin*kh*kw
+    unsigned short* wq;       // 2 x Cout*Cin*kh*kw
+    float* aux;               // 3*Cin + 1 (epilogue constants, weight absmax)
+    float* amax;              // 1: absmax of the (dilated) dz
+    const float* zeros;       // Cin zeros: the epilogue shift
+};
+
+// din += dgrad(dz; w).  sp_is_dz: sp / amax already hold the planes of dz (a stride-1 unit whose weight gradient split them).
+int dgrad_tc(const ConvDesc& d, const float* w_oihw, const Act& dz, const Act& din, const DgradScratch& s, bool sp_is_dz,
+             cudaStream_t st) {
+    DgradTc g = dgrad_tc_geometry(d, dz, din, s.dil, s.landing);
+    g.t.shift = s.zeros;
+    const bool strided = d.sh != 1 || d.sw != 1;
+    if (strided && dilate_for_dgrad(dz, g.src, d.sh, d.sw, st)) return -1;
+    if (!sp_is_dz && split_planes_pow2(g.src.p, s.sp, g.src.numel(), s.amax, st)) return -1;
+    if (flip_oihw(w_oihw, s.wflip, d.Cout, d.Cin, d.kh, d.kw, st)) return -1;
+    if (pack_weight_tc(s.wflip, s.wq, nullptr, nullptr, s.aux, s.aux + 3 * g.t.Cout, g.t.Cout, g.t.Cin, g.t.kh, g.t.kw, st))
+        return -1;
+    if (tc_aux_div_pow2(s.aux, g.t.Cout, s.amax, st)) return -1;      // planes of dz carry pow2_factor: divide it out
+    if (conv_tc_planes(g.t, s.wq, s.aux, g.src, s.sp, g.landing, nullptr, g.landing.p, nullptr, st)) return -1;
+    return add_inplace(din.p, g.landing.p, din.numel(), st);
+}
+
 int walk_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dcor, cudaStream_t st) {
     const int B = ts->units.front().z.B;
     const size_t rows = (size_t)T_STEPS * B, nseq = rows * 1024;
@@ -406,24 +456,11 @@ int walk_backward(hn_model* m, TrainState* ts, const float* dbon, const float* d
         MARK(2);
         if (u.is_stem) { MARK(3); continue; }                      // the image needs no gradient
         const Act din = grad_of(ts, u.in);
-        ConvDesc t;                                               // the transposed convolution as a stride-1 conv
-        t.Cin = u.d.Cout; t.Cout = u.d.Cin; t.kh = u.d.kh; t.kw = u.d.kw;
-        t.ph = u.d.kh - 1 - u.d.ph; t.pw = u.d.kw - 1 - u.d.pw; t.shift = ts->zeros;
-        Act src = dz;
-        if (strided) { src = din; src.C = u.d.Cout; src.p = ts->dil_scratch; }
-        Act landing = din; landing.p = ts->dtmp;
-        if (m->use_tc && conv_tc_supported(t, src, landing)) {
+        if (m->use_tc && dgrad_tc_supported(u.d, dz, din)) {
             // tensor cores: planes of the (dilated) dz, flipped weights packed as planes, fp32 result added to the gradient
-            if (strided && dilate_for_dgrad(dz, src, u.d.sh, u.d.sw, st)) return -1;
-            unsigned short* wq = reinterpret_cast<unsigned short*>(ts->wd_scratch);
-            if (!sp_is_dz && split_planes_pow2(src.p, sp, src.numel(), amax, st)) return -1;
-            if (flip_oihw(m->T(c.wkey), ts->dw_scratch, u.d.Cout, u.d.Cin, u.d.kh, u.d.kw, st)) return -1;
-            if (pack_weight_tc(ts->dw_scratch, wq, nullptr, nullptr, ts->aux_tmp, ts->aux_tmp + 3 * t.Cout, t.Cout, t.Cin, t.kh,
-                               t.kw, st))
-                return -1;
-            if (tc_aux_div_pow2(ts->aux_tmp, t.Cout, amax, st)) return -1;
-            if (conv_tc_planes(t, wq, ts->aux_tmp, src, sp, landing, nullptr, landing.p, nullptr, st)) return -1;
-            if (add_inplace(din.p, landing.p, din.numel(), st)) return -1;
+            const DgradScratch s = {ts->dil_scratch, ts->dtmp, sp, ts->dw_scratch,
+                                    reinterpret_cast<unsigned short*>(ts->wd_scratch), ts->aux_tmp, amax, ts->zeros};
+            if (dgrad_tc(u.d, m->T(c.wkey), dz, din, s, sp_is_dz, st)) return -1;
         } else {
             if (pack_dgrad_weight(m->T(c.wkey), ts->wd_scratch, u.d.Cout, u.d.Cin, u.d.kh, u.d.kw, st)) return -1;
             if (conv_dgrad_f32(u.d, ts->wd_scratch, dz, din, true, ts->dil_scratch, ts->ones, ts->zeros, st)) return -1;
@@ -612,6 +649,40 @@ int hn_conv2d_wgrad_tc(const float* in, int B, int H, int W, int Cin, const floa
     int rc = split_planes(a.p, ap, a.numel(), st) || split_planes_pow2(z.p, zp, z.numel(), amax, st) ||
              conv_wgrad_tc(d, a, ap, z, zp, amax, tmp, st) || ohwi_to_oihw(tmp, dw_oihw, Cout, Cin, kh, kw, st);
     cudaFreeAsync(tmp, st); cudaFreeAsync(amax, st); cudaFreeAsync(ap, st); cudaFreeAsync(zp, st);
+    return rc;
+}
+
+// Data gradient on the tensor cores through the training step's own dgrad_tc, added to din; the scratch TrainState
+// provides there is allocated here.  Fails for shapes the kernel does not take.
+int hn_conv2d_dgrad_tc(int B, int H, int W, int Cin, const float* w_oihw, const float* dz, int Cout, int kh, int kw, int sh,
+                       int sw, int ph, int pw, float* din, void* stream) {
+    HN_CHECK(w_oihw && dz && din, "hn_conv2d_dgrad_tc: NULL argument");
+    HN_CHECK(B >= 1 && H >= 1 && W >= 1 && kh >= 1 && kw >= 1 && sh >= 1 && sw >= 1, "hn_conv2d_dgrad_tc: bad geometry");
+    cudaStream_t st = (cudaStream_t)stream;
+    ConvDesc d;
+    d.Cin = Cin; d.Cout = Cout; d.kh = kh; d.kw = kw; d.sh = sh; d.sw = sw; d.ph = ph; d.pw = pw;
+    const int Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
+    const Act z = mk(const_cast<float*>(dz), B, Ho, Wo, Cout, 1);
+    const Act di = mk(din, B, H, W, Cin, 1);
+    HN_CHECK(dgrad_tc_supported(d, z, di), "hn_conv2d_dgrad_tc: shape not supported by the tensor-core kernel");
+    const bool strided = sh != 1 || sw != 1;
+    const size_t nw = (size_t)Cout * Cin * kh * kw, ndil = strided ? (size_t)B * H * (W + 2) * Cout : 0;
+    const size_t nsrc = strided ? ndil : z.numel();
+    float *dil = nullptr, *landing = nullptr, *wflip = nullptr, *aux = nullptr, *zeros = nullptr;
+    unsigned short *sp = nullptr, *wq = nullptr;
+    if (strided) HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dil), ndil * sizeof(float), st));
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&landing), di.numel() * sizeof(float), st));
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&sp), nsrc * 2 * sizeof(unsigned short), st));
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&wflip), nw * sizeof(float), st));
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&wq), nw * 2 * sizeof(unsigned short), st));
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&aux), (3 * (size_t)Cin + 2) * sizeof(float), st));
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&zeros), (size_t)Cin * sizeof(float), st));
+    const DgradScratch s = {dil, landing, sp, wflip, wq, aux, aux + 3 * Cin + 1, zeros};
+    int rc = fill_f32(zeros, Cin, 0.f, st);
+    if (!rc) rc = dgrad_tc(d, w_oihw, z, di, s, false, st);
+    if (dil) cudaFreeAsync(dil, st);
+    cudaFreeAsync(landing, st); cudaFreeAsync(sp, st); cudaFreeAsync(wflip, st); cudaFreeAsync(wq, st);
+    cudaFreeAsync(aux, st); cudaFreeAsync(zeros, st);
     return rc;
 }
 

@@ -62,7 +62,7 @@ int hn_model_forward(hn_model* m, const float* x_nchw_dev, int batch, int in_cha
                      float* bon_dev, float* cor_dev, void* stream);
 
 /* Throughput form of hn_model_forward for streams of batches.  The forward is split over two internal streams:
- * the encoder + height reduction of call i+1 (all 148 SMs, tensor-core bound) run while the bi-LSTM recurrence + head
+ * the encoder + height reduction of call i+1 (all SMs, tensor-core bound) run while the bi-LSTM recurrence + head
  * of call i (16-CTA clusters on 64 SMs, latency-bound: 512 dependent steps) are still in flight.  Ordering contract
  * on `stream`: x must be ready in stream order at the call; x may be reused by work enqueued on `stream` after the
  * call returns; bon/cor of call i are complete for work enqueued on `stream` after call i+1 returns, or after
@@ -100,12 +100,14 @@ int hn_dropout_mask(unsigned long long seed, int which, double p, float* out_dev
 int hn_model_get_tensor(hn_model* m, const char* key, float* out, long long numel, int on_device, void* stream);
 
 /* Training step (row f1; reference train.py:44-58 feed_forward + :272-281 backward).  hn_train_forward = the train-mode
- * forward above (same arguments) but on exact-fp32 kernels and with a tape: every conv output and activation is kept.
+ * forward above (same arguments) but with a tape: every conv output and activation is kept.
  * hn_train_backward takes d(loss)/d(bon) [batch][2][1024] and d(loss)/d(cor) [batch][1][1024] (device) -- the losses
  * themselves (train.py:53-56: L1 + BCE-with-logits) and the optimizer (train.py:216-223) stay with the caller -- and
  * leaves d(loss)/d(parameter) for every state_dict parameter in the reference's layout (nn.Conv2d OIHW, nn.LSTM
- * [4H][in], ...), read back with hn_model_get_grad (device pointer).  One backward per forward.  First correct path:
- * fp32 CUDA-core kernels; no tensor-core dgrad/wgrad, loss scaling or gradient all-reduce yet. */
+ * [4H][in], ...), read back with hn_model_get_grad (device pointer).  One backward per forward.  With option
+ * "tensor_cores" on, the encoder and height-reduction convolutions, their data gradients (hn_conv2d_dgrad_tc) and their
+ * weight gradients (hn_conv2d_wgrad_tc, see hn_wgrad_tc_enabled) run on the split-fp16 wgmma kernels where those take the
+ * shape, everything else on exact fp32 CUDA-core kernels; no loss scaling or gradient all-reduce. */
 int hn_train_forward(hn_model* m, const float* x_nchw_dev, int batch, int in_channels, float* bon_dev, float* cor_dev,
                      const unsigned char* bn_train, const double* bn_factor, int n_bn, unsigned long long seed,
                      double rnn_dropout, double head_dropout, const float* rnn_mask_dev, const float* head_mask_dev,
@@ -218,7 +220,9 @@ int hn_rotate_panorama(const void* img_dev, int in_is_f64, double* out_dev, int 
  * in:  [B][H][W + 2*in_halo][Cin]   out: [B][Ho][Wo + 2*out_halo][Cout]   (fp32, device)
  * w_packed: [kh*kw*Cin][Cout], k = (dy*kw + dx)*Cin + c;  scale/shift: [Cout];
  * ph = zero padding along H, pw = circular padding along W (<= in_halo).
- * impl: 0 = exact fp32 CUDA-core kernel, 1 = split-fp16 wgmma tensor-core kernel. */
+ * impl: 0 = exact fp32 CUDA-core kernel, 1 = split-fp16 wgmma tensor-core kernel (split-plane output, merged to fp32),
+ * 2 = the same kernel writing fp32 directly (the epilogue of the LSTM input projections, of the raw pass of a train-mode
+ * convolution and of the data gradient; no residual). */
 int hn_conv2d(const float* in_dev, int B, int H, int W, int Cin, int in_halo,
               const float* w_packed_dev, const float* scale_dev, const float* shift_dev,
               const float* residual_dev, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
@@ -238,6 +242,20 @@ int hn_conv2d_wgrad_tc(const float* in, int B, int H, int W, int Cin, const floa
  * CTAs.  -1 for a shape the kernel does not take. */
 int hn_wgrad_tc_plan(int B, int H, int W, int Cin, int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int sms, int plan[10]);
 int hn_wgrad_tc_enabled(void);   /* 1: the training step uses that kernel where it applies (env HN_WGRAD_TC=0/1 overrides the default) */
+/* The data gradient on the tensor cores exactly as the training step computes it (zero-dilated dz for a strided conv,
+ * power-of-two scaled planes of dz, flipped weights as planes, the transposed conv with fp32 output) and ADDED to din:
+ * dz [B][Ho][Wo+2][Cout] and din [B][H][W+2][Cin], halo-1 NHWC fp32 with circular halo columns; w_oihw: the forward
+ * weights [Cout][Cin][kh][kw].  Returns -1 for a shape the tensor-core kernel does not take. */
+int hn_conv2d_dgrad_tc(int B, int H, int W, int Cin, const float* w_oihw, const float* dz, int Cout, int kh, int kw, int sh,
+                       int sw, int ph, int pw, float* din, void* stream);
+/* Host-side launch plan of the tensor-core convolution (no GPU work; sms = SM count to plan for) for the conv hn_conv2d
+ * impl 1 (out_f32 = 0) or 2 (out_f32 = 1) would run, with or without a residual.  plan[18] = kernel (1 gemm_tc_kernel,
+ * 0 conv_tc_kernel), BN, mode (0 GEMM rows, 1 conv rows), M (rows), tile columns, rows per tile, tiles per output row,
+ * rowbox, box rows, box images, dx reuse, parity (stride 2 along W), K chunks, chunks per accumulation segment, L2 prefetch
+ * distance, tiles along Cout, tiles, CTAs.  Reads the same HN_TC_* switches as the launch.  -1 for a shape the kernel
+ * does not take. */
+int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
+                    int out_halo, int out_f32, int has_residual, int sms, int plan[18]);
 int hn_bn_forward_backward(const float* z, int B, int H, int W, int C, const float* gamma, const float* beta,
                            float* running_mean, float* running_var, double factor, int train, int relu, const float* res,
                            float* y, const float* dy, float* dz, float* dres, float* dgamma, float* dbeta, float* bn_scratch,

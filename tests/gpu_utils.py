@@ -1,6 +1,11 @@
 """Helpers for the -m gpu tests: torch is used only to build inputs in the library's halo-NHWC
 layout and to hold device memory; every computation under test goes through the C ABI."""
 import ctypes
+import hashlib
+import json
+import math
+import os
+
 import torch
 import torch.nn.functional as F
 
@@ -60,3 +65,154 @@ def conv2d_reference(x, w, scale, shift, stride, ph, pw, relu, residual=None):
     if relu:
         y = F.relu(y)
     return y
+
+
+def record(name, payload):
+    """Appends one JSON line of measured errors to $HN_TEST_RECORD_DIR/<name> when that variable names a directory (kept
+    outside the source tree, which may be read-only); without it nothing is written."""
+    d = os.environ.get('HN_TEST_RECORD_DIR')
+    if d and os.path.isdir(d):
+        with open(os.path.join(d, name), 'a') as f:
+            f.write(json.dumps(payload) + '\n')
+
+
+# ---- elementwise error bound of the split-fp16 tensor-core convolution (conv_tc.cuh plane format)
+# An operand v is carried as fp16 hi = fp16(v/16) and lo = fp16(v/16 - hi); the MMAs take hi*hi, hi*lo and lo*hi.
+#  * operands: a normal lo leaves |v| * 2^-22 of each operand, and the dropped lo*lo is |x||w| * 2^-22 at most: 3 * 2^-22 per
+#    product; fp32 accumulation in the tensor cores (256-deep segments) and in the register sum adds a few 2^-24 of the
+#    magnitude sum.  C_OPERAND = 8 covers both with margin:  C_OPERAND * 2^-21 * (|x| conv |w|);
+#  * activations below 2 in magnitude have a subnormal lo, i.e. an absolute resolution of 16 * 2^-25 = 2^-21 per element
+#    (2^-20 with margin):  2^-20 * (1 conv |w|);
+#  * both terms are in accumulator units and pass through the epilogue scale |scale|;
+#  * the output: fp32 rounding, or for plane outputs the re-split (2^-22 |y|, and 2^-21 absolute below 2): 2^-21 |y|
+#    (+ 2^-21 for planes); a plane residual adds its own representation error, 2^-21 (|r| + 1).
+C_OPERAND = 8.0
+EPS21, EPS20 = 2.0 ** -21, 2.0 ** -20
+
+
+def _conv_abs(x, w, stride, ph, pw):
+    if pw:
+        x = torch.cat([x[..., -pw:], x, x[..., :pw]], dim=3)
+    return F.conv2d(x, w, None, stride=stride, padding=(ph, 0))
+
+
+def tc_case_inputs(c, dev, seed=None):
+    g = torch.Generator().manual_seed(seed if seed is not None else
+                                      int(hashlib.sha1(c['name'].encode()).hexdigest()[:8], 16))
+    B, Ci, H, W, Co, k = c['B'], c['Cin'], c['H'], c['W'], c['Cout'], c['k']
+    x = torch.randn(B, Ci, H, W, generator=g)
+    w = torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5
+    scale = torch.rand(Co, generator=g) + 0.5
+    shift = torch.randn(Co, generator=g) * 0.1
+    Ho = (H + 2 * c['ph'] - k) // c['stride'][0] + 1
+    Wo = (W + 2 * c['pw'] - k) // c['stride'][1] + 1
+    res = torch.randn(B, Co, Ho, Wo, generator=g) if c['residual'] else None
+    return [t.to(dev) if t is not None else None for t in (x, w, scale, shift, res)]
+
+
+CANARY = 12345.5
+
+
+def run_tc_case(c, dev='cuda:0'):
+    """Runs one case of tests/tc_cases.py through hn_conv2d (impl 1, or 2 for fp32 output) and checks it against the fp64
+    reference elementwise.  Returns (worst err / bound, sha1 of the output bytes); raises AssertionError on a violation."""
+    lib = _lib.lib()
+    x, w, scale, shift, res = tc_case_inputs(c, dev)
+    B, Ci, H, W, Co, k = c['B'], c['Cin'], c['H'], c['W'], c['Cout'], c['k']
+    sh, sw = c['stride']
+    ph, pw, hi, ho = c['ph'], c['pw'], c['in_halo'], c['out_halo']
+    Ho, Wo = (H + 2 * ph - k) // sh + 1, (W + 2 * pw - k) // sw + 1
+    xin = to_halo_nhwc(x, hi)
+    wp = pack_weight(w)
+    n_out = B * Ho * (Wo + 2 * ho) * Co
+    buf = torch.full((n_out + 4096,), float('nan'), device=dev)
+    buf[n_out:] = CANARY
+    out = buf[:n_out].view(B, Ho, Wo + 2 * ho, Co)
+    resin = to_halo_nhwc(res, ho) if res is not None else None
+    impl = 2 if c['out_f32'] else 1
+    rc = lib.hn_conv2d(xin.data_ptr(), B, H, W, Ci, hi, wp.data_ptr(), scale.data_ptr(), shift.data_ptr(),
+                       resin.data_ptr() if resin is not None else None, Co, k, k, sh, sw, ph, pw, int(c['relu']),
+                       out.data_ptr(), ho, impl, torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(rc, 'hn_conv2d')
+    torch.cuda.synchronize(dev)
+    assert not torch.isnan(out).any(), f"{c['name']}: output elements left unwritten"
+    assert bool((buf[n_out:] == CANARY).all()), f"{c['name']}: write past the end of the output"
+    if ho:
+        assert torch.equal(out[:, :, 0], out[:, :, -2]) and torch.equal(out[:, :, -1], out[:, :, 1]), \
+            f"{c['name']}: halo columns are not the circular wrap"
+    y = from_halo_nhwc(out, ho).double()
+    xd, wd = x.double(), w.double()
+    ref = conv2d_reference(xd, wd, scale, shift, (sh, sw), ph, pw, c['relu'], res.double() if res is not None else None)
+    acc = _conv_abs(xd.abs(), wd.abs(), (sh, sw), ph, pw)
+    ones = _conv_abs(torch.ones_like(xd[:1]), wd.abs(), (sh, sw), ph, pw)
+    sc = scale.double().abs().view(1, -1, 1, 1)
+    bound = sc * (C_OPERAND * EPS21 * acc + EPS20 * ones) + EPS21 * ref.abs()
+    if not c['out_f32']:
+        bound = bound + EPS21
+    if res is not None:
+        bound = bound + EPS21 * (res.double().abs() + 1.0)
+    ratio = _worst_ratio(y - ref, bound)
+    digest = hashlib.sha1(out.cpu().numpy().tobytes()).hexdigest()
+    return ratio, digest
+
+
+def _worst_ratio(diff, bound):
+    """max |diff| / bound; an exact element counts 0 even where the bound is 0 (a pixel no output depends on)."""
+    err = diff.abs()
+    return torch.where(err == 0, torch.zeros_like(err), err / bound).max().item()
+
+
+def pow2_factor(absmax):
+    """conv_tc.cuh: the power of two that brings the largest magnitude of a gradient to [2^11, 2^12) before the split."""
+    if not absmax > 0 or math.isinf(absmax):
+        return 1.0
+    e = math.frexp(absmax)[1]
+    return 2.0 ** max(-100, min(100, 12 - e))
+
+
+def run_dgrad_case(B, Ci, H, W, Co, k, stride, dz_scale=1.0, prefill=False, zero=False, seed=0, dev='cuda:0'):
+    """hn_conv2d_dgrad_tc (the training step's tensor-core data gradient) against torch.autograd in fp64.  din starts as
+    the prefill (zeros or random, circular halo) and must come back as prefill + gradient within the bound of run_tc_case
+    applied to the power-of-two scaled planes of dz.  Returns worst err / bound."""
+    g = torch.Generator().manual_seed(seed)
+    p = k // 2
+    sh, sw = stride
+    Ho, Wo = (H + 2 * p - k) // sh + 1, (W + 2 * p - k) // sw + 1
+    w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(dev)
+    dz = (torch.randn(B, Co, Ho, Wo, generator=g) * dz_scale).to(dev)
+    if zero:
+        dz.zero_()
+    pre = (torch.randn(B, Ci, H, W, generator=g) if prefill else torch.zeros(B, Ci, H, W)).to(dev)
+    dzin = to_halo_nhwc(dz, 1)
+    n = B * H * (W + 2) * Ci
+    buf = torch.full((n + 4096,), CANARY, device=dev)
+    din = buf[:n].view(B, H, W + 2, Ci)
+    din.copy_(to_halo_nhwc(pre, 1))
+    rc = _lib.lib().hn_conv2d_dgrad_tc(B, H, W, Ci, w.data_ptr(), dzin.data_ptr(), Co, k, k, sh, sw, p, p, din.data_ptr(),
+                                       torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(rc, 'hn_conv2d_dgrad_tc')
+    torch.cuda.synchronize(dev)
+    assert torch.isfinite(din).all(), 'non-finite data gradient'
+    assert bool((buf[n:] == CANARY).all()), 'write past the end of din'
+    assert torch.equal(din[:, :, 0], din[:, :, -2]) and torch.equal(din[:, :, -1], din[:, :, 1]), 'halo is not the wrap'
+    got = from_halo_nhwc(din, 1).double()
+    if zero:
+        assert torch.equal(got, pre.double()), 'an all-zero dz must leave din exactly as it was'
+        return 0.0
+
+    def grad(wt, d):
+        xv = torch.zeros(B, Ci, H, W, dtype=torch.float64, device=dev, requires_grad=True)
+        _conv_abs(xv, wt, stride, p, p).backward(d)
+        return xv.grad
+
+    wd = w.double()
+    ref = grad(wd, dz.double())
+    acc = grad(wd.abs(), dz.double().abs())
+    ones = grad(wd.abs(), torch.ones_like(dz.double()))
+    f = pow2_factor(dz.abs().max().item())
+    bound = C_OPERAND * EPS21 * acc + EPS20 / f * ones + EPS21 * (ref.abs() + pre.double().abs())
+    return _worst_ratio(got - (pre.double() + ref), bound)
+
+
+def device_sms(dev=0):
+    return torch.cuda.get_device_properties(dev).multi_processor_count

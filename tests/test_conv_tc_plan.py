@@ -1,0 +1,123 @@
+"""Host plan of the tensor-core convolution (hn_conv_tc_plan = what conv_tc_planes launches), no GPU needed:
+* every conv_tc_planes launch of the model (tc_cases.model_launches: eval and train forwards, the training step's raw pass
+  and data gradients, the LSTM projections) has a plan whose tiles cover the output exactly once;
+* coverage guard: every variant key (tc_cases.variant_key) the model reaches on a 132-SM H100 SXM is reached by a case of
+  the -m gpu table (tc_cases.ALL_CASES).  A heuristic change that sends the model into a new variant fails here until a
+  unit case for it is added."""
+import pytest
+
+import __graft_entry__ as entry
+from horizonnet_b200 import _lib
+import tc_cases as T
+
+BM = 128
+
+
+@pytest.fixture(scope='module', autouse=True)
+def _built():
+    entry.build()
+
+
+def _check(c, p, sms):
+    name = c['name']
+    k, (sh, sw), B = c['k'], c['stride'], c['B']
+    Ho, Wo = (c['H'] + 2 * c['ph'] - k) // sh + 1, (c['W'] + 2 * c['pw'] - k) // sw + 1
+    assert p['n_tiles'] * p['BN'] == c['Cout'], name
+    assert p['num_kc'] == k * k * c['Cin'] // 64 and p['seg'] >= 1, name
+    if p['mode'] == 0:                            # GEMM rows: every halo-NHWC pixel once
+        assert k == 1 and (sh, sw) == (1, 1) and c['in_halo'] == c['out_halo'], name
+        assert p['M'] == B * c['H'] * (c['W'] + 2 * c['in_halo']), name
+        m_tiles = -(-p['M'] // BM)
+    else:                                         # conv rows: B*Ho rows x Wo columns once
+        assert p['M'] == B * Ho and p['tw'] * p['rows_per_tile'] == BM and p['wsegs'] * p['tw'] == Wo, name
+        m_tiles = -(-p['M'] // p['rows_per_tile']) * p['wsegs']
+        assert (m_tiles // p['wsegs'] - 1) * p['rows_per_tile'] < p['M'] <= m_tiles // p['wsegs'] * p['rows_per_tile'], name
+        assert p['parity'] == (sw == 2), name
+        if p['rowbox']:
+            assert p['box_rows'] * p['box_imgs'] == p['rows_per_tile'], name
+            assert (p['box_imgs'] == 1 and Ho % p['rows_per_tile'] == 0) or p['box_rows'] == Ho, name
+        else:
+            assert p['box_rows'] == p['box_imgs'] == 1, name
+        if p['dxr']:                              # the 130-pixel input row of the last tile stays inside Wp
+            Wp = c['W'] + 2 * c['in_halo']
+            assert p['rows_per_tile'] == 1 and k == 3 and sw == 1, name
+            assert p['wsegs'] * BM + (c['in_halo'] - c['pw']) + 2 <= Wp, name
+    assert p['num_tiles'] == m_tiles * p['n_tiles'], name
+    assert p['grid'] == min(p['num_tiles'], sms), name
+    if p['gemm_kernel']:
+        assert p['BN'] == 64 and not c['out_f32'] and c['Cin'] <= 256, name
+    if c['out_f32']:
+        assert not p['gemm_kernel'], name
+
+
+@pytest.mark.parametrize('sms', [132, 114])                 # H100 SXM, H100 PCIe
+@pytest.mark.parametrize('B', [1, 2, 3, 8, 32])
+def test_every_model_launch_has_a_plan_covering_its_output_once(B, sms):
+    launches = T.model_launches(B)
+    assert len(launches) == 4 * 68 + 2
+    for c in launches:
+        p = T.plan(c, sms)
+        if c['Cin'] % 64:
+            assert p is None, c['name']           # ghc0.3's data gradient (32 channels in) stays on conv_dgrad_f32
+            continue
+        assert p is not None, (c['name'], _lib.lib().hn_last_error())
+        _check(c, p, sms)
+
+
+def test_unit_cases_have_consistent_plans():
+    for c in T.ALL_CASES:
+        p = T.plan(c)
+        assert p is not None, (c['name'], _lib.lib().hn_last_error())
+        _check(c, p, T.SMS)
+
+
+def test_unit_cases_reach_every_variant_key_of_the_model():
+    model = {}
+    for B in (1, 2, 3, 8, 32):
+        for c in T.model_launches(B):
+            p = T.plan(c)
+            if p is not None:
+                model.setdefault(T.variant_key(c, p), f"{c['name']} @ B={B}")
+    cases = {T.variant_key(c, T.plan(c)) for c in T.ALL_CASES}
+    missing = {k: v for k, v in model.items() if k not in cases}
+    assert not missing, '\n'.join(f'{dict(zip(T.KEY_FIELDS, k))}  (e.g. {v})' for k, v in missing.items())
+    print(f'{len(model)} variant keys of the model, all reached by the {len(T.ALL_CASES)} unit cases')
+
+
+def test_unit_cases_include_the_named_variants():
+    plans = {c['name']: (c, T.plan(c)) for c in T.ALL_CASES}
+
+    def has(pred):
+        return any(pred(c, p) for c, p in plans.values())
+    tiles_per_cta = lambda p: p['num_tiles'] / p['grid']
+    ragged = lambda p: p['mode'] == 0 and p['M'] % BM != 0
+    assert has(lambda c, p: p['BN'] == 128 and tiles_per_cta(p) >= 3)
+    for res in (False, True):                     # K = 64 with a live L2 prefetch, 3+ tiles per CTA, ragged last M tile
+        assert has(lambda c, p: p['gemm_kernel'] and p['num_kc'] == 1 and p['pf'] and c['residual'] == res and
+                   tiles_per_cta(p) >= 3 and ragged(p))
+    assert has(lambda c, p: p['gemm_kernel'] and p['num_kc'] == 4 and tiles_per_cta(p) >= 3 and ragged(p))
+    assert has(lambda c, p: p['gemm_kernel'] and c['Cout'] == 1024 and tiles_per_cta(p) >= 3 and ragged(p))
+    for kc in (8, 16, 32):                        # conv_tc_kernel mode 0 at K = 512, 1024, 2048
+        assert has(lambda c, p: not p['gemm_kernel'] and p['mode'] == 0 and p['num_kc'] == kc)
+    for bn in (64, 128):
+        for ws in (1, 2):
+            assert has(lambda c, p: p['dxr'] and p['BN'] == bn and p['wsegs'] == ws)
+    assert has(lambda c, p: p['BN'] == 32 and c['stride'] == (2, 1) and c['W'] == 256)
+    assert has(lambda c, p: p['parity'] and p['rowbox'] and c['stride'][0] == 2)
+    assert has(lambda c, p: p['parity'] and not p['rowbox'])
+    assert has(lambda c, p: p['box_imgs'] > 1 and c['B'] in (3, 5) and p['M'] % p['rows_per_tile'] != 0)
+    assert has(lambda c, p: p['num_kc'] * 64 == 18432)
+    for B in (2, 9):                              # LSTM projection shape, fp32 output
+        assert has(lambda c, p: c['out_f32'] and c['in_halo'] == 0 and c['W'] == 256 * B and c['Cin'] == 1024 and
+                   c['Cout'] == 4096)
+
+
+def test_plan_rejects_what_the_kernel_does_not_take():
+    bad = [T.launch('cin48', 2, 16, 32, 48, 64, 3, (1, 1)),                       # Cin % 64
+           T.launch('cout96', 2, 16, 32, 64, 96, 3, (1, 1)),                      # Cout > 64, not a multiple of 128
+           T.launch('w24', 2, 16, 24, 64, 64, 3, (1, 1)),                         # W = 24: not a power-of-two tile width
+           T.launch('f32res', 2, 16, 32, 64, 64, 1, (1, 1), out_f32=True, residual=True)]
+    for c in bad:
+        assert T.plan(c) is None, c['name']
+    assert b'residual' in _lib.lib().hn_last_error()
+    assert T.plan(T.launch('ok', 2, 16, 32, 64, 64, 3, (1, 1))) is not None

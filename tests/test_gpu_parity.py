@@ -81,33 +81,14 @@ def test_conv_kernel_vs_torch(case, impl):
 
 
 # ------------------------------------------------------------------------------- LSTM kernel
-@pytest.mark.parametrize('T,B', [(5, 1), (24, 7), (16, 32), (12, 40)])
+@pytest.mark.parametrize('T,B', [(5, 1), (24, 7), (16, 32), (12, 40), (256, 1), (256, 32)])
 def test_lstm_layer_vs_oracle(T, B):
-    g = torch.Generator().manual_seed(T * 100 + B)
-    xproj = torch.randn(T, B, 4096, generator=g) * 0.5
-    whh = [torch.rand(2048, 512, generator=g) * 0.08 - 0.04 for _ in range(2)]
-    zero = torch.zeros(2048)
-    ref = []
-    for d in range(2):
-        # oracle recurrence with the projection already applied: feed identity input weights
-        xp = xproj[:, :, d * 2048:(d + 1) * 2048]
-        h = torch.zeros(B, 512); c = torch.zeros(B, 512)
-        out = torch.empty(T, B, 512)
-        for t in (range(T - 1, -1, -1) if d else range(T)):
-            gates = xp[t] + h @ whh[d].t()
-            i, f, gg, o = gates.chunk(4, dim=1)
-            c = torch.sigmoid(f) * c + torch.sigmoid(i) * torch.tanh(gg)
-            h = torch.sigmoid(o) * torch.tanh(c)
-            out[t] = h
-        ref.append(out)
-    ref = torch.cat(ref, dim=2)
-    out = torch.full((T, B, 1024), float('nan'), device=DEV)
-    xd, w0, w1 = xproj.to(DEV), whh[0].to(DEV), whh[1].to(DEV)
-    rc = _lib.lib().hn_lstm_layer(xd.data_ptr(), w0.data_ptr(), w1.data_ptr(), out.data_ptr(), T, B,
-                                  torch.cuda.current_stream().cuda_stream)
-    _lib.check(rc, 'hn_lstm_layer')
-    torch.cuda.synchronize()
-    assert (out.cpu() - ref).abs().max().item() < 2e-6
+    """One bidirectional layer against an fp64 recurrence of the same input projection, up to the model's T = 256;
+    B = 40 takes two batch-chunk launches.  tc_runner.lstm_error also runs the cooperative kernel (test_tc_kernels.py)."""
+    from tc_runner import lstm_error
+    err = lstm_error(T, B, DEV)
+    gu.record('lstm_errors.jsonl', {'T': T, 'B': B, 'err': err})
+    assert err < 2e-6, err
 
 
 def test_lstm_layer_matches_oracle_function():
@@ -679,15 +660,6 @@ WGRAD_TC_CASES = [
 ]
 
 
-def _record(name, payload):
-    """Measured errors of the new kernels, kept next to the gpurun logs when that directory exists."""
-    import json
-    d = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'gpurun_out')
-    if os.path.isdir(d):
-        with open(os.path.join(d, name), 'a') as f:
-            f.write(json.dumps(payload) + '\n')
-
-
 @pytest.mark.parametrize('case', WGRAD_TC_CASES)
 def test_conv_wgrad_tc_vs_autograd(case):
     """Weight gradient on the tensor-core kernel (wgrad_tc.cu: pixel-axis GEMM over MN-major plane tiles) against
@@ -718,7 +690,7 @@ def test_conv_wgrad_tc_vs_autograd(case):
     scale = ref.abs().max().item()
     err = (dw.cpu().double() - ref).abs().max().item() / scale
     err32 = (dw32.cpu().double() - ref).abs().max().item() / scale
-    _record('wgrad_tc_errors.jsonl', {'case': list(case[:6]) + list(stride), 'err_tc': err, 'err_fp32': err32})
+    gu.record('wgrad_tc_errors.jsonl', {'case': list(case[:6]) + list(stride), 'err_tc': err, 'err_fp32': err32})
     assert err <= 2e-5, (err, err32)
 
 
@@ -731,7 +703,7 @@ def test_conv_wgrad_tc_rejects_shapes_it_does_not_take():
     assert b'not supported' in _lib.lib().hn_last_error()
 
 
-def test_training_step_weight_gradients_tcgen05_vs_fp32_kernels(monkeypatch):
+def test_training_step_weight_gradients_wgmma_vs_fp32_kernels(monkeypatch):
     """The whole backward of one batch-2 step with the weight gradients on the tensor-core kernel (HN_WGRAD_TC=1) against the
     same step with the fp32 CUDA-core weight-gradient kernel (=0): same tape, same dz, so every parameter gradient
     agrees to rounding."""
@@ -752,7 +724,7 @@ def test_training_step_weight_gradients_tcgen05_vs_fp32_kernels(monkeypatch):
     gmax = max(float(v.abs().max()) for v in grads['0'].values())
     worst = sorted(((float((grads['1'][k] - v).abs().max()) / (float(v.abs().max()) + 1e-4 * gmax), k)
                     for k, v in grads['0'].items()), reverse=True)
-    _record('wgrad_tc_errors.jsonl', {'whole_step_worst': worst[:5]})
+    gu.record('wgrad_tc_errors.jsonl', {'whole_step_worst': worst[:5]})
     assert worst[0][0] < 1e-4, worst[:8]
 
 

@@ -1,0 +1,135 @@
+"""-m gpu: every launch variant of the tensor-core convolution kernels (conv_tc.cu) against fp64, elementwise.
+
+* forward cases of tests/tc_cases.py through hn_conv2d impl 1 (split-plane output) and impl 2 (fp32 output: the epilogue of
+  the LSTM projections, of the training step's raw pass and of its data gradients), with the error bound of
+  gpu_utils.run_tc_case: NaN-filled output that must be written everywhere, circular halo columns, a canary behind the
+  output;
+* the tensor-core data gradient of the training step (hn_conv2d_dgrad_tc) against torch.autograd in fp64;
+* the HN_TC_* switches that select other code paths, and the cooperative LSTM kernel (HN_LSTM_CLUSTER=0), each in a fresh
+  process (tests/tc_runner.py), since the library reads them once per process.
+Worst err / bound per case and variant key go to $HN_TEST_RECORD_DIR/tc_errors.jsonl when that variable is set
+(gpu_utils.record)."""
+import json
+import os
+import subprocess
+import sys
+
+import pytest
+import torch
+
+import __graft_entry__ as entry
+from horizonnet_b200 import _lib
+import gpu_utils as gu
+import tc_cases
+
+pytestmark = pytest.mark.gpu
+HERE = os.path.dirname(os.path.abspath(__file__))
+
+
+@pytest.fixture(scope='module', autouse=True)
+def _built():
+    entry.build()
+    _lib.lib()
+
+
+def _key(c):
+    return dict(zip(tc_cases.KEY_FIELDS, tc_cases.variant_key(c, tc_cases.plan(c, gu.device_sms()))))
+
+
+@pytest.mark.parametrize('c', tc_cases.ALL_CASES, ids=lambda c: c['name'])
+def test_conv_tc_variant_vs_fp64(c):
+    ratio, _ = gu.run_tc_case(c)
+    gu.record('tc_errors.jsonl', {'test': 'conv', 'case': c['name'], 'ratio': ratio, 'key': _key(c)})
+    assert ratio <= 1.0, ratio
+
+
+def test_fp32_output_rejects_a_residual():
+    x = torch.zeros(1, 1, 8, 66 * 64, device='cuda:0')
+    w = torch.zeros(64 * 64, device='cuda:0')
+    v = torch.ones(64, device='cuda:0')
+    out = torch.zeros(1, 8, 66, 64, device='cuda:0')
+    rc = _lib.lib().hn_conv2d(x.data_ptr(), 1, 8, 64, 64, 1, w.data_ptr(), v.data_ptr(), v.data_ptr(), out.data_ptr(), 64,
+                              1, 1, 1, 1, 0, 0, 0, out.data_ptr(), 1, 2, None)
+    assert rc != 0 and b'residual' in _lib.lib().hn_last_error()
+
+
+# B, Cin, H, W, Cout, k, stride: data gradients of the model's unit kinds
+DGRAD_CASES = [
+    (2, 64, 32, 128, 64, 3, (1, 1)),          # 3x3 stride 1 (layer1 conv2): dx reuse
+    (2, 128, 32, 64, 128, 3, (2, 2)),         # 3x3 stride 2 (layer2-4 .0.conv2): dilated dz
+    (2, 256, 32, 64, 512, 1, (2, 2)),         # 1x1 stride 2 (downsample)
+    (3, 256, 16, 64, 128, 3, (2, 1)),         # 3x3 stride (2, 1) (height reduction)
+    (2, 512, 16, 32, 128, 1, (1, 1)),         # 1x1 stride 1, Cin > 256 (conv1 of layer3)
+]
+
+
+@pytest.mark.parametrize('dz_scale', [1.0, 1e-6, 1e-12])
+@pytest.mark.parametrize('case', DGRAD_CASES, ids=str)
+def test_dgrad_tc_vs_autograd(case, dz_scale):
+    B, Ci, H, W, Co, k, st = case
+    ratio = gu.run_dgrad_case(B, Ci, H, W, Co, k, st, dz_scale=dz_scale, seed=hash(case) % 1000)
+    gu.record('tc_errors.jsonl', {'test': 'dgrad', 'case': list(case[:6]) + list(st), 'dz_scale': dz_scale, 'ratio': ratio})
+    assert ratio <= 1.0, ratio
+
+
+@pytest.mark.parametrize('case', DGRAD_CASES[:4], ids=str)
+def test_dgrad_tc_accumulates_into_din(case):
+    B, Ci, H, W, Co, k, st = case
+    ratio = gu.run_dgrad_case(B, Ci, H, W, Co, k, st, prefill=True, seed=7)
+    gu.record('tc_errors.jsonl', {'test': 'dgrad_prefill', 'case': list(case[:6]) + list(st), 'ratio': ratio})
+    assert ratio <= 1.0, ratio
+    assert gu.run_dgrad_case(B, Ci, H, W, Co, k, st, prefill=True, zero=True, seed=8) == 0.0
+
+
+def test_dgrad_tc_rejects_shapes_the_kernel_does_not_take():
+    z = torch.zeros(1 << 16, device='cuda:0')
+    # ghc0.3 (64 -> 32): the transposed conv has 32 input channels
+    assert _lib.lib().hn_conv2d_dgrad_tc(1, 4, 16, 64, z.data_ptr(), z.data_ptr(), 32, 3, 3, 2, 1, 1, 1, z.data_ptr(),
+                                         None) != 0
+    assert b'not supported' in _lib.lib().hn_last_error()
+
+
+def _run(kind, names, env):
+    e = dict(os.environ)
+    e.update(env)
+    p = subprocess.run([sys.executable, os.path.join(HERE, 'tc_runner.py'), kind] + list(names), env=e,
+                       capture_output=True, text=True, timeout=900)
+    assert p.returncode == 0, (env, p.stdout[-2000:], p.stderr[-4000:])
+    return {r['name']: r for r in (json.loads(l) for l in p.stdout.splitlines() if l.startswith('{'))}
+
+
+# switch -> (cases whose plan it changes, plan field it turns off or None, bitwise equal to the default run)
+SWITCHES = {
+    'HN_TC_DXR': (['dxr_bn64_w2', 'dxr_bn128_w1', 'f32_3x3'], 'dxr', False),
+    'HN_TC_ROWBOX': (['rowbox_s1', 'images_s1', 'h2_images', 's2_parity_images', 'f32_3x3_rowbox'], 'rowbox', True),
+    'HN_TC_ROWBOX2': (['s2_parity_rowbox2', 'h2_rowbox2', 'h2_images_bn128'], 'rowbox', False),
+    'HN_TC_GEMM': (['gemm_k64_res_pf', 'gemm_k256', 'gemm_cout1024'], 'gemm_kernel', False),
+    'HN_TC_PF': (['gemm_k64_res_pf', 'gemm_k64_pf'], 'pf', True),
+    'HN_TC_SEG': (['h2_k18432', 'gemm_k64_res_pf', 'dxr_bn128_w2', 'xproj_b2'], None, False),
+}
+
+
+def test_switched_off_paths_stay_inside_the_bound():
+    names = sorted({n for v in SWITCHES.values() for n in v[0]})
+    base = _run('conv', names, {})
+    for sw, (cases, field, bitwise) in SWITCHES.items():
+        got = _run('conv', cases, {sw: '1' if sw == 'HN_TC_SEG' else '0'})
+        for n in cases:
+            r = got[n]
+            gu.record('tc_errors.jsonl', {'test': 'switch', 'switch': sw, 'case': n, 'ratio': r['ratio']})
+            assert r['ratio'] <= 1.0, (sw, n, r['ratio'])
+            if field:
+                assert base[n]['plan'][field] and not r['plan'][field], (sw, n)       # the switch took the other path
+            else:
+                assert r['plan']['seg'] == 1
+            if bitwise:
+                assert r['digest'] == base[n]['digest'], (sw, n)                     # data movement only
+
+
+def test_cooperative_lstm_kernel_vs_fp64():
+    """HN_LSTM_CLUSTER=0: the cooperative L2-exchange kernel, also the fallback when two 16-CTA clusters cannot be
+    co-scheduled; the model's T = 256, and B = 40 for two batch-chunk launches."""
+    got = _run('lstm', ['256,1', '256,32', '12,40', '256,40'], {'HN_LSTM_CLUSTER': '0'})
+    for n, r in got.items():
+        gu.record('tc_errors.jsonl', {'test': 'lstm_coop', 'case': n, 'err': r['err']})
+    assert len(got) == 4 and all(r['err'] < 2e-6 for r in got.values()), got

@@ -13,6 +13,7 @@ import torch
 
 import __graft_entry__ as entry
 from horizonnet_b200 import _lib
+from tc_cases import resnet50_rnn_convs
 
 KT = 64
 
@@ -29,32 +30,6 @@ def plan(B, H, W, Ci, Co, k, stride, sms=132):
     if rc != 0:
         return None
     return dict(zip(('tw', 'rpt', 'wsegs', 'box_rows', 'imgs', 'num_kt', 'kt_per_slice', 'slices', 'items', 'ctas'), out))
-
-
-def resnet50_rnn_convs():
-    """(name, H, W, Cin, Cout, k, stride) of every conv unit behind the stem, input geometry at 512 x 1024."""
-    out = []
-    planes, nblk = (64, 128, 256, 512), (3, 4, 6, 3)
-    H, W, inpl = 128, 256, 64
-    for l in range(4):
-        p = planes[l]
-        for b in range(nblk[l]):
-            s = 2 if (b == 0 and l > 0) else 1
-            n = f'layer{l + 1}.{b}'
-            out.append((n + '.conv1', H, W, inpl, p, 1, (1, 1)))
-            if b == 0:
-                out.append((n + '.downsample', H, W, inpl, 4 * p, 1, (s, s)))
-            out.append((n + '.conv2', H, W, p, p, 3, (s, s)))
-            out.append((n + '.conv3', H // s, W // s, p, 4 * p, 1, (1, 1)))
-            inpl, H, W = 4 * p, H // s, W // s
-    for s in range(4):
-        c = planes[s] * 4
-        ch = (c, c // 2, c // 2, c // 4, c // 8)
-        h, w = 128 >> s, 256 >> s
-        for j in range(4):
-            out.append((f'ghc{s}.{j}', h, w, ch[j], ch[j + 1], 3, (2, 1)))
-            h //= 2
-    return out
 
 
 @pytest.mark.parametrize('B', [1, 2, 3, 8])
