@@ -81,8 +81,13 @@ struct Smem {
     static constexpr int B_PLANE = BN * BKC * 2;
     static constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
     static constexpr int BAR_OFF = NST * STAGE;
-    static constexpr int TOTAL = BAR_OFF + 256 + 1024;    // barriers + alignment slack
+    static constexpr int CST_OFF = BAR_OFF + 256;         // epilogue constants scale[Cout], shift[Cout]
+    static constexpr int TOTAL = CST_OFF + 1024;          // + alignment slack; the launch adds 8 * Cout bytes of constants
 };
+constexpr int MAX_SMEM = 227 * 1024;
+// dynamic shared memory of conv_tc_kernel<BN> for Cout output channels
+template <int BN>
+constexpr int conv_smem_bytes(int cout) { return Smem<BN>::TOTAL + 8 * cout; }
 
 // 12 wgmma of one 64-channel K chunk as one wgmma group: hi*hi (overwrites the accumulator when `fresh`), hi*lo, lo*hi
 template <int R>
@@ -107,6 +112,24 @@ __device__ __forceinline__ void chunk_mma(float (&acc)[R], uint32_t a_hi, uint32
     chunk_issue(acc, a_hi, a_lo, b_hi, b_lo, fresh);
     wgmma_wait0();
     reg_fence(acc);
+}
+
+// output pixel (halo-NHWC index into the output planes) of tile row r of M tile mt, and whether it exists
+__device__ __forceinline__ size_t tile_pixel(const TcArgs& a, int mt, int r, bool& valid) {
+    if (a.mode == 0) {
+        const long long m = (long long)mt * BM + r;
+        valid = m < a.M;
+        return (size_t)m;
+    }
+    const int rg = mt / a.wsegs;
+    const int wo = (mt - rg * a.wsegs) * a.tw + (r % a.tw);
+    const int R = rg * a.rows_per_tile + r / a.tw;
+    valid = R < a.M;
+    return (size_t)R * a.Wop + wo + a.out_halo;
+}
+
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
 }
 
 template <int BN>
@@ -141,8 +164,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int i = 0; i < 2; ++i) { mbar_init(afull_bar + i, 1); mbar_init(aempty_bar + i, CONS_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    __syncthreads();
     pdl_wait();                                              // everything below reads / writes activations
+    // the epilogue constants, read from shared memory: global loads of them would sit in the epilogue's chain of output
+    // stores (the pointers may alias) and each wait out its latency.  Loaded after pdl_wait: in the training step the
+    // kernel before this one may have written them.
+    float* cst = reinterpret_cast<float*>(smem + S::CST_OFF);
+    for (int i = threadIdx.x; i < 2 * a.Cout; i += NTHREADS) cst[i] = (i < a.Cout) ? a.scale[i] : a.shift[i - a.Cout];
+    __syncthreads();
 
     if (warp == 0) {
         // =============================== TMA producer ===============================
@@ -238,6 +266,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         uint32_t phase = 0, aph = 0;
         for (int tile = tile0; tile < a.num_tiles; tile += tstride) {
             const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
+            if (a.res && !(a.dbg & 1)) {
+                // The epilogue reads the residual inside its chain of output stores (the pointers may alias, so the
+                // compiler keeps the order), where every load waits out its full latency.  Pull the tile's residual
+                // rows into L2 now, while its MMAs run: lane l of a warp takes row l % 16 of the warp's 16 rows in
+                // plane l / 16, BN * 2 bytes = BN / 64 lines of 128 B (one for BN < 64).
+                bool ok;
+                const size_t px = tile_pixel(a, mt, wg * 64 + (warp & 3) * 16 + (lane & 15), ok);
+                if (ok) {
+                    const unsigned short* row = a.res + (lane >> 4) * a.out_plane + px * (size_t)a.Cout + nt * BN;
+#pragma unroll
+                    for (int l = 0; l < (BN + 63) / 64; ++l) prefetch_l2(row + l * 64);
+                }
+            }
 #pragma unroll
             for (int j = 0; j < BN / 2; ++j) sum[j] = 0.f;
             int seg_pos = 0, held = -1;      // held: ring stage whose wgmma group may still be in flight
@@ -298,16 +339,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
                 has_halo[h] = false;
                 halo_pix[h] = 0;
-                if (a.mode == 0) {
-                    const long long m = (long long)mt * BM + r;
-                    valid[h] = m < a.M;
-                    pix[h] = (size_t)m;
-                } else {
+                pix[h] = tile_pixel(a, mt, r, valid[h]);
+                if (a.mode == 1) {
                     const int rg = mt / a.wsegs;
                     const int wo = (mt - rg * a.wsegs) * a.tw + (r % a.tw);
                     const int R = rg * a.rows_per_tile + r / a.tw;
-                    valid[h] = R < a.M;
-                    pix[h] = (size_t)R * a.Wop + wo + a.out_halo;
                     if (a.out_halo) {
                         if (wo == 0) { has_halo[h] = true; halo_pix[h] = (size_t)R * a.Wop + a.Wo + 1; }
                         else if (wo == a.Wo - 1) { has_halo[h] = true; halo_pix[h] = (size_t)R * a.Wop; }
@@ -317,8 +353,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
                 const int n = nt * BN + 8 * j + 2 * (lane & 3);          // output channel of the pair
-                const float2 sc = __ldg(reinterpret_cast<const float2*>(a.scale + n));
-                const float2 sf = __ldg(reinterpret_cast<const float2*>(a.shift + n));
+                const float2 sc = *reinterpret_cast<const float2*>(cst + n);
+                const float2 sf = *reinterpret_cast<const float2*>(cst + a.Cout + n);
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     if (!valid[h]) continue;
@@ -1079,9 +1115,10 @@ bool tc_prefetch_on() {
 
 template <int BN>
 int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcArgs& a, int grid, cudaStream_t st) {
-    using S = Smem<BN>;
-    HN_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    HN_CUDA_OK(launch_tc(conv_tc_kernel<BN>, grid, S::TOTAL, st, tmA, tmB, a));
+    const int bytes = conv_smem_bytes<BN>(a.Cout);
+    HN_CHECK(bytes <= MAX_SMEM, "conv_tc: too many output channels for the epilogue constants in shared memory");
+    HN_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    HN_CUDA_OK(launch_tc(conv_tc_kernel<BN>, grid, bytes, st, tmA, tmB, a));
     HN_LAUNCH_OK();
     return 0;
 }
