@@ -17,17 +17,23 @@
 //              stride 2 along H for the stride-(2,1) convs, whole images when an image has fewer rows than a tile);
 //              the 3x3 taps are shifted box coordinates, zero H padding is TMA out-of-bounds fill, circular W padding
 //              is the halo column, stride-2 in W reads a parity view -- and B (hi, lo: BN x 64 weights, K-major);
-//              3-stage mbarrier ring of 64 KB stages (4 stages of 48 KB for BN <= 64).
+//              3-stage mbarrier ring of 64 KB stages (4 stages of 48 KB for BN <= 64).  After a tile's last K chunk it
+//              claims the next stage as the tile's epilogue slot (one stage holds exactly one output tile, BM x BN x 4 B)
+//              and TMA-loads the residual tile into it, so the residual lands while the last chunks compute.
 //              "dxr" mode (3x3, one 128-pixel row per tile): one 130-pixel box per (dy, chunk) feeds all three dx taps
 //              through wgmma descriptors whose start address is shifted by dx rows (the swizzle is a function of the
-//              absolute shared-memory address), so each input row crosses L2 -> SM once instead of three times.
+//              absolute shared-memory address), so each input row crosses L2 -> SM once instead of three times.  The
+//              ring then holds two input-row slots and NST weight slots; a weight slot holds exactly half an output tile,
+//              so the epilogue slot is the next two weight slots (hi plane in the first, lo plane in the second).
 //   warps 4-7, 8-11   two consumer warpgroups; warpgroup g owns tile rows [64g, 64g + 64) x all BN columns: per chunk
 //              12 wgmma m64nBNk16 (3 products x 4 K-steps of 16, one wgmma group; the group of the previous chunk stays in
 //              flight until this one is issued) into a register accumulator that is restarted every
 //              `seg` chunks and added into a second register sum with round-to-nearest fp32 adds (bounds whatever
-//              rounding the tensor-core accumulation applies over K up to 18432); then the epilogue straight from
-//              the accumulator fragments: folded BN scale/shift, residual add, ReLU, re-split into hi/lo planes (or
-//              fp32) incl. the circular halo columns.  The producer keeps filling the ring during the epilogue.
+//              rounding the tensor-core accumulation applies over K up to 18432); then the epilogue in the slot:
+//              folded BN scale/shift, + the residual the slot holds, ReLU, re-split into hi/lo planes (or fp32) written
+//              in place, the circular halo columns stored directly.  The consumers go straight on to the next tile.
+//   warp 3     store warp: TMA-stores each finished output tile from its slot and hands the stage back to the producer
+//              once the TMA engine has read it.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cstdlib>
@@ -114,29 +120,177 @@ __device__ __forceinline__ void chunk_mma(float (&acc)[R], uint32_t a_hi, uint32
     reg_fence(acc);
 }
 
-// output pixel (halo-NHWC index into the output planes) of tile row r of M tile mt, and whether it exists
-__device__ __forceinline__ size_t tile_pixel(const TcArgs& a, int mt, int r, bool& valid) {
-    if (a.mode == 0) {
-        const long long m = (long long)mt * BM + r;
-        valid = m < a.M;
-        return (size_t)m;
-    }
-    const int rg = mt / a.wsegs;
-    const int wo = (mt - rg * a.wsegs) * a.tw + (r % a.tw);
-    const int R = rg * a.rows_per_tile + r / a.tw;
-    valid = R < a.M;
-    return (size_t)R * a.Wop + wo + a.out_halo;
+// tile row of accumulator element pair h (0: d[4j], d[4j+1]; 1: d[4j+2], d[4j+3]) of this thread's wgmma fragment
+__device__ __forceinline__ int frag_row(int wg, int warp, int lane, int h) {
+    return wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+}
+// byte offset of the column pair (c, c + 1), c even, of tile row r in a [rows][64 fp16] buffer with 128-byte swizzle
+__device__ __forceinline__ uint32_t swz_pair_off(int r, int c) {
+    return (uint32_t)(r * 128 + ((((c >> 3) ^ (r & 7)) << 4)) + (c & 7) * 2);
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_f2(uint32_t addr, float a, float b) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+// named barrier of one consumer warpgroup (ids 1, 2; id 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
+
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, const void* src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                     reinterpret_cast<uint64_t>(tm)),
+                 "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* tm, const void* src, int c0, int c1, int c2, int c3, int c4) {
+    asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(
+                     reinterpret_cast<uint64_t>(tm)),
+                 "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+                 : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_cnt(uint64_t* bar, uint32_t count) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 
-__device__ __forceinline__ void prefetch_l2(const void* p) {
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+// circular halo columns of output rows (hn_common.cuh): wp = Wo + 1 copies wo = 0, wp = 0 copies wo = Wo - 1.
+// Halo pixel that tile row r is copied to, or -1: rowbase = pixel index of wp = 0 of the tile's first output row, Wop
+// pixels per output row, tw tile columns per output row starting at column wo0, `rows` output rows of the tile that exist
+__device__ __forceinline__ long long halo_pixel(int r, long long rowbase, int Wop, int tw, int rows, int wo0, int Wo) {
+    const unsigned rr = (unsigned)r / (unsigned)tw;
+    const int wo = wo0 + (r - (int)rr * tw);
+    if ((int)rr >= rows) return -1;
+    const long long base = rowbase + (long long)rr * Wop;
+    return wo == 0 ? base + Wo + 1 : (wo == Wo - 1 ? base : -1);
+}
+struct HaloStore {
+    void* out;                // output planes (hi; lo at + out_plane) or fp32 output
+    size_t out_plane;
+    int C, n0;                // channels, first channel of the buffer
+    long long pix[2];         // halo_pixel of this thread's fragment rows (frag_row h = 0, 1)
+};
+
+// In-place epilogue of a C-channel output tile held as fragments `acc` (rows of this warpgroup): y = acc*sc + sf
+// (+ the residual the buffer holds) (ReLU), re-split into the hi / lo planes e_hi / e_lo of the buffer: [128][64] fp16
+// with 128-byte swizzle for C = 64, unswizzled [128][32] fp16 for C = 32.  conv_tc_kernel, gemm_tc_kernel and the conv3
+// stage of bott_tc_kernel share it, so their results agree bit for bit.
+template <int C>
+__device__ __forceinline__ void epi_inplace(const float (&acc)[C / 2], const float* sc, const float* sf, uint32_t e_hi,
+                                            uint32_t e_lo, bool has_res, bool relu, int wg, int warp, int lane,
+                                            const HaloStore* halo = nullptr) {
+    static_assert(C == 64 || C == 32, "epi_inplace: 64 or 32 channels");
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int r = frag_row(wg, warp, lane, h);
+        const long long hp = halo ? halo->pix[h] : -1;
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j) {
+            const int c = 8 * j + 2 * (lane & 3);
+            const float2 k = *reinterpret_cast<const float2*>(sc + c);
+            const float2 f = *reinterpret_cast<const float2*>(sf + c);
+            float y0 = fmaf(acc[4 * j + 2 * h], k.x, f.x);
+            float y1 = fmaf(acc[4 * j + 2 * h + 1], k.y, f.y);
+            const uint32_t off = C == 64 ? swz_pair_off(r, c) : (uint32_t)(r * 64 + c * 2);
+            if (has_res) {                                    // y is in plane units here: no rescaling needed
+                const float2 fh = unpack_half2(ld_shared_u32(e_hi + off)), fl = unpack_half2(ld_shared_u32(e_lo + off));
+                y0 += fh.x + fl.x;
+                y1 += fh.y + fl.y;
+            }
+            if (relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+            uint32_t ph, pl;
+            split2_scaled(y0, y1, ph, pl);
+            st_shared_u32(e_hi + off, ph);
+            st_shared_u32(e_lo + off, pl);
+            if (hp >= 0) {
+                unsigned short* o = static_cast<unsigned short*>(halo->out) + (size_t)hp * halo->C + halo->n0 + c;
+                *reinterpret_cast<uint32_t*>(o) = ph;
+                *reinterpret_cast<uint32_t*>(o + halo->out_plane) = pl;
+            }
+        }
+    }
+}
+// the same for fp32 output (no residual): 32 channels into a [128][32] fp32 buffer with 128-byte swizzle
+__device__ __forceinline__ void epi_f32(const float (&acc)[16], const float* sc, const float* sf, uint32_t e, bool relu,
+                                        int wg, int warp, int lane, const HaloStore* halo) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int r = frag_row(wg, warp, lane, h);
+        const long long hp = halo->pix[h];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int c = 8 * j + 2 * (lane & 3);
+            const float2 k = *reinterpret_cast<const float2*>(sc + c);
+            const float2 f = *reinterpret_cast<const float2*>(sf + c);
+            float y0 = fmaf(acc[4 * j + 2 * h], k.x, f.x);
+            float y1 = fmaf(acc[4 * j + 2 * h + 1], k.y, f.y);
+            if (relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+            st_shared_f2(e + (uint32_t)(r * 128 + ((((c >> 2) ^ (r & 7)) << 4)) + (c & 3) * 4), y0, y1);
+            if (hp >= 0) *reinterpret_cast<float2*>(static_cast<float*>(halo->out) + (size_t)hp * halo->C + halo->n0 + c) = make_float2(y0, y1);
+        }
+    }
+}
+
+// Output tile of conv_tc_kernel in its epilogue slot: NPART parts of 128 rows x CW channels, `row_bytes` per row --
+// planes: hi plane then lo plane, each as BN / CW channel boxes (CW = 64, 128-byte swizzle; CW = 32 for BN = 32,
+// unswizzled); fp32: BN / 32 boxes of 32 channels (128-byte swizzle).  Every layout is BM * BN * 4 bytes, in two halves
+// of BM * BN * 2 bytes (the planes, or the first and last fp32 boxes) that may sit apart: the first half at `x`, the
+// second at `y`.
+template <int BN>
+struct EpiLayout {
+    int cw, nj, npart, row_bytes;
+    __device__ __forceinline__ explicit EpiLayout(bool f32)
+        : cw(f32 ? 32 : (BN < 64 ? BN : 64)), nj(BN / cw), npart(f32 ? BN / 32 : 2 * (BN / cw)), row_bytes(f32 ? 128 : 2 * cw) {}
+    __device__ __forceinline__ uint8_t* part(uint8_t* x, uint8_t* y, int k) const {
+        const int half = npart > 1 ? npart / 2 : 1;
+        return (k < half ? x : y) + (k % half) * BM * row_bytes;
+    }
+};
+
+// Output rows of M tile mt (mode 1): the first output row R0, how many of its rows_per_tile rows exist, first column
+__device__ __forceinline__ void tile_rows(const TcArgs& a, int mt, int& R0, int& valid_rows, int& wo0) {
+    const int rg = mt / a.wsegs;
+    wo0 = (mt - rg * a.wsegs) * a.tw;
+    R0 = rg * a.rows_per_tile;
+    valid_rows = min(a.rows_per_tile, a.M - R0);
+}
+
+// Residual load (`bar` counts the bytes) or output store of part k of tile (mt, nt) through tensor map tm (conv_tc_map):
+// mode 0 one box {cw, 128 rows}; mode 1 one box of all rows when `rowbox` makes them consecutive, else one box per
+// output row that exists
+template <int BN, bool STORE>
+__device__ __forceinline__ void tile_boxes(const TcArgs& a, const EpiLayout<BN>& L, const CUtensorMap* tm, uint8_t* x,
+                                           uint8_t* y, uint64_t* bar, int mt, int nt, int k) {
+    const int c0 = nt * BN + (k % L.nj) * L.cw, plane = k / L.nj;
+    uint8_t* dst = L.part(x, y, k);
+    if (a.mode == 0) {
+        if (STORE) tma_store_3d(tm, dst, c0, mt * BM, plane);
+        else tma_load_3d(dst, tm, bar, c0, mt * BM, plane);
+        return;
+    }
+    int R0, valid_rows, wo0;
+    tile_rows(a, mt, R0, valid_rows, wo0);
+    const int nbox = a.rowbox ? 1 : valid_rows;
+    for (int rr = 0; rr < nbox; ++rr) {
+        const int R = R0 + rr, b = R / a.Ho, ho = R - b * a.Ho;
+        uint8_t* d = dst + rr * a.tw * L.row_bytes;
+        if (STORE) tma_store_5d(tm, d, c0, wo0 + a.out_halo, ho, b, plane);
+        else tma_load_5d(d, tm, bar, c0, wo0 + a.out_halo, ho, b, plane);
+    }
 }
 
 template <int BN>
 __global__ void __launch_bounds__(NTHREADS, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
+conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+               const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO, const TcArgs a) {
     using S = Smem<BN>;
     constexpr int NST = S::NST;
+    constexpr int HALF_TILE = BM * BN * 2;     // one output plane; half an output tile
+    static_assert(2 * HALF_TILE <= S::STAGE, "an output tile must fit one ring stage");
     pdl_trigger();
     const int tile0 = (int)blockIdx.x;
     const int tstride = (int)gridDim.x;
@@ -144,121 +298,139 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::BAR_OFF);
     uint64_t* empty_bar = full_bar + NST;
-    uint64_t* afull_bar = empty_bar + NST;           // [2] dxr mode: input-row slot filled
+    uint64_t* oready_bar = empty_bar + NST;          // [NST] all 8 consumer warps have written the output tile in that stage
+    uint64_t* afull_bar = oready_bar + NST;         // [2] dxr mode: input-row slot filled
     uint64_t* aempty_bar = afull_bar + 2;           // [2] dxr mode: the three taps have read the input-row slot
     // dxr mode re-partitions the operand ring: two input-row slots (hi + lo plane, 136 rows of 128 B each, 130 used)
     // followed by NST weight-tile slots
     constexpr int AX_PLANE = 17 * 1024;
     constexpr int AX_SLOT = 2 * AX_PLANE;
     constexpr int BX_OFF = 2 * AX_SLOT;
-    static_assert(BX_OFF + NST * 2 * S::B_PLANE <= NST * S::STAGE, "dxr layout does not fit the operand ring");
-
+    constexpr int BX_SLOT = 2 * S::B_PLANE;
+    static_assert(BX_OFF + NST * BX_SLOT <= NST * S::STAGE, "dxr layout does not fit the operand ring");
+    static_assert(BX_SLOT == HALF_TILE, "a dxr weight slot holds half an output tile");
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const bool has_res = a.res != nullptr && !(a.dbg & 1);
+    // Ring sequence per tile: the tile's K chunks, then its epilogue slot -- one ring stage, which holds exactly one output
+    // tile, or in dxr mode two consecutive weight slots, each holding half of one (x: first half, y: second half).
+    // The producer fills the slot with the residual tile, the consumers turn it into the output tile in place, the store
+    // warp hands it to the TMA engine and releases the slot's stages to the producer.
+    const int epi_stages = a.dxr ? 2 : 1;
+    auto slot_x = [&](int st) { return smem + (a.dxr ? BX_OFF + st * BX_SLOT : st * S::STAGE); };
+    auto slot_y = [&](int st) { return a.dxr ? slot_x(st + 1 == NST ? 0 : st + 1) : slot_x(st) + HALF_TILE; };
 
     if (warp == 0 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmO)) : "memory");
     }
     if (warp == 1 && lane == 0) {
-        for (int i = 0; i < NST; ++i) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, CONS_WARPS); }
+        for (int i = 0; i < NST; ++i) {
+            mbar_init(full_bar + i, 1);
+            mbar_init(empty_bar + i, CONS_WARPS);
+            mbar_init(oready_bar + i, CONS_WARPS);
+        }
         for (int i = 0; i < 2; ++i) { mbar_init(afull_bar + i, 1); mbar_init(aempty_bar + i, CONS_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     pdl_wait();                                              // everything below reads / writes activations
-    // the epilogue constants, read from shared memory: global loads of them would sit in the epilogue's chain of output
-    // stores (the pointers may alias) and each wait out its latency.  Loaded after pdl_wait: in the training step the
-    // kernel before this one may have written them.
+    // the epilogue constants, loaded after pdl_wait: in the training step the kernel before this one may have written them
     float* cst = reinterpret_cast<float*>(smem + S::CST_OFF);
     for (int i = threadIdx.x; i < 2 * a.Cout; i += NTHREADS) cst[i] = (i < a.Cout) ? a.scale[i] : a.shift[i - a.Cout];
     __syncthreads();
 
     if (warp == 0) {
         // =============================== TMA producer ===============================
-        if (lane == 0 && a.dxr) {
-            // 3x3 conv, one output row of 128 pixels per tile: per (dy, channel chunk) ONE box of 130 input pixels,
-            // then the three weight tiles of that (dy, chunk)
-            int ast = 0, bst = 0;
-            uint32_t aph = 0, bph = 0;
-            const int ndyc = a.num_kc / a.kw;
-            for (int tile = tile0; tile < a.num_tiles; tile += tstride) {
-                const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-                const int rg = mt / a.wsegs;
-                const int wo0 = (mt - rg * a.wsegs) * a.tw;
-                const int b = rg / a.Ho, ho = rg - b * a.Ho;
-                for (int dyc = 0; dyc < ndyc; ++dyc) {
-                    const int dy = dyc / a.kc_per_tap, cc = dyc - dy * a.kc_per_tap;
-                    const int hin = ho * a.sh + dy - a.ph;
-                    mbar_wait(aempty_bar + ast, aph ^ 1);
-                    uint8_t* sAx = smem + ast * AX_SLOT;
-                    mbar_expect_tx(afull_bar + ast, 2u * 130u * 128u);
-                    tma_load_4d(sAx, &tmA, afull_bar + ast, cc * BKC, wo0 + a.woff, hin, b);
-                    tma_load_4d(sAx + AX_PLANE, &tmA, afull_bar + ast, cc * BKC, wo0 + a.woff, hin, a.Bimg + b);
-                    if (++ast == 2) { ast = 0; aph ^= 1; }
-                    for (int dx = 0; dx < 3; ++dx) {
-                        mbar_wait(empty_bar + bst, bph ^ 1);
-                        uint8_t* sB = smem + BX_OFF + bst * 2 * S::B_PLANE;
-                        mbar_expect_tx(full_bar + bst, 2u * S::B_PLANE);
-                        const int kb = ((dy * a.kw + dx) * a.kc_per_tap + cc) * BKC;
-                        tma_load_3d(sB, &tmB, full_bar + bst, kb, nt * BN, 0);
-                        tma_load_3d(sB + S::B_PLANE, &tmB, full_bar + bst, kb, nt * BN, 1);
-                        if (++bst == NST) { bst = 0; bph ^= 1; }
-                    }
-                }
-            }
-        } else if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
+        if (lane == 0) {
+            int stage = 0, ast = 0;
+            uint32_t phase = 0, aph = 0;
             for (int tile = tile0; tile < a.num_tiles; tile += tstride) {
                 const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
                 int valid_rows = 1, row0 = 0, wo0 = 0;
-                if (a.mode == 1) {
-                    const int rg = mt / a.wsegs;
-                    wo0 = (mt - rg * a.wsegs) * a.tw;
-                    row0 = rg * a.rows_per_tile;
-                    valid_rows = min(a.rows_per_tile, a.M - row0);
-                }
-                // a row box always delivers the full tile (rows past the end are out-of-bounds zero fill, full byte count)
-                const uint32_t a_bytes = (a.mode == 0) ? 2u * S::A_PLANE
-                                                       : (uint32_t)(2 * (a.rowbox ? a.rows_per_tile : valid_rows) * a.tw * BKC * 2);
-                for (int kc = 0; kc < a.num_kc; ++kc) {
-                    mbar_wait(empty_bar + stage, phase ^ 1);
-                    uint8_t* sA = smem + stage * S::STAGE;
-                    uint8_t* sB = sA + 2 * S::A_PLANE;
-                    const int tap = kc / a.kc_per_tap;
-                    const int c0 = (kc - tap * a.kc_per_tap) * BKC;
-                    mbar_expect_tx(full_bar + stage, a_bytes + 2u * S::B_PLANE);
-                    if (a.mode == 0) {
-                        tma_load_3d(sA, &tmA, full_bar + stage, c0, mt * BM, 0);
-                        tma_load_3d(sA + S::A_PLANE, &tmA, full_bar + stage, c0, mt * BM, 1);
-                    } else {
-                        const int dy = tap / a.kw, dx = tap - dy * a.kw;
-                        // rowbox: the tile's output rows map to consecutive input rows of one image: one box per plane
-                        const int nbox = a.rowbox ? 1 : valid_rows;
-                        for (int rr = 0; rr < nbox; ++rr) {
-                            const int R = row0 + rr;
-                            const int b = R / a.Ho, ho = R - b * a.Ho;
-                            const int hin = ho * a.sh + dy - a.ph;
-                            uint8_t* dst = sA + rr * a.tw * (BKC * 2);
-                            if (a.parity) {
-                                const int p = dx + a.woff;
-                                tma_load_5d(dst, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin, b);
-                                tma_load_5d(dst + S::A_PLANE, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin,
-                                            a.Bimg + b);
-                            } else {
-                                tma_load_4d(dst, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin, b);
-                                tma_load_4d(dst + S::A_PLANE, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin,
-                                            a.Bimg + b);
-                            }
+                if (a.mode == 1) tile_rows(a, mt, row0, valid_rows, wo0);
+                if (a.dxr) {
+                    // 3x3 conv, one output row of 128 pixels per tile: per (dy, channel chunk) ONE box of 130 input pixels,
+                    // then the three weight tiles of that (dy, chunk)
+                    const int ndyc = a.num_kc / a.kw;
+                    const int b = row0 / a.Ho, ho = row0 - b * a.Ho;
+                    for (int dyc = 0; dyc < ndyc; ++dyc) {
+                        const int dy = dyc / a.kc_per_tap, cc = dyc - dy * a.kc_per_tap;
+                        const int hin = ho * a.sh + dy - a.ph;
+                        mbar_wait(aempty_bar + ast, aph ^ 1);
+                        uint8_t* sAx = smem + ast * AX_SLOT;
+                        mbar_expect_tx(afull_bar + ast, 2u * 130u * 128u);
+                        tma_load_4d(sAx, &tmA, afull_bar + ast, cc * BKC, wo0 + a.woff, hin, b);
+                        tma_load_4d(sAx + AX_PLANE, &tmA, afull_bar + ast, cc * BKC, wo0 + a.woff, hin, a.Bimg + b);
+                        if (++ast == 2) { ast = 0; aph ^= 1; }
+                        for (int dx = 0; dx < 3; ++dx) {
+                            mbar_wait(empty_bar + stage, phase ^ 1);
+                            uint8_t* sB = smem + BX_OFF + stage * BX_SLOT;
+                            mbar_expect_tx(full_bar + stage, 2u * S::B_PLANE);
+                            const int kb = ((dy * a.kw + dx) * a.kc_per_tap + cc) * BKC;
+                            tma_load_3d(sB, &tmB, full_bar + stage, kb, nt * BN, 0);
+                            tma_load_3d(sB + S::B_PLANE, &tmB, full_bar + stage, kb, nt * BN, 1);
+                            if (++stage == NST) { stage = 0; phase ^= 1; }
                         }
                     }
-                    tma_load_3d(sB, &tmB, full_bar + stage, kc * BKC, nt * BN, 0);
-                    tma_load_3d(sB + S::B_PLANE, &tmB, full_bar + stage, kc * BKC, nt * BN, 1);
+                } else {
+                    // a row box always delivers the full tile (rows past the end are out-of-bounds zero fill, full byte count)
+                    const uint32_t a_bytes = (a.mode == 0) ? 2u * S::A_PLANE
+                                                           : (uint32_t)(2 * (a.rowbox ? a.rows_per_tile : valid_rows) * a.tw * BKC * 2);
+                    for (int kc = 0; kc < a.num_kc; ++kc) {
+                        mbar_wait(empty_bar + stage, phase ^ 1);
+                        uint8_t* sA = smem + stage * S::STAGE;
+                        uint8_t* sB = sA + 2 * S::A_PLANE;
+                        const int tap = kc / a.kc_per_tap;
+                        const int c0 = (kc - tap * a.kc_per_tap) * BKC;
+                        mbar_expect_tx(full_bar + stage, a_bytes + 2u * S::B_PLANE);
+                        if (a.mode == 0) {
+                            tma_load_3d(sA, &tmA, full_bar + stage, c0, mt * BM, 0);
+                            tma_load_3d(sA + S::A_PLANE, &tmA, full_bar + stage, c0, mt * BM, 1);
+                        } else {
+                            const int dy = tap / a.kw, dx = tap - dy * a.kw;
+                            // rowbox: the tile's output rows map to consecutive input rows of one image: one box per plane
+                            const int nbox = a.rowbox ? 1 : valid_rows;
+                            for (int rr = 0; rr < nbox; ++rr) {
+                                const int R = row0 + rr;
+                                const int b = R / a.Ho, ho = R - b * a.Ho;
+                                const int hin = ho * a.sh + dy - a.ph;
+                                uint8_t* dst = sA + rr * a.tw * (BKC * 2);
+                                if (a.parity) {
+                                    const int p = dx + a.woff;
+                                    tma_load_5d(dst, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin, b);
+                                    tma_load_5d(dst + S::A_PLANE, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin,
+                                                a.Bimg + b);
+                                } else {
+                                    tma_load_4d(dst, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin, b);
+                                    tma_load_4d(dst + S::A_PLANE, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin,
+                                                a.Bimg + b);
+                                }
+                            }
+                        }
+                        tma_load_3d(sB, &tmB, full_bar + stage, kc * BKC, nt * BN, 0);
+                        tma_load_3d(sB + S::B_PLANE, &tmB, full_bar + stage, kc * BKC, nt * BN, 1);
+                        if (++stage == NST) { stage = 0; phase ^= 1; }
+                    }
+                }
+                // epilogue slot: the residual tile lands while the tile's last chunks compute
+                const int st0 = stage;
+                for (int e = 0; e < epi_stages; ++e) {
+                    mbar_wait(empty_bar + stage, phase ^ 1);
+                    if (e > 0 || !has_res) mbar_arrive(full_bar + stage);
                     if (++stage == NST) { stage = 0; phase ^= 1; }
+                }
+                if (has_res) {
+                    const EpiLayout<BN> L(false);
+                    // boxes per output row move only the rows that exist; a box past the end delivers its full size
+                    const int rows = (a.mode == 0 || a.rowbox) ? BM : valid_rows * a.tw;
+                    mbar_expect_tx(full_bar + st0, (uint32_t)(rows * BN * 4));
+                    for (int k = 0; k < L.npart; ++k)
+                        tile_boxes<BN, false>(a, L, &tmR, slot_x(st0), slot_y(st0), full_bar + st0, mt, nt, k);
                 }
             }
         }
     } else if (warp >= CONS_WARP0) {
-        // =============================== consumers: MMA + epilogue ===============================
+        // =============================== consumers: MMA + in-place epilogue ===============================
         const int wg = (warp - CONS_WARP0) >> 2;         // tile rows [64 wg, 64 wg + 64)
         const uint32_t a_row_off = (uint32_t)(wg * 64 * 128);
         float acc[BN / 2], sum[BN / 2];
@@ -266,19 +438,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         uint32_t phase = 0, aph = 0;
         for (int tile = tile0; tile < a.num_tiles; tile += tstride) {
             const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-            if (a.res && !(a.dbg & 1)) {
-                // The epilogue reads the residual inside its chain of output stores (the pointers may alias, so the
-                // compiler keeps the order), where every load waits out its full latency.  Pull the tile's residual
-                // rows into L2 now, while its MMAs run: lane l of a warp takes row l % 16 of the warp's 16 rows in
-                // plane l / 16, BN * 2 bytes = BN / 64 lines of 128 B (one for BN < 64).
-                bool ok;
-                const size_t px = tile_pixel(a, mt, wg * 64 + (warp & 3) * 16 + (lane & 15), ok);
-                if (ok) {
-                    const unsigned short* row = a.res + (lane >> 4) * a.out_plane + px * (size_t)a.Cout + nt * BN;
-#pragma unroll
-                    for (int l = 0; l < (BN + 63) / 64; ++l) prefetch_l2(row + l * 64);
-                }
-            }
 #pragma unroll
             for (int j = 0; j < BN / 2; ++j) sum[j] = 0.f;
             int seg_pos = 0, held = -1;      // held: ring stage whose wgmma group may still be in flight
@@ -314,7 +473,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     for (int dx = 0; dx < 3; ++dx, ++kc) {
                         mbar_wait(full_bar + stage, phase);
                         // tap dx = the same 130-pixel row read from pixel dx on: start address + dx rows of 128 B
-                        step(sAx + dx * 128, AX_PLANE, smem_u32(smem + BX_OFF + stage * 2 * S::B_PLANE), stage,
+                        step(sAx + dx * 128, AX_PLANE, smem_u32(smem + BX_OFF + stage * BX_SLOT), stage,
                              kc == a.num_kc - 1, dx == 2);
                         if (++stage == NST) { stage = 0; phase ^= 1; }
                     }
@@ -331,92 +490,84 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
 
-            // ---- epilogue from the fragments: this thread holds rows r0, r0 + 8 and columns 8j + 2(lane%4) + {0,1}
-            size_t pix[2], halo_pix[2];
-            bool valid[2], has_halo[2];
+            // ---- epilogue in the slot
+            HaloStore halo = {a.out_f32 ? static_cast<void*>(a.out_f32) : a.out, a.out_plane, a.Cout, 0, {-1, -1}};
+            if (a.mode == 1 && a.out_halo && !(a.dbg & 2)) {
+                int R0, rows, wo0;
+                tile_rows(a, mt, R0, rows, wo0);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
-                has_halo[h] = false;
-                halo_pix[h] = 0;
-                pix[h] = tile_pixel(a, mt, r, valid[h]);
-                if (a.mode == 1) {
-                    const int rg = mt / a.wsegs;
-                    const int wo = (mt - rg * a.wsegs) * a.tw + (r % a.tw);
-                    const int R = rg * a.rows_per_tile + r / a.tw;
-                    if (a.out_halo) {
-                        if (wo == 0) { has_halo[h] = true; halo_pix[h] = (size_t)R * a.Wop + a.Wo + 1; }
-                        else if (wo == a.Wo - 1) { has_halo[h] = true; halo_pix[h] = (size_t)R * a.Wop; }
-                    }
+                for (int h = 0; h < 2; ++h)
+                    halo.pix[h] = halo_pixel(frag_row(wg, warp, lane, h), (long long)R0 * a.Wop, a.Wop, a.tw, rows, wo0, a.Wo);
+            }
+            const int st0 = stage;
+            const uint32_t x = smem_u32(slot_x(st0)), y = smem_u32(slot_y(st0));
+            for (int e = 0; e < epi_stages; ++e) {
+                mbar_wait(full_bar + stage, phase);
+                if (++stage == NST) { stage = 0; phase ^= 1; }
+            }
+            const float* sc = cst + nt * BN;
+            const float* sf = cst + a.Cout + nt * BN;
+            if (a.out_f32) {
+                // fp32 boxes of 32 channels, the first half at x (BN = 32: its one box; the plan keeps that out of dxr)
+                constexpr int HQ = BN / 64 > 0 ? BN / 64 : 1;
+#pragma unroll
+                for (int q = 0; q < BN / 32; ++q) {
+                    halo.n0 = nt * BN + 32 * q;
+                    epi_f32(*reinterpret_cast<const float(*)[16]>(sum + 16 * q), sc + 32 * q, sf + 32 * q,
+                            (q < HQ ? x : y) + (q % HQ) * BM * 128, a.relu != 0, wg, warp, lane, &halo);
+                }
+            } else if (BN == 32) {
+                halo.n0 = nt * BN;
+                epi_inplace<32>(*reinterpret_cast<const float(*)[16]>(sum), sc, sf, x, y, has_res, a.relu != 0, wg, warp,
+                                lane, &halo);
+            } else {
+#pragma unroll
+                for (int j = 0; j < BN / 64; ++j) {
+                    halo.n0 = nt * BN + 64 * j;
+                    epi_inplace<64>(*reinterpret_cast<const float(*)[32]>(sum + 32 * j), sc + 64 * j, sf + 64 * j,
+                                    x + j * BM * 128, y + j * BM * 128, has_res, a.relu != 0, wg, warp, lane, &halo);
                 }
             }
-#pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const int n = nt * BN + 8 * j + 2 * (lane & 3);          // output channel of the pair
-                const float2 sc = *reinterpret_cast<const float2*>(cst + n);
-                const float2 sf = *reinterpret_cast<const float2*>(cst + a.Cout + n);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    if (!valid[h]) continue;
-                    float y0 = fmaf(sum[4 * j + 2 * h], sc.x, sf.x);
-                    float y1 = fmaf(sum[4 * j + 2 * h + 1], sc.y, sf.y);
-                    const size_t e = pix[h] * (size_t)a.Cout + n;
-                    if (a.res && !(a.dbg & 1)) {        // y is in plane units here: no rescaling needed
-                        const float2 fh = unpack_half2(__ldg(reinterpret_cast<const unsigned int*>(a.res + e)));
-                        const float2 fl = unpack_half2(__ldg(reinterpret_cast<const unsigned int*>(a.res + a.out_plane + e)));
-                        y0 += fh.x + fl.x;
-                        y1 += fh.y + fl.y;
-                    }
-                    if (a.relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
-                    if (a.dbg & 2) continue;
-                    const size_t eh = halo_pix[h] * (size_t)a.Cout + n;
-                    if (a.out_f32) {
-                        const float2 v = make_float2(y0, y1);
-                        *reinterpret_cast<float2*>(a.out_f32 + e) = v;
-                        if (has_halo[h]) *reinterpret_cast<float2*>(a.out_f32 + eh) = v;
-                    } else {
-                        uint32_t ph, pl;
-                        split2_scaled(y0, y1, ph, pl);
-                        *reinterpret_cast<uint32_t*>(a.out + e) = ph;
-                        *reinterpret_cast<uint32_t*>(a.out + a.out_plane + e) = pl;
-                        if (has_halo[h]) {
-                            *reinterpret_cast<uint32_t*>(a.out + eh) = ph;
-                            *reinterpret_cast<uint32_t*>(a.out + a.out_plane + eh) = pl;
-                        }
-                    }
+            // make the generic-proxy writes visible to the TMA engine and tell the store warp
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            __syncwarp();
+            if (lane == 0) mbar_arrive(oready_bar + st0);
+        }
+    } else if (warp == 3) {
+        // =============================== store warp ===============================
+        // one thread follows the ring to each tile's epilogue slot, stores the output tile from it with TMA and
+        // releases the slot's stages to the producer once the engine has read it
+        if (lane == 0) {
+            int stage = 0;
+            uint32_t ophase = 0;                   // bit s: phase of oready_bar[s]
+            for (int tile = tile0; tile < a.num_tiles; tile += tstride) {
+                const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
+                stage = (stage + a.num_kc) % NST;
+                mbar_wait(oready_bar + stage, (ophase >> stage) & 1);
+                ophase ^= 1u << stage;
+                if (!(a.dbg & 2)) {
+                    const EpiLayout<BN> L(a.out_f32 != nullptr);
+                    for (int k = 0; k < L.npart; ++k)
+                        tile_boxes<BN, true>(a, L, &tmO, slot_x(stage), slot_y(stage), nullptr, mt, nt, k);
+                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                }
+                for (int e = 0; e < epi_stages; ++e) {
+                    mbar_arrive_cnt(empty_bar + stage, CONS_WARPS);
+                    if (++stage == NST) stage = 0;
                 }
             }
+            asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");          // all stores have landed
         }
     }
 }
 
-// tile row of accumulator element pair h (0: d[4j], d[4j+1]; 1: d[4j+2], d[4j+3]) of this thread's wgmma fragment
-__device__ __forceinline__ int frag_row(int wg, int warp, int lane, int h) {
-    return wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
-}
-// byte offset of the column pair (c, c + 1), c even, of tile row r in a [rows][64 fp16] buffer with 128-byte swizzle
-__device__ __forceinline__ uint32_t swz_pair_off(int r, int c) {
-    return (uint32_t)(r * 128 + ((((c >> 3) ^ (r & 7)) << 4)) + (c & 7) * 2);
-}
-__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
-    uint32_t v;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
-    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ void st_shared_f2(uint32_t addr, float a, float b) {
-    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
-}
-// named barrier of one consumer warpgroup (ids 1, 2; id 0 is __syncthreads)
-__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
-
 // ================================================================================================
 // gemm_tc_kernel: 1x1 stride-1 convolutions in GEMM mode with K <= 256 (conv3 / conv1 of layer1-3: the
-// bottlenecks).  These layers are bound by the epilogue, not by the MMAs: in conv_tc_kernel the residual
-// loads and the output stores of a tile sit in the epilogue's dependency chain.  Here all epilogue traffic is
-// asynchronous: the producer warp TMA-loads the residual tile (hi, lo planes, 128 rows x 64 channels, 128-byte
+// bottlenecks).  These layers are bound by the epilogue, not by the MMAs.  Like conv_tc_kernel's, all epilogue
+// traffic is asynchronous, but with two dedicated epilogue buffers instead of a ring stage per tile (measured faster
+// than conv_tc_kernel<128> on 7 of these 15 launches of the batch-32 forward, DESIGN section 3): the producer warp
+// TMA-loads the residual tile (hi, lo planes, 128 rows x 64 channels, 128-byte
 // swizzle) into one of two epilogue buffers a whole tile ahead, the consumer warpgroups update it IN PLACE from their
 // accumulator fragments (BN scale/shift, + residual, ReLU, re-split) and one thread (warp 3) hands the buffer to the
 // TMA engine for the store.  Tiles are 128 x 64 so that a 3-stage operand ring (48 KB/stage) and the two 32 KB
@@ -436,65 +587,12 @@ struct GSmem {
     static constexpr int TOTAL = CST_OFF + 2 * MAX_COUT * 4 + 1024;
 };
 
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, const void* src, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                     reinterpret_cast<uint64_t>(tm)),
-                 "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
-                 : "memory");
-}
 __device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* tm, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(reinterpret_cast<uint64_t>(tm)),
                  "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
 }
 
-// circular halo columns of an output row (hn_common.cuh): wp = Wo + 1 copies wo = 0, wp = 0 copies wo = Wo - 1
-struct HaloStore {
-    unsigned short* out;      // output planes (hi; lo at + out_plane)
-    size_t out_plane;
-    long long rowbase;        // pixel index of wp = 0 of the tile's output row
-    int wo0, Wo, C, n0;       // first column of the tile, row width, channels, first channel of the 64-channel tile
-};
-
-// In-place epilogue of a 64-channel output tile held as fragments `acc` (rows of this warpgroup): y = acc*sc + sf
-// (+ the residual the buffer holds) (ReLU), re-split into the hi / lo planes of the swizzled buffer e_hi / e_lo.
-// gemm_tc_kernel and the conv3 stage of bott_tc_kernel share it, so their results agree bit for bit.
-__device__ __forceinline__ void epi_inplace64(const float (&acc)[32], const float* sc, const float* sf, uint32_t e_hi,
-                                              uint32_t e_lo, bool has_res, bool relu, int wg, int warp, int lane,
-                                              const HaloStore* halo = nullptr) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int r = frag_row(wg, warp, lane, h);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int c = 8 * j + 2 * (lane & 3);
-            const float2 k = *reinterpret_cast<const float2*>(sc + c);
-            const float2 f = *reinterpret_cast<const float2*>(sf + c);
-            float y0 = fmaf(acc[4 * j + 2 * h], k.x, f.x);
-            float y1 = fmaf(acc[4 * j + 2 * h + 1], k.y, f.y);
-            const uint32_t off = swz_pair_off(r, c);
-            if (has_res) {                                    // y is in plane units here: no rescaling needed
-                const float2 fh = unpack_half2(ld_shared_u32(e_hi + off)), fl = unpack_half2(ld_shared_u32(e_lo + off));
-                y0 += fh.x + fl.x;
-                y1 += fh.y + fl.y;
-            }
-            if (relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
-            uint32_t ph, pl;
-            split2_scaled(y0, y1, ph, pl);
-            st_shared_u32(e_hi + off, ph);
-            st_shared_u32(e_lo + off, pl);
-            if (halo) {
-                const int wo = halo->wo0 + r;
-                const long long hp = wo == 0 ? halo->rowbase + halo->Wo + 1 : (wo == halo->Wo - 1 ? halo->rowbase : -1);
-                if (hp >= 0) {
-                    unsigned short* o = halo->out + (size_t)hp * halo->C + halo->n0 + c;
-                    *reinterpret_cast<uint32_t*>(o) = ph;
-                    *reinterpret_cast<uint32_t*>(o + halo->out_plane) = pl;
-                }
-            }
-        }
-    }
-}
 
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -602,7 +700,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             const int eb = it & 1;
             mbar_wait(rfull_bar + eb, (it >> 1) & 1);
             const uint32_t e_hi = smem_u32(smem + S::EPI_OFF + eb * S::EBUF);
-            epi_inplace64(sum, cst + nt * GBN, cst + a.Cout + nt * GBN, e_hi, e_hi + S::E_PLANE, has_res, a.relu != 0, wg,
+            epi_inplace<64>(sum, cst + nt * GBN, cst + a.Cout + nt * GBN, e_hi, e_hi + S::E_PLANE, has_res, a.relu != 0, wg,
                           warp, lane);
             // make the generic-proxy writes visible to the TMA engine and tell the store warp
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -860,7 +958,7 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // bott_tc_kernel: conv2 (3x3, stride 1, 64 -> 64) + BN + ReLU  FUSED WITH  conv3 (1x1, 64 -> C3) + BN + identity + ReLU
 // of a layer1 bottleneck (torchvision Bottleneck.forward; reference model.py:78).  Per tile of 128 pixels of one
 // output row, each consumer warpgroup (64 of the pixels):
-//   stage 1   computes the conv2 tile exactly as conv_tc_kernel<64> in "dxr" mode does (same wgmma order, segments,
+//   stage 1   computes the conv2 tile exactly as conv_tc_kernel<64> does (same wgmma order, segments,
 //             epilogue maths), but writes the BN+ReLU'd result as hi/lo planes into SHARED memory (t2, [128 px][64 ch]
 //             rows of 128 B, 128-byte swizzle: exactly a K-major wgmma A operand) instead of HBM;
 //   stage 2   runs conv3 as C3 / 64 tiles of 128 x 64 with A = t2, B = conv3 weights, the residual tile TMA-loaded into
@@ -1030,7 +1128,7 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
             const int rg = tile / a.wsegs;
             const int wo0 = (tile - rg * a.wsegs) * BM;
-            // ---- conv2 (identical to conv_tc_kernel<64> in dxr mode)
+            // ---- conv2 (identical to conv_tc_kernel<64>)
 #pragma unroll
             for (int j = 0; j < 32; ++j) sum[j] = 0.f;
             int seg_pos = 0, kc = 0;
@@ -1072,7 +1170,10 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> wgmma operand reads
             wg_sync(wg);
             // ---- conv3: one 128 x 64 tile per 64 output channels, in-place epilogue on the residual tile
-            const HaloStore halo = {a.out, a.out_plane, (long long)rg * a.Wop, wo0, a.Wo, a.C3, 0};
+            HaloStore halo = {a.out, a.out_plane, a.C3, 0, {-1, -1}};
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                halo.pix[h] = halo_pixel(frag_row(wg, warp, lane, h), (long long)rg * a.Wop, a.Wop, BM, 1, wo0, a.Wo);
             for (int j = 0; j < n3; ++j, ++g3) {
                 mbar_wait(full_bar + bst, bph);
                 const uint32_t sB = smem_u32(smem + S::B_OFF + bst * S::B_STAGE);
@@ -1085,7 +1186,7 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 const uint32_t e_hi = smem_u32(smem + S::E_OFF + eb * S::EBUF);
                 HaloStore hj = halo;
                 hj.n0 = j * 64;
-                epi_inplace64(sum, cst + 128 + j * 64, cst + 128 + a.C3 + j * 64, e_hi, e_hi + S::E_PLANE, true, true, wg,
+                epi_inplace<64>(sum, cst + 128 + j * 64, cst + 128 + a.C3 + j * 64, e_hi, e_hi + S::E_PLANE, true, true, wg,
                               warp, lane, &hj);
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                 __syncwarp();
@@ -1114,13 +1215,37 @@ bool tc_prefetch_on() {
 }
 
 template <int BN>
-int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcArgs& a, int grid, cudaStream_t st) {
+int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO, const TcArgs& a,
+           int grid, cudaStream_t st) {
     const int bytes = conv_smem_bytes<BN>(a.Cout);
     HN_CHECK(bytes <= MAX_SMEM, "conv_tc: too many output channels for the epilogue constants in shared memory");
     HN_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    HN_CUDA_OK(launch_tc(conv_tc_kernel<BN>, grid, bytes, st, tmA, tmB, a));
+    HN_CUDA_OK(launch_tc(conv_tc_kernel<BN>, grid, bytes, st, tmA, tmB, tmR, tmO, a));
     HN_LAUNCH_OK();
     return 0;
+}
+
+// Tensor map of an output-geometry tensor (output or residual) as the epilogue of a tile with BN channels moves it (see
+// EpiLayout): planes (hi, lo: an outer dimension of 2) or fp32 (an outer dimension of 1).  Mode 0 {Cout, M pixels,
+// plane}, box {cw, 128}; mode 1 {Cout, Wop, Ho, B, plane} -- the plane has its own dimension, so a box clipped past the
+// last image never spills into the lo plane -- box {cw, tw, box rows, box images} with `rowbox`, else {cw, tw, 1, 1}.
+int conv_tc_map(CUtensorMap* tm, const void* base, const TcPlan& pl, const Act& out, int Cout, bool f32) {
+    const cuuint64_t es = f32 ? 4 : 2, C = (cuuint64_t)Cout, plane_bytes = (cuuint64_t)out.numel() * es;
+    const cuuint32_t cw = f32 ? 32u : (pl.BN < 64 ? (cuuint32_t)pl.BN : 64u);
+    const CUtensorMapDataType dt = f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    const CUtensorMapSwizzle sw = (cw * es == 128) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE;
+    const cuuint64_t planes = f32 ? 1 : 2;
+    if (pl.mode == 0) {
+        cuuint64_t dims[3] = {C, (cuuint64_t)pl.M, planes};
+        cuuint64_t str[2] = {C * es, plane_bytes};
+        cuuint32_t box[3] = {cw, (cuuint32_t)BM, 1};
+        return make_map(tm, base, 3, dims, str, box, -1, 1, dt, sw);
+    }
+    const cuuint64_t Wop = out.Wp();
+    cuuint64_t dims[5] = {C, Wop, (cuuint64_t)out.H, (cuuint64_t)out.B, planes};
+    cuuint64_t str[4] = {C * es, C * es * Wop, C * es * Wop * out.H, plane_bytes};
+    cuuint32_t box[5] = {cw, (cuuint32_t)pl.tw, pl.rowbox ? (cuuint32_t)pl.box_rows : 1u, pl.rowbox ? (cuuint32_t)pl.box_imgs : 1u, 1};
+    return make_map(tm, base, 5, dims, str, box, -1, 1, dt, sw);
 }
 
 }  // namespace
@@ -1189,9 +1314,11 @@ int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32,
             if (out.H % p->rows_per_tile == 0) { p->rowbox = 1; p->box_rows = p->rows_per_tile; }
             else if (p->rows_per_tile % out.H == 0) { p->rowbox = 1; p->box_rows = out.H; p->box_imgs = p->rows_per_tile / out.H; }
         }
-        // dx reuse (HN_TC_DXR=0 disables)
+        // dx reuse (HN_TC_DXR=0 disables).  Its epilogue slot is two weight slots, each half an output tile: a plane, or
+        // half of the fp32 boxes -- which needs two of them (BN >= 64)
         static const int dxr_mode = [] { const char* e = getenv("HN_TC_DXR"); return e ? atoi(e) : 1; }();
         p->dxr = (dxr_mode != 0 && !p->parity && d.kw == 3 && p->rows_per_tile == 1 && p->tw == BM &&
+                  !(out_f32 && BN < 64) &&
                   (long long)p->wsegs * BM + (in.halo - d.pw) + 2 <= (long long)in.Wp()) ? 1 : 0;
         m_tiles = (long long)((p->M + p->rows_per_tile - 1) / p->rows_per_tile) * p->wsegs;
     }
@@ -1245,13 +1372,8 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
             cuuint32_t box[3] = {BKC, BM, 1};
             if (make_map(&tmA, in_planes, 3, dims, str, box)) return -1;
         }
-        {
-            cuuint64_t dims[3] = {(cuuint64_t)d.Cout, (cuuint64_t)Mtot, 2};
-            cuuint64_t str[2] = {(cuuint64_t)d.Cout * 2, (cuuint64_t)out_plane * 2};
-            cuuint32_t box[3] = {GBN, BM, 1};
-            if (make_map(&tmO, out_planes, 3, dims, str, box)) return -1;
-            if (make_map(&tmR, res_planes ? res_planes : out_planes, 3, dims, str, box)) return -1;
-        }
+        if (conv_tc_map(&tmO, out_planes, pl, out, d.Cout, false)) return -1;
+        if (conv_tc_map(&tmR, res_planes ? res_planes : out_planes, pl, out, d.Cout, false)) return -1;
         HN_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GSmem::TOTAL));
         HN_CUDA_OK(launch_tc(gemm_tc_kernel, pl.grid, GSmem::TOTAL, st, tmA, tmB, tmR, tmO, a));
         HN_LAUNCH_OK();
@@ -1288,10 +1410,15 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
         }
     }
     if (a.num_tiles == 0) return 0;
+    CUtensorMap tmR, tmO;
+    const bool f32 = out_f32 != nullptr;
+    const void* obase = f32 ? static_cast<const void*>(out_f32) : static_cast<const void*>(out_planes);
+    if (conv_tc_map(&tmO, obase, pl, out, d.Cout, f32)) return -1;
+    if (conv_tc_map(&tmR, res_planes ? static_cast<const void*>(res_planes) : obase, pl, out, d.Cout, f32)) return -1;
     switch (BN) {
-        case 128: return launch<128>(tmA, tmB, a, pl.grid, st);
-        case 64: return launch<64>(tmA, tmB, a, pl.grid, st);
-        default: return launch<32>(tmA, tmB, a, pl.grid, st);
+        case 128: return launch<128>(tmA, tmB, tmR, tmO, a, pl.grid, st);
+        case 64: return launch<64>(tmA, tmB, tmR, tmO, a, pl.grid, st);
+        default: return launch<32>(tmA, tmB, tmR, tmO, a, pl.grid, st);
     }
 }
 

@@ -11,6 +11,7 @@ its predecessor, HN_TC_PDL=0 gives the clean attribution.
 """
 import argparse
 import json
+import math
 import os
 import re
 import subprocess
@@ -49,6 +50,22 @@ def model_bytes(c, p):
     else:
         a_tile = kc * 128 * 64 * 4
     return n * (a_tile + b_tile)
+
+
+def round_fit(rows, sms):
+    """Least-squares fit of the conv_tc_kernel<128> launches: us per tile round = slope * K chunks + intercept, a round
+    being the ceil(num_tiles / sms) tiles each persistent CTA runs.  The intercept is the fixed cost paid once per tile."""
+    pts = [(r['num_kc'], r['us'] / math.ceil(r['num_tiles'] / sms)) for r in rows if r['kernel'] == 'conv_tc_kernel<128>']
+    n = len(pts)
+    if n < 2:
+        return None
+    mx, my = sum(x for x, _ in pts) / n, sum(y for _, y in pts) / n
+    sxx = sum((x - mx) ** 2 for x, _ in pts)
+    slope = sum((x - mx) * (y - my) for x, y in pts) / sxx
+    icpt = my - slope * mx
+    return {'launches': n, 'us_per_chunk': round(slope, 3), 'us_per_tile': round(icpt, 2),
+            'max_residual_us': round(max(abs(y - slope * x - icpt) for x, y in pts), 2),
+            'tile_rounds': sum(math.ceil(r['num_tiles'] / sms) for r in rows if r['kernel'] == 'conv_tc_kernel<128>')}
 
 
 def card():
@@ -127,11 +144,12 @@ def main():
     res = {'card': card(), 'batch': B, 'reps': args.reps, 'env': env,
            'what': 'median device duration over the reps of each convolution launch of the plain forward (torch.profiler)',
            'family_ms': fam, 'conv_tc_kernel_ms': round(sum(r['us'] for r in rows if 'conv_tc_kernel' in r['kernel']) / 1e3, 3),
-           'total_ms': round(sum(r['us'] for r in rows) / 1e3, 3), 'launches': rows}
+           'total_ms': round(sum(r['us'] for r in rows) / 1e3, 3),
+           'round_fit': round_fit(rows, torch.cuda.get_device_properties(dev).multi_processor_count), 'launches': rows}
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     with open(args.out, 'w') as f:
         json.dump(res, f, indent=1)
-    print(json.dumps({k: res[k] for k in ('card', 'env', 'family_ms', 'conv_tc_kernel_ms', 'total_ms')}))
+    print(json.dumps({k: res[k] for k in ('card', 'env', 'family_ms', 'conv_tc_kernel_ms', 'total_ms', 'round_fit')}))
 
 
 if __name__ == '__main__':
