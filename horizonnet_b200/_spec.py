@@ -1,9 +1,10 @@
-"""Architecture spec of the one model family on the hot path: ``resnet50`` + bi-LSTM head.
+"""Architecture spec of the model family on the hot path: ``resnet50`` + bi-LSTM head, or + per-column MLP head.
 
 Everything here is derived from the *checkpoint layout* the reference writes
-(reference misc/utils.py:49-58, model.py:189-246) -- 448 keys, probed from the reference and
-pinned by tests/golden/state_dict_keys.json.  The C library builds the same graph from the same
-key names (csrc/model.cu), so this file is the single Python-side description of names + shapes.
+(reference misc/utils.py:49-58, model.py:189-246) -- 448 keys with the bi-LSTM, 434 with the MLP head
+(``use_rnn=False``), probed from the reference and pinned by tests/golden/state_dict_keys.json and
+state_dict_keys_norn.json.  The C library builds the same graph from the same key names (csrc/model.cu),
+so this file is the single Python-side description of names + shapes.
 """
 from collections import OrderedDict
 
@@ -26,8 +27,9 @@ def _bn(prefix, c, out):
     out[prefix + '.num_batches_tracked'] = ((), 'bn_count')
 
 
-def state_dict_spec():
-    """OrderedDict key -> (shape, kind) in the reference's own key order."""
+def state_dict_spec(use_rnn=True):
+    """OrderedDict key -> (shape, kind) in the reference's own key order; use_rnn=False: the MLP head of
+    model.py:234-243 (linear.0 = Linear(1024, 512), linear.3 = Linear(512, 12)) instead of bi_rnn + linear."""
     out = OrderedDict()
     enc = 'feature_extractor.encoder.'
     out[enc + 'conv1.1.weight'] = ((64, 3, 7, 7), 'enc_conv')       # wrapped by LR_PAD -> '.1'
@@ -54,6 +56,12 @@ def state_dict_spec():
             out[p + '0.1.bias'] = ((chans[j + 1],), 'ghc_bias')
             _bn(p + '1', chans[j + 1], out)
     c_last = sum(c * h for c, h in zip(encoder_channels(), (8, 4, 2, 1))) // OUT_SCALE   # 1024
+    if not use_rnn:
+        out['linear.0.weight'] = ((RNN_HIDDEN, c_last), 'mlp_weight')
+        out['linear.0.bias'] = ((RNN_HIDDEN,), 'mlp_bias')
+        out['linear.3.weight'] = ((3 * STEP_COLS, RNN_HIDDEN), 'head_weight')
+        out['linear.3.bias'] = ((3 * STEP_COLS,), 'head_bias')
+        return out
     for layer in range(2):
         for suffix in ('', '_reverse'):
             in_sz = c_last if layer == 0 else 2 * RNN_HIDDEN

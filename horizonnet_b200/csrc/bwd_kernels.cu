@@ -536,23 +536,25 @@ __device__ __forceinline__ float head_grad(const float* __restrict__ dbon, const
     return s == 0 ? dcor[(size_t)b * 1024 + t * 4 + k] : dbon[((size_t)b * 2 + (s - 1)) * 1024 + t * 4 + k];
 }
 
-// d rnn[t][b][j] = sum_o d[t][b][o] * W[o][j]
+// d rnn[t][b][j] = sum_o d[t][b][o] * W[o][j]      (K inputs per row: 1024 bi-LSTM head, 512 last MLP layer)
+template <int K>
 __global__ void head_bwd_input_kernel(const float* __restrict__ dbon, const float* __restrict__ dcor,
                                       const float* __restrict__ w, float* __restrict__ drnn, int T, int B) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t total = (size_t)T * B * 1024;
+    const size_t total = (size_t)T * B * K;
     if (i >= total) return;
-    const int j = (int)(i & 1023);
-    const int row = (int)(i >> 10);
+    const int j = (int)(i % K);
+    const int row = (int)(i / K);
     const int t = row / B, b = row - t * B;
     float acc = 0.f;
 #pragma unroll
-    for (int o = 0; o < 12; ++o) acc = fmaf(head_grad(dbon, dcor, t, b, o), __ldg(w + o * 1024 + j), acc);
+    for (int o = 0; o < 12; ++o) acc = fmaf(head_grad(dbon, dcor, t, b, o), __ldg(w + o * K + j), acc);
     drnn[i] = acc;
 }
 
-// dW[o][j] += sum_{t,b} d[t][b][o] * rnn[t][b][j];  db[o] += sum d   (grid: (4, 12, row splits), 256 threads = 256 j;
+// dW[o][j] += sum_{t,b} d[t][b][o] * rnn[t][b][j];  db[o] += sum d   (grid: (K / 256, 12, row splits), 256 threads = 256 j;
 // every block sums its rows in fp64 and adds the partial sum to the zeroed outputs)
+template <int K>
 __global__ void head_bwd_weight_kernel(const float* __restrict__ dbon, const float* __restrict__ dcor,
                                        const float* __restrict__ rnn, float* __restrict__ dw, float* __restrict__ db, int T,
                                        int B) {
@@ -564,11 +566,17 @@ __global__ void head_bwd_weight_kernel(const float* __restrict__ dbon, const flo
     for (int row = r0; row < r1; ++row) {
         const int t = row / B, b = row - t * B;
         const float d = head_grad(dbon, dcor, t, b, o);
-        acc += (double)d * (double)rnn[(size_t)row * 1024 + j];
+        acc += (double)d * (double)rnn[(size_t)row * K + j];
         accb += (double)d;
     }
-    atomicAdd(dw + o * 1024 + j, (float)acc);
+    atomicAdd(dw + o * K + j, (float)acc);
     if (j == 0) atomicAdd(db + o, (float)accb);
+}
+
+// dx[i] = 0 where the ReLU output y[i] was not positive (the gradient of relu at its input)
+__global__ void relu_bwd_inplace_kernel(float* __restrict__ dx, const float* __restrict__ y, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && !(y[i] > 0.f)) dx[i] = 0.f;
 }
 
 // out[c] = sum_r x[r][c]      (grid over column chunks of 256 x row splits; atomics)
@@ -1090,13 +1098,28 @@ int ghc_to_sequence_bwd(const float* dseq, const Act dghc[4], cudaStream_t st) {
     return 0;
 }
 
-int head_bwd(const float* dbon, const float* dcor, const float* rnn, const float* w, float* drnn, float* dw, float* db, int T,
-             int B, cudaStream_t st) {
-    head_bwd_input_kernel<<<blocks_for((size_t)T * B * 1024), 256, 0, st>>>(dbon, dcor, w, drnn, T, B);
+template <int K>
+static int head_bwd_k(const float* dbon, const float* dcor, const float* rnn, const float* w, float* drnn, float* dw, float* db,
+                      int T, int B, cudaStream_t st) {
+    head_bwd_input_kernel<K><<<blocks_for((size_t)T * B * K), 256, 0, st>>>(dbon, dcor, w, drnn, T, B);
     HN_LAUNCH_OK();
-    HN_CUDA_OK(cudaMemsetAsync(dw, 0, 12 * 1024 * sizeof(float), st));
+    HN_CUDA_OK(cudaMemsetAsync(dw, 0, 12 * K * sizeof(float), st));
     HN_CUDA_OK(cudaMemsetAsync(db, 0, 12 * sizeof(float), st));
-    head_bwd_weight_kernel<<<dim3(4, 12, 16), 256, 0, st>>>(dbon, dcor, rnn, dw, db, T, B);
+    head_bwd_weight_kernel<K><<<dim3(K / 256, 12, 16), 256, 0, st>>>(dbon, dcor, rnn, dw, db, T, B);
+    HN_LAUNCH_OK();
+    return 0;
+}
+
+int head_bwd(const float* dbon, const float* dcor, const float* rnn, const float* w, float* drnn, float* dw, float* db, int T,
+             int B, int K, cudaStream_t st) {
+    if (K == 1024) return head_bwd_k<1024>(dbon, dcor, rnn, w, drnn, dw, db, T, B, st);
+    if (K == 512) return head_bwd_k<512>(dbon, dcor, rnn, w, drnn, dw, db, T, B, st);
+    return fail("head_bwd: K must be 1024 or 512");
+}
+
+int relu_bwd_inplace(float* dx, const float* y, size_t n, cudaStream_t st) {
+    if (n == 0) return 0;
+    relu_bwd_inplace_kernel<<<blocks_for(n), 256, 0, st>>>(dx, y, n);
     HN_LAUNCH_OK();
     return 0;
 }

@@ -47,8 +47,10 @@ int bn_bwd(const Act& dy, const Act& y, const Act& z, const float* bn, bool trai
 
 int maxpool_bwd(const Act& x, const Act& dp, float* dx, cudaStream_t st);                      // dx accumulated (atomics)
 int ghc_to_sequence_bwd(const float* dseq, const Act dghc[4], cudaStream_t st);                // accumulated (atomics)
+// K = 1024 (bi-LSTM head) or 512 (last layer of the MLP head): rnn / drnn [T][B][K], w / dw [12][K]
 int head_bwd(const float* dbon, const float* dcor, const float* rnn, const float* w, float* drnn, float* dw, float* db, int T,
-             int B, cudaStream_t st);
+             int B, int K, cudaStream_t st);
+int relu_bwd_inplace(float* dx, const float* y, size_t n, cudaStream_t st);           // dx *= (y > 0)
 int col_sum(const float* x, size_t rows, int cols, float* out, cudaStream_t st);
 
 int lstm_gather(const float* hout, const float* xp, float* hprev, float* xpd, int T, int B, cudaStream_t st);

@@ -1,6 +1,7 @@
 // hn_model: weight registry (reference checkpoint layout, misc/utils.py:49-65), BN folding and
 // weight packing, activation workspace, and the forward schedule of HorizonNet('resnet50', rnn)
 // (reference model.py:254-281), plus the C ABI (include/horizonnet_b200.h).
+#include <algorithm>
 #include <cstring>
 #include <map>
 #include <memory>
@@ -77,6 +78,26 @@ __global__ void nhwc_to_nchw_kernel(const float* __restrict__ in, float* __restr
     out[i] = in[(((size_t)b * H + h) * (W + 2 * halo) + w + halo) * C + c];
 }
 
+// MLP head layer 1 epilogue: y = acc * 1 + linear.0.bias
+__global__ void bias_constants_kernel(const float* __restrict__ bias, float* __restrict__ scale, float* __restrict__ shift,
+                                      int C) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= C) return;
+    scale[i] = 1.f;
+    shift[i] = bias[i];
+}
+
+// rows [T][B][C] -> [B][T][C] (test hook: the MLP hidden layer in the reference's [B, W, C] layout)
+__global__ void rows_to_batch_major_kernel(const float* __restrict__ in, float* __restrict__ out, int T, int B, int C) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t total = (size_t)T * B * C;
+    if (i >= total) return;
+    const int c = (int)(i % C);
+    const int t = (int)((i / C) % T);
+    const int b = (int)(i / C / T);
+    out[i] = in[((size_t)t * B + b) * C + c];
+}
+
 // seq [T][B][1024] -> feature [B][1024][T]
 __global__ void seq_to_feature_kernel(const float* __restrict__ seq, float* __restrict__ out, int T, int B) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -141,6 +162,17 @@ void build_graph(hn_model* m) {
                 "reduce_height_module.ghc_lst." + std::to_string(s) + ".layer." + std::to_string(j) + ".layers.";
             m->ghc[s][j] = make_conv(m, p + "0.1.weight", p + "1", p + "0.1.bias", ch[j], ch[j + 1], 3, 2, 1, 1);
         }
+    }
+    if (!m->use_rnn) {
+        // model.py:234-243: Linear(1024, 512), ReLU, Dropout, Linear(512, 12)
+        m->add_slot("linear.0.weight", 512ll * 1024);
+        m->add_slot("linear.0.bias", 512);
+        m->add_slot("linear.3.weight", 12 * 512);
+        m->add_slot("linear.3.bias", 12);
+        ConvLayer& c = m->mlp1;
+        c.d.Cin = 1024; c.d.Cout = 512; c.d.kh = c.d.kw = 1; c.d.sh = c.d.sw = 1; c.d.ph = c.d.pw = 0; c.d.relu = 1;
+        c.wkey = "linear.0.weight"; c.biaskey = "linear.0.bias";
+        return;
     }
     for (int layer = 0; layer < 2; ++layer)
         for (int dir = 0; dir < 2; ++dir) {
@@ -248,13 +280,16 @@ int conv_bn(hn_model* m, const ConvLayer& c, const Act& in, const Act& out, cons
 extern "C" {
 
 const char* hn_last_error(void) { return g_err.c_str(); }
-int hn_abi_version(void) { return 3; }
+int hn_abi_version(void) { return 4; }
 const char* hn_build_digest(void) { return HN_BUILD_DIGEST; }
 long long hn_kernel_launches(void) { return g_launches.load(); }
 
-int hn_model_create(int device, int max_batch, hn_model** out) {
+int hn_model_create(int device, int max_batch, hn_model** out) { return hn_model_create_head(device, max_batch, 1, out); }
+
+int hn_model_create_head(int device, int max_batch, int use_rnn, hn_model** out) {
     HN_CHECK(out != nullptr, "hn_model_create: out is NULL");
     HN_CHECK(max_batch >= 1 && max_batch <= 1024, "hn_model_create: max_batch must be in 1..1024");
+    HN_CHECK(use_rnn == 0 || use_rnn == 1, "hn_model_create_head: use_rnn must be 0 or 1");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return fail("hn_model_create: no CUDA device -- libhorizonnet_b200 has no CPU path");
@@ -266,11 +301,22 @@ int hn_model_create(int device, int max_batch, hn_model** out) {
     std::unique_ptr<hn_model> m(new hn_model());
     m->device = device;
     m->max_batch = max_batch;
+    m->use_rnn = use_rnn;
     if (const char* e = getenv("HN_TC_STEM")) m->stem_tc_on = atoi(e);
     build_graph(m.get());
     for (auto& s : m->slots)
         if (!s.ignored && m->alloc_t(&s.dev, (size_t)s.numel)) return -1;
     const size_t B = (size_t)max_batch;
+    if (!use_rnn) {
+        // MLP head: no projections / recurrence buffers.  XP stays as scratch: stem weight packing at finalize and the
+        // plane merge of the "feature" test stage.
+        struct { float** p; size_t n; } head_bufs[] = {
+            {&m->XP, std::max((size_t)256 * B * 1024, (size_t)4096 * 1024)},
+            {&m->HID, 256 * B * 512}, {&m->HIDD, 256 * B * 512},
+        };
+        for (auto& b : head_bufs)
+            if (m->alloc_t(b.p, b.n)) return -1;
+    }
     struct { float** p; size_t n; } bufs[] = {
         {&m->S0, B * 256 * 514 * 64},   {&m->S1, B * 128 * 258 * 64},  {&m->X[0], B * 128 * 258 * 256},
         {&m->X[1], B * 128 * 258 * 256}, {&m->IDN, B * 128 * 258 * 256}, {&m->T1, B * 128 * 258 * 128},
@@ -278,7 +324,6 @@ int hn_model_create(int device, int max_batch, hn_model** out) {
         {&m->F[2], B * 32 * 66 * 1024}, {&m->F[3], B * 16 * 34 * 2048}, {&m->G[0], B * 64 * 258 * 128},
         {&m->G[1], B * 64 * 258 * 128}, {&m->GO[0], B * 8 * 258 * 32},  {&m->GO[1], B * 4 * 130 * 64},
         {&m->GO[2], B * 2 * 66 * 128},  {&m->GO[3], B * 1 * 34 * 256},  {&m->SEQ, 256 * B * 1024},
-        {&m->XP, (256 * B * 4096 > (size_t)4096 * 1024) ? 256 * B * 4096 : (size_t)4096 * 1024},       {&m->R1, 256 * B * 1024},       {&m->R2, 256 * B * 1024},       {&m->R1S, 256 * B * 1024},
         {&m->x_in, B * 3 * 512 * 1024}, {&m->bon_out, B * 2 * 1024},    {&m->cor_out, B * 1024},
         {&m->x_slot[1], B * 3 * 512 * 1024},
         {&m->bon_slot[1], B * 2 * 1024},  {&m->cor_slot[1], B * 1024},
@@ -286,7 +331,14 @@ int hn_model_create(int device, int max_batch, hn_model** out) {
     };
     for (auto& b : bufs)
         if (m->alloc_t(b.p, b.n)) return -1;
-    if (m->alloc(reinterpret_cast<void**>(&m->counters), lstm_scratch_bytes())) return -1;
+    if (use_rnn) {
+        struct { float** p; size_t n; } rnn_bufs[] = {
+            {&m->XP, (256 * B * 4096 > (size_t)4096 * 1024) ? 256 * B * 4096 : (size_t)4096 * 1024},       {&m->R1, 256 * B * 1024},       {&m->R2, 256 * B * 1024},       {&m->R1S, 256 * B * 1024},
+        };
+        for (auto& b : rnn_bufs)
+            if (m->alloc_t(b.p, b.n)) return -1;
+        if (m->alloc(reinterpret_cast<void**>(&m->counters), lstm_scratch_bytes())) return -1;
+    }
     if (m->alloc_t(&m->error_flag, 1)) return -1;
     if (m->alloc_t(&m->tta_ints, 128)) return -1;
     if (m->alloc_t(&m->trn_sums, 2 * 4096) || m->alloc_t(&m->trn_scale, 4096) || m->alloc_t(&m->trn_shift, 4096) ||
@@ -373,6 +425,26 @@ int hn_model_finalize(hn_model* m) {
     for (int s = 0; s < 4; ++s)
         for (int j = 0; j < 4; ++j)
             if (pack_conv(m, m->ghc[s][j], st)) return -1;
+    if (!m->use_rnn) {
+        // MLP layer 1: OIHW [512][1024] -> [K=1024][N=512], epilogue 1 * acc + linear.0.bias, ReLU in the kernel
+        ConvLayer& c = m->mlp1;
+        if (!c.w) {
+            if (m->alloc_t(&c.w, (size_t)512 * 1024) || m->alloc_t(&c.scale, 512) || m->alloc_t(&c.shift, 512)) return -1;
+            if (m->alloc_t(&c.wq, (size_t)2 * 512 * 1024) || m->alloc_t(&c.tc_scale, 3 * 512 + 1)) return -1;
+        }
+        pack_oihw_kernel<<<(512 * 1024 + 255) / 256, 256, 0, st>>>(m->T(c.wkey), c.w, 512, 1024, 1, 1);
+        HN_LAUNCH_OK();
+        bias_constants_kernel<<<2, 256, 0, st>>>(m->T(c.biaskey), c.scale, c.shift, 512);
+        HN_LAUNCH_OK();
+        if (pack_weight_tc(m->T(c.wkey), c.wq, c.scale, c.shift, c.tc_scale, c.tc_scale + 3 * 512, 512, 1024, 1, 1, st)) return -1;
+        c.d.w = c.w; c.d.scale = c.scale; c.d.shift = c.shift;
+        HN_CUDA_OK(cudaMemcpyAsync(m->head_w, m->T("linear.3.weight"), 12 * 512 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        HN_CUDA_OK(cudaMemcpyAsync(m->head_b, m->T("linear.3.bias"), 12 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        HN_CUDA_OK(cudaStreamSynchronize(st));
+        m->bn_stale = false;
+        m->finalized = true;
+        return 0;
+    }
     for (int layer = 0; layer < 2; ++layer) {
         ConvLayer& c = m->xproj[layer];
         if (!c.w) {
@@ -505,8 +577,29 @@ static int forward_sequence(hn_model* m, const Act gout[4], cudaStream_t st) {
     return ghc_to_sequence(gout, m->SEQ, st, m->use_tc != 0);
 }
 
+// (3') model.py:270-279 (use_rnn=False): per-column MLP over the rows of SEQ.  Layer 1 (1024 -> 512, bias, ReLU) is the
+// same GEMM-row convolution as the LSTM projections; dropout (train mode) on the hidden layer; layer 2 + the scatter.
+static int forward_mlp(hn_model* m, int B, float* bon, float* cor, cudaStream_t st, const TrainCtx* tr) {
+    const size_t nh = (size_t)256 * B * 512;
+    const Act a = mk(m->SEQ, 1, 1, 256 * B, 1024, 0);
+    const Act h = mk(m->HID, 1, 1, 256 * B, 512, 0);
+    if (run_conv(m, m->mlp1, a, h, nullptr, st, CLS_HEAD, true)) return -1;
+    const float* head_in = m->HID;
+    if (tr && tr->head_p > 0.0) {         // train mode: linear[2] = nn.Dropout(0.5) on the post-ReLU hidden layer
+        Scope sc(m, CLS_HEAD, 0.0, st);
+        HN_CUDA_OK(cudaMemcpyAsync(m->HIDD, m->HID, nh * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        if (tr->mask[1] ? multiply_inplace(m->HIDD, tr->mask[1], nh, st)
+                        : dropout_inplace(m->HIDD, nh, tr->head_p, tr->seed, 1, false, st))
+            return -1;
+        head_in = m->HIDD;
+    }
+    Scope sc(m, CLS_HEAD, 2.0 * 256 * B * 12 * 512, st);
+    return linear_head(head_in, m->head_w, m->head_b, bon, cor, 256, B, 512, st);
+}
+
 // (3) model.py:264-281: 2-layer bidirectional LSTM (eval: dropout = identity), linear head, reshape, split
 static int forward_rnn(hn_model* m, int B, float* bon, float* cor, cudaStream_t st, const TrainCtx* tr = nullptr) {
+    if (!m->use_rnn) return forward_mlp(m, B, bon, cor, st, tr);
     const float* lin = m->SEQ;
     float* louts[2] = {m->R1, m->R2};
     for (int layer = 0; layer < 2; ++layer) {
@@ -542,7 +635,7 @@ static int forward_rnn(hn_model* m, int B, float* bon, float* cor, cudaStream_t 
     }
     {
         Scope sc(m, CLS_HEAD, 2.0 * 256 * B * 12 * 1024, st);
-        if (linear_head(m->R2, m->head_w, m->head_b, bon, cor, 256, B, st)) return -1;
+        if (linear_head(m->R2, m->head_w, m->head_b, bon, cor, 256, B, 1024, st)) return -1;
     }
     return 0;
 }
@@ -611,6 +704,8 @@ int hn_model_forward_train(hn_model* m, const float* x, int B, int in_channels, 
              "hn_model_forward_train: bn_train / bn_factor need hn_model_num_bn() entries");
     HN_CHECK(rnn_dropout >= 0.0 && rnn_dropout < 1.0 && head_dropout >= 0.0 && head_dropout < 1.0,
              "hn_model_forward_train: dropout probabilities must be in [0, 1)");
+    HN_CHECK(m->use_rnn || (rnn_dropout == 0.0 && !rnn_mask),
+             "hn_model_forward_train: the MLP head (use_rnn = 0) has no LSTM: rnn_dropout must be 0 and rnn_mask NULL");
     HN_ON_DEVICE(m->device);
     cudaStream_t st = (cudaStream_t)stream;
     if (m->rnn_inflight) {
@@ -835,7 +930,16 @@ int hn_model_stage(hn_model* m, const char* stage, float* out, long long capacit
         dims[0] = B; dims[1] = 1024; dims[2] = 256; dims[3] = 0;
         return 0;
     }
+    if (s == "mlp_hidden") {      // post-ReLU, pre-dropout hidden layer -> [B][256][512] (reference linear[1], model.py:272)
+        if (m->use_rnn) return fail("hn_model_stage: 'mlp_hidden' exists only in the MLP-head model (use_rnn = 0)");
+        const size_t nh = (size_t)256 * B * 512;
+        rows_to_batch_major_kernel<<<(unsigned)((nh + 255) / 256), 256, 0, st>>>(m->HID, out, 256, B, 512);
+        HN_LAUNCH_OK();
+        dims[0] = B; dims[1] = 256; dims[2] = 512; dims[3] = 0;
+        return 0;
+    }
     if (s == "rnn_out") {
+        if (!m->use_rnn) return fail("hn_model_stage: 'rnn_out' does not exist in the MLP-head model (use_rnn = 0)");
         HN_CUDA_OK(cudaMemcpyAsync(out, m->R2, total * sizeof(float), cudaMemcpyDeviceToDevice, st));
         dims[0] = 256; dims[1] = B; dims[2] = 1024; dims[3] = 0;
         return 0;

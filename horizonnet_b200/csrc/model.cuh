@@ -14,7 +14,8 @@
 namespace hn {
 
 int ghc_to_sequence(const Act ghc[4], float* seq, cudaStream_t st, bool split);
-int linear_head(const float* rnn, const float* w, const float* bias, float* bon, float* cor, int T, int B,
+// K = 1024: the bi-LSTM head (rnn [T][B][1024]); K = 512: the last layer of the MLP head (hidden [T][B][512])
+int linear_head(const float* rnn, const float* w, const float* bias, float* bon, float* cor, int T, int B, int K,
                 cudaStream_t st);
 int lstm_layer(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, float* out, int T, int B,
                void* scratch, int* error_flag, cudaStream_t st);
@@ -98,8 +99,10 @@ struct hn_model {
     struct Block { ConvLayer c1, c2, c3, ds; bool has_ds = false; };
     std::vector<Block> blocks[4];
     ConvLayer ghc[4][4];
+    int use_rnn = 1;                                 // 0: per-column MLP head instead of the bi-LSTM (model.py:234-243)
     ConvLayer xproj[2];                              // LSTM input projections as 1x1 convs, N = 4096
-    float* head_w = nullptr;
+    ConvLayer mlp1;                                  // MLP head layer 1 (linear.0 + ReLU) as a 1x1 conv, N = 512
+    float* head_w = nullptr;                         // [12][1024] linear.weight, or [12][512] linear.3.weight
     float* head_b = nullptr;
     const float* whh[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};
     std::vector<std::string> bn_names;               // state_dict prefixes of the 69 BatchNorm2d modules, graph order
@@ -119,6 +122,7 @@ struct hn_model {
     float* G[2] = {nullptr, nullptr};
     float* GO[4] = {nullptr, nullptr, nullptr, nullptr};
     float *SEQ = nullptr, *XP = nullptr, *R1 = nullptr, *R2 = nullptr, *R1S = nullptr;
+    float *HID = nullptr, *HIDD = nullptr;           // MLP head: hidden layer [T][B][512] after ReLU, and after dropout
     unsigned int* counters = nullptr;
     int* error_flag = nullptr;
     float *x_in = nullptr, *bon_out = nullptr, *cor_out = nullptr;    // for forward_host

@@ -5,8 +5,9 @@
 //   (permute to [T=256, B, 1024]) in one pass.  Because (W+2)*f == 256+2f the interpolate scale is
 //   exactly 1/f, so out[col] = (1-l)*x[i0] + l*x[i0+1] with s = (col+0.5)/f + 0.5 in halo
 //   coordinates, i0 = floor(s), l = s - i0 (all exactly representable in fp32; f=1 is the identity).
-// head_kernel: model.py:266-269, Linear(1024 -> 12) + the [T,B,3,4] -> [B,3,T*4] scatter;
-//   channel 0 = cor, 1..2 = bon (model.py:278-279).
+// head_kernel<K>: model.py:266-269, Linear(K -> 12) + the [T,B,3,4] -> [B,3,T*4] scatter;
+//   channel 0 = cor, 1..2 = bon (model.py:278-279).  K = 1024: the bi-LSTM head; K = 512: the last layer of the
+//   per-column MLP head of use_rnn=False (model.py:238-243, :270-275), whose rows are the same t*B + b.
 #include "hn_common.cuh"
 #include "conv_tc.cuh"
 
@@ -54,30 +55,32 @@ __global__ void __launch_bounds__(256) ghc_to_sequence_kernel(const GhcSrc s, fl
     }
 }
 
-__global__ void __launch_bounds__(256) head_kernel(const float* __restrict__ rnn,   // [T][B][1024]
-                                                   const float* __restrict__ w,     // [12][1024]
+template <int K>
+__global__ void __launch_bounds__(256) head_kernel(const float* __restrict__ rnn,   // [T][B][K]
+                                                   const float* __restrict__ w,     // [12][K]
                                                    const float* __restrict__ bias,  // [12]
                                                    float* __restrict__ bon,         // [B][2][1024]
                                                    float* __restrict__ cor,         // [B][1][1024]
                                                    int T, int B) {
-    __shared__ __align__(16) float ws[12 * 1024];
-    for (int i = threadIdx.x; i < 12 * 1024 / 4; i += 256)
+    static_assert(K % 128 == 0, "one float4 per lane per 128 inputs");
+    __shared__ __align__(16) float ws[12 * K];
+    for (int i = threadIdx.x; i < 12 * K / 4; i += 256)
         reinterpret_cast<float4*>(ws)[i] = __ldg(reinterpret_cast<const float4*>(w) + i);
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int row = blockIdx.x * 8 + warp;           // row = t*B + b
     if (row >= T * B) return;
     const int t = row / B, b = row - t * B;
-    const float4* x = reinterpret_cast<const float4*>(rnn + (size_t)row * 1024);
+    const float4* x = reinterpret_cast<const float4*>(rnn + (size_t)row * K);
     float acc[12];
 #pragma unroll
     for (int o = 0; o < 12; ++o) acc[o] = 0.f;
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
+    for (int q = 0; q < K / 128; ++q) {
         const float4 xv = x[q * 32 + lane];
 #pragma unroll
         for (int o = 0; o < 12; ++o) {
-            const float4 wv = reinterpret_cast<const float4*>(ws + o * 1024)[q * 32 + lane];
+            const float4 wv = reinterpret_cast<const float4*>(ws + o * K)[q * 32 + lane];
             acc[o] = fmaf(xv.x, wv.x, acc[o]);
             acc[o] = fmaf(xv.y, wv.y, acc[o]);
             acc[o] = fmaf(xv.z, wv.z, acc[o]);
@@ -119,9 +122,11 @@ int ghc_to_sequence(const Act ghc[4], float* seq, cudaStream_t st, bool split) {
     return 0;
 }
 
-int linear_head(const float* rnn, const float* w, const float* bias, float* bon, float* cor, int T, int B,
+int linear_head(const float* rnn, const float* w, const float* bias, float* bon, float* cor, int T, int B, int K,
                 cudaStream_t st) {
-    head_kernel<<<(T * B + 7) / 8, 256, 0, st>>>(rnn, w, bias, bon, cor, T, B);
+    if (K == 1024) head_kernel<1024><<<(T * B + 7) / 8, 256, 0, st>>>(rnn, w, bias, bon, cor, T, B);
+    else if (K == 512) head_kernel<512><<<(T * B + 7) / 8, 256, 0, st>>>(rnn, w, bias, bon, cor, T, B);
+    else return fail("linear_head: K must be 1024 or 512");
     HN_LAUNCH_OK();
     return 0;
 }

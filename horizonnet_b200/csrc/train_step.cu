@@ -60,6 +60,7 @@ struct TrainState {
     float *seq = nullptr, *xp[2] = {nullptr, nullptr}, *r[2] = {nullptr, nullptr}, *rm[2] = {nullptr, nullptr};
     float *hprev = nullptr, *gates = nullptr, *cell = nullptr, *dgates = nullptr, *dc = nullptr;
     float *da = nullptr, *db = nullptr, *whh_t = nullptr;
+    float *mh = nullptr, *mhd = nullptr;          // MLP head: hidden layer [T][B][512] after ReLU, and after dropout
     unsigned int* barrier = nullptr;
     std::vector<Unit> units;
     Act stem_y, pool_y, gout[4];
@@ -217,6 +218,20 @@ int walk_forward(hn_model* m, TrainState* ts, const float* x, int B, int in_chan
 
     // ---- model.py:152-155, 175-178, 263: sequence; :264-266 bi-LSTM, dropouts, head
     if (ghc_to_sequence(ts->gout, ts->seq, st, false)) return -1;
+    if (!m->use_rnn) {
+        // model.py:270-275: MLP per row, layer 1 on the exact fp32 kernel; both hidden layers stay on the tape
+        const size_t nh = (size_t)T_STEPS * B * 512;
+        const Act a = mk(ts->seq, 1, 1, T_STEPS * B, 1024, 0);
+        const Act h = mk(ts->mh, 1, 1, T_STEPS * B, 512, 0);
+        if (conv_f32(m->mlp1.d, a, h, nullptr, st)) return -1;
+        HN_CUDA_OK(cudaMemcpyAsync(ts->mhd, ts->mh, nh * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        // hn_model_stage("mlp_hidden") shows the hidden layer of the last forward, this one included
+        HN_CUDA_OK(cudaMemcpyAsync(m->HID, ts->mh, nh * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        if (tr.head_p > 0.0 && (tr.mask[1] ? multiply_inplace(ts->mhd, tr.mask[1], nh, st)
+                                           : dropout_inplace(ts->mhd, nh, tr.head_p, tr.seed, 1, false, st)))
+            return -1;
+        return linear_head(ts->mhd, m->head_w, m->head_b, bon, cor, T_STEPS, B, 512, st);
+    }
     const size_t nseq = (size_t)T_STEPS * B * 1024;
     const float* lin = ts->seq;
     for (int layer = 0; layer < 2; ++layer) {
@@ -237,7 +252,7 @@ int walk_forward(hn_model* m, TrainState* ts, const float* x, int B, int in_chan
         }
         lin = ts->rm[layer];
     }
-    return linear_head(ts->rm[1], m->head_w, m->head_b, bon, cor, T_STEPS, B, st);
+    return linear_head(ts->rm[1], m->head_w, m->head_b, bon, cor, T_STEPS, B, 1024, st);
 }
 
 int ensure_buffers(hn_model* m, TrainState* ts, int B, const TrainCtx& tr) {
@@ -263,6 +278,13 @@ int ensure_buffers(hn_model* m, TrainState* ts, int B, const TrainCtx& tr) {
     if (ts->alloc_t(&ts->stem_in, (size_t)B * 512 * 1030 * 3)) return -1;
     const size_t rows = (size_t)T_STEPS * B;
     if (ts->alloc_t(&ts->seq, rows * 1024) || ts->alloc_t(&ts->da, rows * 1024) || ts->alloc_t(&ts->db, rows * 1024)) return -1;
+    if (!m->use_rnn) {
+        if (ts->alloc_t(&ts->mh, rows * 512) || ts->alloc_t(&ts->mhd, rows * 512)) return -1;
+        HN_CUDA_OK(cudaStreamSynchronize(0));
+        ts->B = B;
+        ts->sized = true;
+        return 0;
+    }
     for (int l = 0; l < 2; ++l)
         if (ts->alloc_t(&ts->xp[l], rows * 4096) || ts->alloc_t(&ts->r[l], rows * 1024) || ts->alloc_t(&ts->rm[l], rows * 1024))
             return -1;
@@ -337,18 +359,52 @@ int dgrad_tc(const ConvDesc& d, const float* w_oihw, const Act& dz, const Act& d
     return add_inplace(din.p, g.landing.p, din.numel(), st);
 }
 
-int walk_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dcor, cudaStream_t st) {
+#define GRAD(key) grad_buffer(m, ts, key)
+// MLP head (model.py:238-243, :270-275): from the scatter back to d(sequence), left in *dseq
+int mlp_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dcor, cudaStream_t st, float** dseq) {
+    const int B = ts->units.front().z.B;
+    const size_t rows = (size_t)T_STEPS * B;
+    const TrainCtx& tr = ts->ctx;
+    const size_t nh = rows * 512;
+    float* dh = ts->da;               // d(hidden), [rows][512]
+    if (head_bwd(dbon, dcor, ts->mhd, m->T("linear.3.weight"), dh, GRAD("linear.3.weight"), GRAD("linear.3.bias"), T_STEPS,
+                 B, 512, st))
+        return -1;
+    if (tr.head_p > 0.0 && (tr.mask[1] ? multiply_inplace(dh, tr.mask[1], nh, st)
+                                       : dropout_inplace(dh, nh, tr.head_p, tr.seed, 1, false, st)))
+        return -1;
+    if (relu_bwd_inplace(dh, ts->mh, nh, st)) return -1;
+    if (col_sum(dh, rows, 512, GRAD("linear.0.bias"), st)) return -1;
+    // dW1 = dH^T SEQ: the weight gradient of a 1x1 "convolution" over the T*B rows, like W_ih of the LSTM
+    const Act xa = mk(ts->seq, 1, 1, (int)rows, 1024, 0);
+    const Act dg = mk(dh, 1, 1, (int)rows, 512, 0);
+    ConvDesc wi; wi.Cin = 1024; wi.Cout = 512;
+    if (m->use_tc && wgrad_tc_on() && conv_wgrad_tc_supported(wi, xa, dg)) {
+        unsigned short* xpl = reinterpret_cast<unsigned short*>(ts->pl_scratch);
+        unsigned short* gpl = reinterpret_cast<unsigned short*>(ts->pl_scratch + rows * 1024);
+        float* gmax = ts->aux_tmp + 3 * 4096 + 1;
+        if (split_planes(ts->seq, xpl, rows * 1024, st) || split_planes_pow2(dh, gpl, nh, gmax, st)) return -1;
+        if (conv_wgrad_tc(wi, xa, xpl, dg, gpl, gmax, GRAD("linear.0.weight"), st)) return -1;
+    } else if (conv_wgrad_f32(wi, xa, dg, GRAD("linear.0.weight"), st)) return -1;
+    // d(sequence) = dH W1      (W1 [512][1024] is already conv_f32's [K][N] packing)
+    ConvDesc di; di.Cin = 512; di.Cout = 1024; di.w = m->T("linear.0.weight"); di.scale = ts->ones; di.shift = ts->zeros;
+    if (conv_f32(di, dg, mk(ts->db, 1, 1, (int)rows, 1024, 0), nullptr, st)) return -1;
+    *dseq = ts->db;
+    HN_CUDA_OK(cudaEventRecord(ts->ev[1], st));
+    HN_CUDA_OK(cudaEventRecord(ts->ev[2], st));          // no recurrence: the bi-LSTM phase is empty
+    return 0;
+}
+
+// linear head and bi-LSTM BPTT: from the scatter back to d(sequence), left in *dseq
+int rnn_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dcor, cudaStream_t st, float** dseq) {
     const int B = ts->units.front().z.B;
     const size_t rows = (size_t)T_STEPS * B, nseq = rows * 1024;
     const TrainCtx& tr = ts->ctx;
-    for (auto& e : ts->ev) if (!e) HN_CUDA_OK(cudaEventCreate(&e));
-    HN_CUDA_OK(cudaEventRecord(ts->ev[0], st));
-    HN_CUDA_OK(cudaMemsetAsync(ts->garena, 0, ts->ysize * sizeof(float), st));
-#define GRAD(key) grad_buffer(m, ts, key)
     // ---- linear head (model.py:266) and its dropout (:265)
     float* dout = ts->da;
     float* dnext = ts->db;
-    if (head_bwd(dbon, dcor, ts->rm[1], m->T("linear.weight"), dout, GRAD("linear.weight"), GRAD("linear.bias"), T_STEPS, B, st))
+    if (head_bwd(dbon, dcor, ts->rm[1], m->T("linear.weight"), dout, GRAD("linear.weight"), GRAD("linear.bias"), T_STEPS, B,
+                 1024, st))
         return -1;
     if (tr.head_p > 0.0 && (tr.mask[1] ? multiply_inplace(dout, tr.mask[1], nseq, st)
                                        : dropout_inplace(dout, nseq, tr.head_p, tr.seed, 1, false, st)))
@@ -412,6 +468,18 @@ int walk_backward(hn_model* m, TrainState* ts, const float* dbon, const float* d
         std::swap(dout, dnext);
     }
     HN_CUDA_OK(cudaEventRecord(ts->ev[2], st));
+    *dseq = dout;
+    return 0;
+}
+#undef GRAD
+
+int walk_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dcor, cudaStream_t st) {
+    for (auto& e : ts->ev) if (!e) HN_CUDA_OK(cudaEventCreate(&e));
+    HN_CUDA_OK(cudaEventRecord(ts->ev[0], st));
+    HN_CUDA_OK(cudaMemsetAsync(ts->garena, 0, ts->ysize * sizeof(float), st));
+#define GRAD(key) grad_buffer(m, ts, key)
+    float* dout = nullptr;
+    if (m->use_rnn ? rnn_backward(m, ts, dbon, dcor, st, &dout) : mlp_backward(m, ts, dbon, dcor, st, &dout)) return -1;
     // dout = d(sequence) -> the four height-reduction outputs (model.py:152-155, 175-178, 263)
     Act dg[4];
     for (int s = 0; s < 4; ++s) dg[s] = grad_of(ts, ts->gout[s]);
@@ -488,6 +556,8 @@ int hn_train_forward(hn_model* m, const float* x, int B, int in_channels, float*
     HN_CHECK(in_channels >= 3 && n_bn == (int)m->bn_names.size(), "hn_train_forward: bad in_channels / n_bn");
     HN_CHECK(rnn_dropout >= 0.0 && rnn_dropout < 1.0 && head_dropout >= 0.0 && head_dropout < 1.0,
              "hn_train_forward: dropout probabilities must be in [0, 1)");
+    HN_CHECK(m->use_rnn || (rnn_dropout == 0.0 && !rnn_mask),
+             "hn_train_forward: the MLP head (use_rnn = 0) has no LSTM: rnn_dropout must be 0 and rnn_mask NULL");
     HN_ON_DEVICE(m->device);
     cudaStream_t st = (cudaStream_t)stream;
     if (m->rnn_inflight) {
@@ -531,7 +601,7 @@ int hn_model_get_grad(hn_model* m, const char* key, float* out, long long numel,
 
 // Device time of the phases of the last hn_train_backward: ms[0] linear head, [1] bi-LSTM BPTT (both layers),
 // [2] sequence -> height-reduction outputs, [3] the 69 conv units (BN backward + weight gradient + data gradient).
-// Synchronises with the backward's stream.
+// MLP head: ms[0] is the whole MLP backward and ms[1] is 0.  Synchronises with the backward's stream.
 int hn_train_profile(hn_model* m, double ms[4]) {
     HN_CHECK(m && ms, "hn_train_profile: NULL argument");
     TrainState* ts = state_of(m);
@@ -541,7 +611,7 @@ int hn_train_profile(hn_model* m, double ms[4]) {
     for (int i = 0; i < 4; ++i) {
         float t = 0.f;
         HN_CUDA_OK(cudaEventElapsedTime(&t, ts->ev[i], ts->ev[i + 1]));
-        ms[i] = t;
+        ms[i] = (i == 1 && !m->use_rnn) ? 0.0 : t;          // the MLP head has no recurrence phase
     }
     return 0;
 }

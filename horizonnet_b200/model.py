@@ -2,12 +2,13 @@
 
 Boundary kept from the reference (SURVEY 8b):
   * ``HorizonNet(backbone, use_rnn)`` is an ``nn.Module`` whose parameters/buffers carry exactly
-    the reference's 448 ``state_dict`` keys, so ``misc/utils.py:49-65`` (``save_model`` /
-    ``load_trained_model``) work unchanged with this class;
+    the reference's 448 ``state_dict`` keys (434 with ``use_rnn=False``), so ``misc/utils.py:49-65``
+    (``save_model`` / ``load_trained_model``) work unchanged with this class;
   * ``forward(x[B, C>=3, 512, 1024]) -> (bon[B,2,1024], cor[B,1,1024])`` raw fp32 outputs,
     ``NotImplementedError`` for any other H x W (model.py:255-256);
   * ``.backbone``, ``.use_rnn``, ``.feature_extractor.list_blocks()``, ``.x_mean``, ``.x_std``.
-Only the path BASELINE.json names is built: ``backbone='resnet50'``, ``use_rnn=True``, inference
+Built: ``backbone='resnet50'`` with ``use_rnn=True`` (the path BASELINE.json names) or ``use_rnn=False`` (the
+per-column MLP head of model.py:234-243, what the reference's ``train.py --no_rnn`` trains), inference
 (eval) forward -- plus the train-mode FORWARD (batch-statistics BatchNorm with running-stat updates,
 LSTM / head dropout; train.py:52) and its backward (train.py:278 ``loss.backward()``): with autograd on,
 ``forward`` in train mode returns outputs whose grad_fn runs the library's backward pass and fills
@@ -138,9 +139,10 @@ class HorizonNet(nn.Module):
 
     def __init__(self, backbone, use_rnn):
         super().__init__()
-        if backbone != 'resnet50' or not use_rnn:
+        if backbone != 'resnet50':
             raise NotImplementedError(
-                "horizonnet_b200 implements the BASELINE path only: HorizonNet('resnet50', use_rnn=True)")
+                "horizonnet_b200 implements HorizonNet('resnet50', use_rnn=True) and HorizonNet('resnet50', use_rnn=False) "
+                f"only, not the {backbone!r} backbone")
         self.backbone = backbone
         self.use_rnn = use_rnn
         self.out_scale = 8
@@ -148,12 +150,18 @@ class HorizonNet(nn.Module):
         self.rnn_hidden_size = RNN_HIDDEN
         self.feature_extractor = _Encoder()
         self.reduce_height_module = _HeightStage((256, 512, 1024, 2048), self.out_scale)
-        self.bi_rnn = nn.LSTM(input_size=1024, hidden_size=RNN_HIDDEN, num_layers=2, dropout=0.5,
-                              batch_first=False, bidirectional=True)
-        self.drop_out = nn.Dropout(0.5)
-        self.linear = nn.Linear(2 * RNN_HIDDEN, 3 * STEP_COLS)
+        if use_rnn:
+            self.bi_rnn = nn.LSTM(input_size=1024, hidden_size=RNN_HIDDEN, num_layers=2, dropout=0.5,
+                                  batch_first=False, bidirectional=True)
+            self.drop_out = nn.Dropout(0.5)
+            self.linear = nn.Linear(2 * RNN_HIDDEN, 3 * STEP_COLS)
+            head = self.linear
+        else:                                                         # model.py:234-243
+            self.linear = nn.Sequential(nn.Linear(1024, RNN_HIDDEN), nn.ReLU(inplace=True), nn.Dropout(0.5),
+                                        nn.Linear(RNN_HIDDEN, 3 * STEP_COLS))
+            head = self.linear[-1]
         with torch.no_grad():
-            self.linear.bias.copy_(torch.tensor(HEAD_BIAS))          # model.py:231-233
+            head.bias.copy_(torch.tensor(HEAD_BIAS))                  # model.py:231-233, :241-243
         # bypass nn.Module.__setattr__: runtime state must not become sub-modules / parameters
         object.__setattr__(self, '_handles', {})
         object.__setattr__(self, '_lock', threading.Lock())
@@ -167,7 +175,7 @@ class HorizonNet(nn.Module):
     def _state_tensors(self):
         if self._slots is None:
             slots = []
-            spec = state_dict_spec()
+            spec = state_dict_spec(self.use_rnn)
             for key in spec:
                 *path, leaf = key.split('.')
                 mod = self
@@ -222,7 +230,8 @@ class HorizonNet(nn.Module):
             if h is None:
                 ptr = ctypes.c_void_p()
                 max_batch = max(batch, 1)
-                _lib.check(lib.hn_model_create(key, max_batch, ctypes.byref(ptr)), 'hn_model_create')
+                _lib.check(lib.hn_model_create_head(key, max_batch, 1 if self.use_rnn else 0, ctypes.byref(ptr)),
+                           'hn_model_create_head')
                 h = {'ptr': ptr, 'max_batch': max_batch, 'sig': None}
                 self._handles[key] = h
             sig = self._weight_signature()
@@ -252,11 +261,23 @@ class HorizonNet(nn.Module):
     # ---- train-mode forward (train.py:52 under net.train()) ---------------------------------------
     def _train_mode_active(self):
         """True if any module that behaves differently in training mode is in training mode: a BatchNorm2d (batch
-        statistics), the LSTM (inter-layer dropout) or the head dropout.  torch keeps the flag per module, and
-        train.py:251-256 (--freeze_earlier_blocks) really does mix them."""
-        if (self.bi_rnn.training and self.bi_rnn.dropout > 0) or (self.drop_out.training and self.drop_out.p > 0):
+        statistics), the LSTM (inter-layer dropout) or the head dropout (linear[2] of the MLP head).  torch keeps the
+        flag per module, and train.py:251-256 (--freeze_earlier_blocks) really does mix them."""
+        rnn_p, head_p = self._dropout_ps(active_only=True)
+        if rnn_p > 0 or head_p > 0:
             return True
         return any(m.training for m in self.modules() if isinstance(m, nn.BatchNorm2d))
+
+    def _head_dropout(self):
+        return self.drop_out if self.use_rnn else self.linear[2]
+
+    def _dropout_ps(self, active_only):
+        """(inter-layer LSTM dropout p, head dropout p); active_only: 0 for a module in eval mode.  The MLP head has no
+        LSTM, so its first entry is always 0."""
+        rnn_p = float(self.bi_rnn.dropout) if self.use_rnn and (self.bi_rnn.training or not active_only) else 0.0
+        d = self._head_dropout()
+        head_p = float(d.p) if (d.training or not active_only) else 0.0
+        return rnn_p, head_p
 
     def _bn_modules(self, h):
         if 'bn' not in h:
@@ -267,7 +288,7 @@ class HorizonNet(nn.Module):
 
     def _forward_train(self, x):
         """Batch-statistics BN (+ running-stat update written back into the module buffers, num_batches_tracked
-        incremented), LSTM inter-layer dropout and head dropout.  The dropout seed is drawn from torch's default
+        incremented), LSTM inter-layer dropout and head dropout (MLP head: the dropout of linear[2]).  The dropout seed is drawn from torch's default
         generator (reproducible under torch.manual_seed) and kept in ``last_dropout_seed``; the masks are this
         library's Philox stream, not torch's.
 
@@ -295,12 +316,13 @@ class HorizonNet(nn.Module):
                 factors[i] = float(m.momentum)
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())
         object.__setattr__(self, 'last_dropout_seed', seed)
-        rnn_p = float(self.bi_rnn.dropout) if self.bi_rnn.training else 0.0
-        head_p = float(self.drop_out.p) if self.drop_out.training else 0.0
+        rnn_p, head_p = self._dropout_ps(active_only=True)
         masks = [None, None]
         if getattr(self, 'dropout_masks_override', None) is not None:        # parity-test hook: torch-drawn masks
-            masks = [t.to(device=x.device, dtype=torch.float32).contiguous() for t in self.dropout_masks_override]
-            assert all(t.shape == (256, B, 2 * RNN_HIDDEN) for t in masks)
+            masks = [t.to(device=x.device, dtype=torch.float32).contiguous() if t is not None else None
+                     for t in self.dropout_masks_override]
+            shapes = [(256, B, 2 * RNN_HIDDEN)] * 2 if self.use_rnn else [None, (256, B, RNN_HIDDEN)]
+            assert all((t is None and s is None) or (t is not None and t.shape == s) for t, s in zip(masks, shapes))
         fn = lib.hn_train_forward if tape else lib.hn_model_forward_train
         _lib.check(fn(h['ptr'], x.data_ptr(), B, C, bon.data_ptr(), cor.data_ptr(), flags, factors, len(bns), seed, rnn_p,
                       head_p, masks[0].data_ptr() if masks[0] is not None else None,
@@ -377,11 +399,17 @@ class HorizonNet(nn.Module):
 
     def dropout_masks(self, seed, batch, device):
         """The two multiplicative masks ([256, batch, 1024], values 0 or 1/(1-p)) a train forward with this seed applies:
-        (between the LSTM layers, before the linear head).  Test hook."""
+        (between the LSTM layers, before the linear head).  MLP head: (None, [256, batch, 512]), the mask of linear[2] on
+        the hidden layer, rows t*batch + b.  Test hook."""
         out = []
         dev = torch.device(device)
-        for which, p in ((0, float(self.bi_rnn.dropout)), (1, float(self.drop_out.p))):
-            t = torch.empty(256, batch, 2 * RNN_HIDDEN, device=dev, dtype=torch.float32)
+        rnn_p, head_p = self._dropout_ps(active_only=False)
+        width = 2 * RNN_HIDDEN if self.use_rnn else RNN_HIDDEN
+        for which, p in ((0, rnn_p), (1, head_p)):
+            if which == 0 and not self.use_rnn:
+                out.append(None)
+                continue
+            t = torch.empty(256, batch, width, device=dev, dtype=torch.float32)
             with torch.cuda.device(dev):
                 _lib.check(_lib.lib().hn_dropout_mask(seed, which, p, t.data_ptr(), t.numel(),
                                                       torch.cuda.current_stream(dev).cuda_stream), 'hn_dropout_mask')

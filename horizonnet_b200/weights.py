@@ -1,4 +1,4 @@
-"""Deterministic synthetic checkpoints in the reference's 448-key layout.
+"""Deterministic synthetic checkpoints in the reference's 448-key layout (434 keys with the MLP head).
 
 There is no network on any box, so no trained checkpoint exists; parity tests, smoke() and
 bench.py all need *the same* random-init weights on the build container (where the real reference
@@ -18,10 +18,13 @@ import torch
 from ._spec import state_dict_spec, HEAD_BIAS
 
 
-def synthetic_state_dict(seed=0, bn='identity'):
+def synthetic_state_dict(seed=0, bn='identity', use_rnn=True):
+    """use_rnn=False: the MLP-head layout.  Its encoder and height-reduction tensors come first in the key order and are
+    drawn identically, so they equal the bi-LSTM model's for the same seed; then linear.0 ~ U(+-1/sqrt(1024)) (weight and
+    bias, PyTorch's nn.Linear default), linear.3.weight ~ U(+-1/sqrt(512)), linear.3.bias = the reference's init."""
     rs = np.random.RandomState(seed)
     sd = OrderedDict()
-    for key, (shape, kind) in state_dict_spec().items():
+    for key, (shape, kind) in state_dict_spec(use_rnn).items():
         if kind == 'enc_conv':
             co, ci, kh, kw = shape
             a = rs.standard_normal(shape) * math.sqrt(2.0 / (co * kh * kw))
@@ -36,6 +39,12 @@ def synthetic_state_dict(seed=0, bn='identity'):
             a = rs.uniform(-bound, bound, shape)
         elif kind == 'rnn':
             bound = 1.0 / math.sqrt(512)
+            a = rs.uniform(-bound, bound, shape)
+        elif kind == 'mlp_weight':
+            bound = 1.0 / math.sqrt(shape[1])
+            a = rs.uniform(-bound, bound, shape)
+        elif kind == 'mlp_bias':
+            bound = 1.0 / math.sqrt(sd[key[:-len('bias')] + 'weight'].shape[1])
             a = rs.uniform(-bound, bound, shape)
         elif kind == 'head_weight':
             bound = 1.0 / math.sqrt(shape[1])

@@ -33,14 +33,19 @@ const char* hn_build_digest(void);
 /* Number of kernels this library has launched in this process (bench.py "gpu_launches"). */
 long long hn_kernel_launches(void);
 
-/* ---- model.HorizonNet (reference model.py:185-281), resnet50 + bi-LSTM head only ------------- */
+/* ---- model.HorizonNet (reference model.py:185-281), resnet50 with the bi-LSTM or the MLP head ---- */
 
-/* Creates the model on CUDA device `device`, with activation workspace for up to `max_batch`
- * panoramas per forward.  Replaces HorizonNet.__init__ (model.py:189-246) minus the ImageNet
- * download. */
+/* Creates HorizonNet('resnet50', use_rnn=True) on CUDA device `device`, with activation workspace for up to
+ * `max_batch` panoramas per forward.  Replaces HorizonNet.__init__ (model.py:189-246) minus the ImageNet
+ * download.  Same as hn_model_create_head(device, max_batch, 1, out). */
 int hn_model_create(int device, int max_batch, hn_model** out);
+/* use_rnn = 1: the 2-layer bi-LSTM + Linear(1024, 12) head (model.py:222-233); use_rnn = 0: the per-column MLP head
+ * Linear(1024, 512), ReLU, Dropout(0.5), Linear(512, 12) (model.py:234-243, what train.py --no_rnn builds), which has
+ * 434 state_dict keys: linear.0.* and linear.3.* instead of bi_rnn.* and linear.*.  Every entry point below takes
+ * either model. */
+int hn_model_create_head(int device, int max_batch, int use_rnn, hn_model** out);
 
-/* Number of tensors of the reference checkpoint layout (448, misc/utils.py:49-58) and the i-th key
+/* Number of tensors of the reference checkpoint layout (448, or 434 with the MLP head; misc/utils.py:49-58) and the i-th key
  * with its element count; lets a binding iterate the state_dict without knowing the topology. */
 int hn_model_num_tensors(const hn_model* m);
 int hn_model_tensor_info(const hn_model* m, int index, const char** key, long long* numel);
@@ -74,8 +79,8 @@ int hn_model_forward_async(hn_model* m, const float* x_nchw_dev, int batch, int 
 int hn_model_flush(hn_model* m, void* stream);
 
 /* TRAIN-mode forward: what `net(x)` computes under `net.train()` (reference train.py:52 inside feed_forward,
- * model.py:254-281 with every nn.BatchNorm2d in training mode and both dropouts active) -- the first step of the
- * "next" row f1; the backward pass is NOT built.
+ * model.py:254-281 with every nn.BatchNorm2d in training mode and the dropouts active); the backward pass is
+ * hn_train_forward / hn_train_backward below.
  *   - BatchNorm2d i (i < hn_model_num_bn(m), state_dict prefix hn_model_bn_name(m, i)): bn_train[i] = 1 normalises
  *     with the batch mean / biased variance of the raw conv output and moves running_mean / running_var (the device
  *     copies inside the model, read them back with hn_model_get_tensor) by bn_factor[i] (= the module's momentum, or
@@ -86,6 +91,10 @@ int hn_model_flush(hn_model* m, void* stream);
  *     hn_dropout_mask writes the factors (0 or 1/(1-p)) the forward multiplies with, which = 0 inter-layer
  *     [256][batch][1024], 1 head [256][batch][1024].  torch's own generator stream is not reproduced; for parity
  *     against a torch run, rnn_mask_dev / head_mask_dev (same shapes, or NULL) replace the Philox masks.
+ *   - MLP head (hn_model_create_head with use_rnn = 0): rnn_dropout must be 0 and rnn_mask_dev NULL; head_dropout is
+ *     the p of linear[2] (model.py:240), which acts on the post-ReLU hidden layer: which = 1 over 256*batch*512
+ *     elements, head_mask_dev [256][batch][512] (row t*batch + b, the library's order; the reference's own mask is
+ *     [batch][256][512]).
  * Each convolution runs twice (statistics pass + real pass); eval-mode entry points called afterwards fold the moved
  * running statistics again on their own. */
 int hn_model_num_bn(const hn_model* m);
@@ -114,7 +123,8 @@ int hn_train_forward(hn_model* m, const float* x_nchw_dev, int batch, int in_cha
                      void* stream);
 int hn_train_backward(hn_model* m, const float* dbon_dev, const float* dcor_dev, void* stream);
 int hn_model_get_grad(hn_model* m, const char* key, float* out_dev, long long numel, void* stream);
-/* Device time (ms) of the phases of the last hn_train_backward: head, bi-LSTM BPTT, sequence adjoint, the 69 conv units. */
+/* Device time (ms) of the phases of the last hn_train_backward: head, bi-LSTM BPTT, sequence adjoint, the 69 conv units.
+ * With the MLP head, ms[0] is the whole MLP backward and ms[1] is 0. */
 int hn_train_profile(hn_model* m, double ms[4]);
 /* HN_TRAIN_PROF=1 during the last hn_train_backward: the conv-unit phase split into ms[0] BatchNorm backward, ms[1] weight
  * gradients, ms[2] data gradients (device ms, summed over the units); -1 when that backward was not profiled. */
@@ -151,8 +161,9 @@ int hn_model_infer_tta(hn_model* m, const float* x_dev, int in_channels, int fli
 /* Test hook: copies an intermediate result of the LAST forward, converted to the reference's
  * layout, into `out_dev` (fp32).  Stages: "stem" (conv1+bn1+relu, NCHW [B,64,256,512], model.py:73-75),
  * "layer1".."layer4" (NCHW [B,C,H,W], model.py:78-81),
- * "feature" ([B,1024,256], model.py:175-178), "rnn_out" ([256,B,1024], model.py:264).
- * dims receives the 4 (or 3, last = 0) extents. */
+ * "feature" ([B,1024,256], model.py:175-178), "rnn_out" ([256,B,1024], model.py:264; bi-LSTM model only),
+ * "mlp_hidden" ([B,256,512], the post-ReLU, pre-dropout hidden layer = output of linear[1], model.py:272; MLP model
+ * only).  dims receives the 4 (or 3, last = 0) extents. */
 int hn_model_stage(hn_model* m, const char* stage, float* out_dev, long long capacity, int dims[4],
                    void* stream);
 
@@ -166,7 +177,7 @@ int hn_model_set_option(hn_model* m, const char* name, int value);
 /* With option "profile" = 1 every forward records CUDA-event pairs (on the forward's stream)
  * around each launch; this call waits for them and returns, per op class
  * {0 stem, 1 maxpool, 2 encoder convs, 3 height-reduction convs, 4 upsample/concat tail,
- *  5 LSTM input-projection GEMMs, 6 LSTM recurrence, 7 linear head},
+ *  5 LSTM input-projection GEMMs, 6 LSTM recurrence, 7 linear head (with the MLP head: both of its layers, 5 and 6 stay 0)},
  * the accumulated device milliseconds, algorithmic FLOPs and launch counts (arrays of 8). */
 int hn_model_profile_read(hn_model* m, double* ms, double* flops, long long* launches, int reset);
 
