@@ -1150,20 +1150,18 @@ int lstm_bwd_steps(const float* dout, const float* gates, const float* cell, con
     LstmBwdArgs a;
     a.dout = dout; a.gates = gates; a.cell = cell; a.whh_t[0] = whh_t_f; a.whh_t[1] = whh_t_b; a.dgates = dgates; a.dc = dc;
     a.T = T; a.B = B; a.step = 0;
-    static const bool persistent_on = [] { const char* e = getenv("HN_LSTM_BWD_PERSISTENT"); return !(e && atoi(e) == 0); }();
     int dev = 0, coop = 0, sms = 0, per_sm = 0;
     HN_CUDA_OK(cudaGetDevice(&dev));
     HN_CUDA_OK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
     HN_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    static const bool staged_on = [] { const char* e = getenv("HN_LSTM_BWD_STAGED"); return !(e && atoi(e) == 0); }();
-    const bool staged = staged_on && B <= 16;
+    const bool staged = B <= 16;
     const size_t smem = staged ? (size_t)B * 2048 * sizeof(float) : 0;
     void* kernel = staged ? reinterpret_cast<void*>(lstm_bwd_persistent_kernel<true>)
                           : reinterpret_cast<void*>(lstm_bwd_persistent_kernel<false>);
     if (staged) HN_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     HN_CUDA_OK(staged ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm_bwd_persistent_kernel<true>, 256, smem)
                       : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm_bwd_persistent_kernel<false>, 256, 0));
-    if (persistent_on && barrier && error_flag && coop && per_sm * sms >= 128) {
+    if (barrier && error_flag && coop && per_sm * sms >= 128) {
         // one cooperative launch for the whole sequence (128 co-resident CTAs, grid barrier between the steps)
         HN_CUDA_OK(cudaMemsetAsync(barrier, 0, sizeof(unsigned int), st));
         void* args[] = {&a, &barrier, &error_flag};

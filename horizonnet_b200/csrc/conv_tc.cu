@@ -28,7 +28,7 @@
 //   warps 4-7, 8-11   two consumer warpgroups; warpgroup g owns tile rows [64g, 64g + 64) x all BN columns: per chunk
 //              12 wgmma m64nBNk16 (3 products x 4 K-steps of 16, one wgmma group; the group of the previous chunk stays in
 //              flight until this one is issued) into a register accumulator that is restarted every
-//              `seg` chunks and added into a second register sum with round-to-nearest fp32 adds (bounds whatever
+//              SEG chunks and added into a second register sum with round-to-nearest fp32 adds (bounds whatever
 //              rounding the tensor-core accumulation applies over K up to 18432); then the epilogue in the slot:
 //              folded BN scale/shift, + the residual the slot holds, ReLU, re-split into hi/lo planes (or fp32) written
 //              in place, the circular halo columns stored directly.  The consumers go straight on to the next tile.
@@ -54,6 +54,9 @@ constexpr int BKC = 64;            // fp16 channels per K chunk = one 128-byte s
 constexpr int STAGES = 3;
 constexpr int CONS_WARP0 = 4;      // first consumer warp
 constexpr int CONS_WARPS = 8;
+// K chunks accumulated by the tensor cores before the sum is promoted to the fp32 register sum, in every kernel of this
+// file; one constant keeps bott_tc_kernel's conv2 bit-identical to conv_tc_kernel<64>
+constexpr int SEG = 4;
 
 struct TcArgs {
     int mode;                 // 0: GEMM rows (1x1 stride-1 conv over all halo-NHWC pixels, or plain GEMM); 1: conv rows
@@ -72,11 +75,8 @@ struct TcArgs {
     float* out_f32;           // fp32 output instead of planes (LSTM projections)
     size_t out_plane;         // elements per plane
     int relu;
-    int seg;                  // K chunks per accumulation segment
     int dxr;                  // 1: 3x3 single-row tiles load each (dy, channel chunk) input row ONCE (130 pixels) and the three
                               //    dx taps read it through row-shifted descriptors (L2->SM traffic per tap: 64 -> 43 KB)
-    int rowbox;               // 1: the rows_per_tile output rows of a tile come from consecutive input rows of one image -> one TMA box
-    int dbg;                  // HN_TC_DBG experiment bits: 1 skip residual reads, 2 skip output stores
     int pf;                   // gemm_tc_kernel: L2 prefetch distance (in tiles) of the residual / activation boxes, 0 = off
 };
 
@@ -260,8 +260,7 @@ __device__ __forceinline__ void tile_rows(const TcArgs& a, int mt, int& R0, int&
 }
 
 // Residual load (`bar` counts the bytes) or output store of part k of tile (mt, nt) through tensor map tm (conv_tc_map):
-// mode 0 one box {cw, 128 rows}; mode 1 one box of all rows when `rowbox` makes them consecutive, else one box per
-// output row that exists
+// mode 0 one box {cw, 128 rows}; mode 1 one box of all the tile's rows
 template <int BN, bool STORE>
 __device__ __forceinline__ void tile_boxes(const TcArgs& a, const EpiLayout<BN>& L, const CUtensorMap* tm, uint8_t* x,
                                            uint8_t* y, uint64_t* bar, int mt, int nt, int k) {
@@ -274,13 +273,9 @@ __device__ __forceinline__ void tile_boxes(const TcArgs& a, const EpiLayout<BN>&
     }
     int R0, valid_rows, wo0;
     tile_rows(a, mt, R0, valid_rows, wo0);
-    const int nbox = a.rowbox ? 1 : valid_rows;
-    for (int rr = 0; rr < nbox; ++rr) {
-        const int R = R0 + rr, b = R / a.Ho, ho = R - b * a.Ho;
-        uint8_t* d = dst + rr * a.tw * L.row_bytes;
-        if (STORE) tma_store_5d(tm, d, c0, wo0 + a.out_halo, ho, b, plane);
-        else tma_load_5d(d, tm, bar, c0, wo0 + a.out_halo, ho, b, plane);
-    }
+    const int b = R0 / a.Ho, ho = R0 - b * a.Ho;
+    if (STORE) tma_store_5d(tm, dst, c0, wo0 + a.out_halo, ho, b, plane);
+    else tma_load_5d(dst, tm, bar, c0, wo0 + a.out_halo, ho, b, plane);
 }
 
 template <int BN>
@@ -310,7 +305,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     static_assert(BX_OFF + NST * BX_SLOT <= NST * S::STAGE, "dxr layout does not fit the operand ring");
     static_assert(BX_SLOT == HALF_TILE, "a dxr weight slot holds half an output tile");
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool has_res = a.res != nullptr && !(a.dbg & 1);
+    const bool has_res = a.res != nullptr;
     // Ring sequence per tile: the tile's K chunks, then its epilogue slot -- one ring stage, which holds exactly one output
     // tile, or in dxr mode two consecutive weight slots, each holding half of one (x: first half, y: second half).
     // The producer fills the slot with the residual tile, the consumers turn it into the output tile in place, the store
@@ -373,38 +368,30 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         }
                     }
                 } else {
-                    // a row box always delivers the full tile (rows past the end are out-of-bounds zero fill, full byte count)
-                    const uint32_t a_bytes = (a.mode == 0) ? 2u * S::A_PLANE
-                                                           : (uint32_t)(2 * (a.rowbox ? a.rows_per_tile : valid_rows) * a.tw * BKC * 2);
                     for (int kc = 0; kc < a.num_kc; ++kc) {
                         mbar_wait(empty_bar + stage, phase ^ 1);
                         uint8_t* sA = smem + stage * S::STAGE;
                         uint8_t* sB = sA + 2 * S::A_PLANE;
                         const int tap = kc / a.kc_per_tap;
                         const int c0 = (kc - tap * a.kc_per_tap) * BKC;
-                        mbar_expect_tx(full_bar + stage, a_bytes + 2u * S::B_PLANE);
+                        // one box per plane always delivers the full tile (rows past the end are out-of-bounds zero fill)
+                        mbar_expect_tx(full_bar + stage, 2u * S::A_PLANE + 2u * S::B_PLANE);
                         if (a.mode == 0) {
                             tma_load_3d(sA, &tmA, full_bar + stage, c0, mt * BM, 0);
                             tma_load_3d(sA + S::A_PLANE, &tmA, full_bar + stage, c0, mt * BM, 1);
                         } else {
+                            // the tile's output rows are consecutive rows of one image, or whole images (conv_tc_plan)
                             const int dy = tap / a.kw, dx = tap - dy * a.kw;
-                            // rowbox: the tile's output rows map to consecutive input rows of one image: one box per plane
-                            const int nbox = a.rowbox ? 1 : valid_rows;
-                            for (int rr = 0; rr < nbox; ++rr) {
-                                const int R = row0 + rr;
-                                const int b = R / a.Ho, ho = R - b * a.Ho;
-                                const int hin = ho * a.sh + dy - a.ph;
-                                uint8_t* dst = sA + rr * a.tw * (BKC * 2);
-                                if (a.parity) {
-                                    const int p = dx + a.woff;
-                                    tma_load_5d(dst, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin, b);
-                                    tma_load_5d(dst + S::A_PLANE, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin,
-                                                a.Bimg + b);
-                                } else {
-                                    tma_load_4d(dst, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin, b);
-                                    tma_load_4d(dst + S::A_PLANE, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin,
-                                                a.Bimg + b);
-                                }
+                            const int b = row0 / a.Ho, ho = row0 - b * a.Ho;
+                            const int hin = ho * a.sh + dy - a.ph;
+                            if (a.parity) {
+                                const int p = dx + a.woff;
+                                tma_load_5d(sA, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin, b);
+                                tma_load_5d(sA + S::A_PLANE, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin,
+                                            a.Bimg + b);
+                            } else {
+                                tma_load_4d(sA, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin, b);
+                                tma_load_4d(sA + S::A_PLANE, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin, a.Bimg + b);
                             }
                         }
                         tma_load_3d(sB, &tmB, full_bar + stage, kc * BKC, nt * BN, 0);
@@ -421,9 +408,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
                 if (has_res) {
                     const EpiLayout<BN> L(false);
-                    // boxes per output row move only the rows that exist; a box past the end delivers its full size
-                    const int rows = (a.mode == 0 || a.rowbox) ? BM : valid_rows * a.tw;
-                    mbar_expect_tx(full_bar + st0, (uint32_t)(rows * BN * 4));
+                    mbar_expect_tx(full_bar + st0, (uint32_t)(BM * BN * 4));
                     for (int k = 0; k < L.npart; ++k)
                         tile_boxes<BN, false>(a, L, &tmR, slot_x(st0), slot_y(st0), full_bar + st0, mt, nt, k);
                 }
@@ -446,7 +431,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             // stage `st`.  One wgmma group stays in flight across chunks; `drain` (and the end of a segment) waits for all
             auto step = [&](uint32_t sA, uint32_t a_plane, uint32_t sB, int st, bool last, bool drain) {
                 chunk_issue(acc, sA + a_row_off, sA + a_plane + a_row_off, sB, sB + S::B_PLANE, seg_pos == 0);
-                const bool seg_end = (++seg_pos == a.seg || last);
+                const bool seg_end = (++seg_pos == SEG || last);
                 if (seg_end || drain) {
                     wgmma_wait0();
                     reg_fence(acc);
@@ -492,7 +477,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
             // ---- epilogue in the slot
             HaloStore halo = {a.out_f32 ? static_cast<void*>(a.out_f32) : a.out, a.out_plane, a.Cout, 0, {-1, -1}};
-            if (a.mode == 1 && a.out_halo && !(a.dbg & 2)) {
+            if (a.mode == 1 && a.out_halo) {
                 int R0, rows, wo0;
                 tile_rows(a, mt, R0, rows, wo0);
 #pragma unroll
@@ -545,13 +530,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 stage = (stage + a.num_kc) % NST;
                 mbar_wait(oready_bar + stage, (ophase >> stage) & 1);
                 ophase ^= 1u << stage;
-                if (!(a.dbg & 2)) {
-                    const EpiLayout<BN> L(a.out_f32 != nullptr);
-                    for (int k = 0; k < L.npart; ++k)
-                        tile_boxes<BN, true>(a, L, &tmO, slot_x(stage), slot_y(stage), nullptr, mt, nt, k);
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                }
+                const EpiLayout<BN> L(a.out_f32 != nullptr);
+                for (int k = 0; k < L.npart; ++k)
+                    tile_boxes<BN, true>(a, L, &tmO, slot_x(stage), slot_y(stage), nullptr, mt, nt, k);
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
                 for (int e = 0; e < epi_stages; ++e) {
                     mbar_arrive_cnt(empty_bar + stage, CONS_WARPS);
                     if (++stage == NST) stage = 0;
@@ -690,7 +673,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 chunk_mma(acc, sA + a_row_off, sA + S::A_PLANE + a_row_off, sB, sB + S::B_PLANE, seg_pos == 0);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(empty_bar + stage);
-                if (++seg_pos == a.seg || kc == a.num_kc - 1) {
+                if (++seg_pos == SEG || kc == a.num_kc - 1) {
 #pragma unroll
                     for (int j = 0; j < GBN / 2; ++j) sum[j] += acc[j];
                     seg_pos = 0;
@@ -974,7 +957,6 @@ struct BottArgs {
     int num_tiles;
     int n3;                              // conv3 n-tiles of 64 channels (Cout3 / 64)
     int C3;                              // conv3 output channels
-    int seg;
     const float* scale2; const float* shift2;     // conv2: accumulator -> plane units, shift in plane units
     const float* scale3; const float* shift3;     // conv3
     unsigned short* out; size_t out_plane;        // output planes (halo-column stores)
@@ -1141,7 +1123,7 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     chunk_mma(acc, sAx + dx * 128 + a_row_off, sAx + S::AX_PLANE + dx * 128 + a_row_off, sB, sB + S::B_PLANE,
                               seg_pos == 0);
                     release_b();
-                    if (++seg_pos == a.seg || kc == 8) {
+                    if (++seg_pos == SEG || kc == 8) {
 #pragma unroll
                         for (int j = 0; j < 32; ++j) sum[j] += acc[j];
                         seg_pos = 0;
@@ -1197,23 +1179,6 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 }
 
 // -------------------------------------------------------------------------------- host side
-int tc_segment_chunks() {
-    // K chunks (of 64) accumulated by the tensor cores before the sum is promoted to the fp32 register sum; HN_TC_SEG
-    // overrides (tuning)
-    static int seg = [] {
-        const char* e = getenv("HN_TC_SEG");
-        int v = e ? atoi(e) : 4;
-        return v < 1 ? 1 : v;
-    }();
-    return seg;
-}
-
-bool tc_prefetch_on() {
-    // gemm_tc_kernel prefetches the activation / residual boxes of its K = 64 layers into L2 two tile rounds ahead; HN_TC_PF=0 disables
-    static const bool on = [] { const char* e = getenv("HN_TC_PF"); return !(e && atoi(e) == 0); }();
-    return on;
-}
-
 template <int BN>
 int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO, const TcArgs& a,
            int grid, cudaStream_t st) {
@@ -1228,7 +1193,7 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tm
 // Tensor map of an output-geometry tensor (output or residual) as the epilogue of a tile with BN channels moves it (see
 // EpiLayout): planes (hi, lo: an outer dimension of 2) or fp32 (an outer dimension of 1).  Mode 0 {Cout, M pixels,
 // plane}, box {cw, 128}; mode 1 {Cout, Wop, Ho, B, plane} -- the plane has its own dimension, so a box clipped past the
-// last image never spills into the lo plane -- box {cw, tw, box rows, box images} with `rowbox`, else {cw, tw, 1, 1}.
+// last image never spills into the lo plane -- box {cw, tw, box rows, box images}.
 int conv_tc_map(CUtensorMap* tm, const void* base, const TcPlan& pl, const Act& out, int Cout, bool f32) {
     const cuuint64_t es = f32 ? 4 : 2, C = (cuuint64_t)Cout, plane_bytes = (cuuint64_t)out.numel() * es;
     const cuuint32_t cw = f32 ? 32u : (pl.BN < 64 ? (cuuint32_t)pl.BN : 64u);
@@ -1244,7 +1209,7 @@ int conv_tc_map(CUtensorMap* tm, const void* base, const TcPlan& pl, const Act& 
     const cuuint64_t Wop = out.Wp();
     cuuint64_t dims[5] = {C, Wop, (cuuint64_t)out.H, (cuuint64_t)out.B, planes};
     cuuint64_t str[4] = {C * es, C * es * Wop, C * es * Wop * out.H, plane_bytes};
-    cuuint32_t box[5] = {cw, (cuuint32_t)pl.tw, pl.rowbox ? (cuuint32_t)pl.box_rows : 1u, pl.rowbox ? (cuuint32_t)pl.box_imgs : 1u, 1};
+    cuuint32_t box[5] = {cw, (cuuint32_t)pl.tw, (cuuint32_t)pl.box_rows, (cuuint32_t)pl.box_imgs, 1};
     return make_map(tm, base, 5, dims, str, box, -1, 1, dt, sw);
 }
 
@@ -1261,7 +1226,11 @@ bool conv_tc_supported(const ConvDesc& d, const Act& in, const Act& out) {
     if (d.sw == 2 && (in.Wp() % 2) != 0) return false;
     const int tw = out.W < 128 ? out.W : 128;
     if (tw < 8 || (tw & (tw - 1)) != 0 || out.W % tw != 0) return false;       // 8-row swizzle atoms, exact W tiling
-    return true;
+    // one TMA box per plane loads a tile: its BM / tw output rows are consecutive rows of one image or whole images, and
+    // their input rows are 1 or 2 apart (a traversal stride along H)
+    const int rows_per_tile = BM / tw;
+    if (d.sh != 1 && d.sh != 2) return false;
+    return out.H % rows_per_tile == 0 || rows_per_tile % out.H == 0;
 }
 
 int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32, bool has_residual, int sms, TcPlan* p) {
@@ -1277,10 +1246,10 @@ int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32,
         if (BN == 128 && tiles128 < 110) BN = 64;
     }
     p->num_kc = d.kh * d.kw * (d.Cin / BKC);
-    p->seg = tc_segment_chunks();
+    p->seg = SEG;
     p->box_rows = p->box_imgs = 1;
     long long m_tiles;
-    // asynchronous-epilogue GEMM kernel: plane output, K <= 512, Cout a multiple of 64
+    // asynchronous-epilogue GEMM kernel: plane output, Cin <= 256, Cout a multiple of 64
     static const bool gemm_kernel_on = [] { const char* e = getenv("HN_TC_GEMM"); return !(e && atoi(e) == 0); }();
     if (gemm && gemm_kernel_on && !out_f32 && d.Cin <= 256 && d.Cout % GBN == 0 && d.Cout <= GSmem::MAX_COUT) {
         const long long Mtot = (long long)in.B * in.H * in.Wp();
@@ -1290,7 +1259,7 @@ int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32,
         p->M = (int)Mtot;
         // L2 prefetch two tile rounds ahead for the K = 64 layers (one activation box per tile); the K = 256 layers
         // already keep 8 boxes per tile in flight
-        p->pf = (tc_prefetch_on() && p->num_kc == 1) ? 2 : 0;
+        p->pf = p->num_kc == 1 ? 2 : 0;
         m_tiles = (Mtot + BM - 1) / BM;
     } else if (gemm) {
         p->BN = BN;
@@ -1305,15 +1274,10 @@ int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32,
         p->rows_per_tile = BM / p->tw;
         p->wsegs = out.W / p->tw;
         p->parity = (d.sw == 2);
-        // one box for all rows of a tile when they are consecutive input rows of one image (stride 1 along H)
-        static const bool rowbox_on = [] { const char* e = getenv("HN_TC_ROWBOX"); return !(e && atoi(e) == 0); }();
-        static const bool rowbox2_on = [] { const char* e = getenv("HN_TC_ROWBOX2"); return !(e && atoi(e) == 0); }();
-        // ... or whole images when an image has fewer output rows than a tile (the last height-reduction convs):
-        // the box then spans R / Ho consecutive images of the plane
-        if (rowbox_on && p->rows_per_tile > 1 && (d.sh == 1 || (d.sh == 2 && rowbox2_on))) {
-            if (out.H % p->rows_per_tile == 0) { p->rowbox = 1; p->box_rows = p->rows_per_tile; }
-            else if (p->rows_per_tile % out.H == 0) { p->rowbox = 1; p->box_rows = out.H; p->box_imgs = p->rows_per_tile / out.H; }
-        }
+        // one box for all rows of a tile: consecutive output rows of one image, or whole images when an image has fewer
+        // output rows than a tile (the last height-reduction convs) -- the box then spans R / Ho consecutive images
+        if (out.H % p->rows_per_tile == 0) p->box_rows = p->rows_per_tile;
+        else { p->box_rows = out.H; p->box_imgs = p->rows_per_tile / out.H; }
         // dx reuse (HN_TC_DXR=0 disables).  Its epilogue slot is two weight slots, each half an output tile: a plane, or
         // half of the fp32 boxes -- which needs two of them (BN >= 64)
         static const int dxr_mode = [] { const char* e = getenv("HN_TC_DXR"); return e ? atoi(e) : 1; }();
@@ -1358,8 +1322,6 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
     a.shift = out_f32 ? d.shift : tc_aux + 2 * d.Cout;
     a.res = res_planes; a.out = out_planes; a.out_f32 = out_f32; a.out_plane = out_plane; a.relu = d.relu;
     a.Bimg = in.B;
-    a.seg = pl.seg;
-    { static int dbg = [] { const char* e = getenv("HN_TC_DBG"); return e ? atoi(e) : 0; }(); a.dbg = dbg; }
     a.mode = pl.mode;
     a.M = pl.M;
     if (pl.gemm_kernel) {
@@ -1391,22 +1353,22 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
         a.wsegs = pl.wsegs;
         a.sh = d.sh; a.ph = d.ph; a.woff = in.halo - d.pw;
         a.parity = pl.parity;
-        a.rowbox = pl.rowbox;
         a.dxr = pl.dxr;
-        // stride 2 along H (height-reduction convs): the box spans 2*rows input rows and takes every second one
-        const cuuint32_t boxrows = a.rowbox ? (cuuint32_t)(pl.box_rows * d.sh) : 1u;
-        const int hs = (a.rowbox && d.sh == 2) ? 2 : 1;
+        // stride 2 along H (height-reduction convs): a box of several rows spans 2*rows input rows and takes every second
+        // one; a one-row tile reads its input row without a traversal stride
+        const int hs = pl.rows_per_tile > 1 ? d.sh : 1;
+        const cuuint32_t boxrows = (cuuint32_t)(pl.box_rows * hs);
         const cuuint64_t C2 = (cuuint64_t)d.Cin * 2, Wp = in.Wp();
         if (!a.parity) {
             cuuint64_t dims[4] = {(cuuint64_t)d.Cin, Wp, (cuuint64_t)in.H, (cuuint64_t)2 * in.B};
             cuuint64_t str[3] = {C2, C2 * Wp, C2 * Wp * in.H};
             cuuint32_t box[4] = {BKC, a.dxr ? 130u : (cuuint32_t)a.tw, boxrows, (cuuint32_t)pl.box_imgs};
-            if (make_map(&tmA, in_planes, 4, dims, str, box, hs == 2 ? 2 : -1, hs)) return -1;
+            if (make_map(&tmA, in_planes, 4, dims, str, box, 2, hs)) return -1;
         } else {
             cuuint64_t dims[5] = {(cuuint64_t)d.Cin, 2, Wp / 2, (cuuint64_t)in.H, (cuuint64_t)2 * in.B};
             cuuint64_t str[4] = {C2, 2 * C2, C2 * Wp, C2 * Wp * in.H};
             cuuint32_t box[5] = {BKC, 1, (cuuint32_t)a.tw, boxrows, (cuuint32_t)pl.box_imgs};
-            if (make_map(&tmA, in_planes, 5, dims, str, box, hs == 2 ? 3 : -1, hs)) return -1;
+            if (make_map(&tmA, in_planes, 5, dims, str, box, 3, hs)) return -1;
         }
     }
     if (a.num_tiles == 0) return 0;
@@ -1477,7 +1439,6 @@ int bott_tc_planes(const ConvDesc& d2, const unsigned short* wq2, const float* a
     HN_CHECK(tiles < (1ll << 31) && (long long)out.B * out.H * out.Wp() < (1ll << 31), "bott_tc: too many tiles");
     a.num_tiles = (int)tiles;
     a.n3 = d3.Cout / 64; a.C3 = d3.Cout;
-    a.seg = tc_segment_chunks();
     a.scale2 = aux2 + 64; a.shift2 = aux2 + 2 * 64;                        // plane units (conv_tc.cuh: tc_aux)
     a.scale3 = aux3 + d3.Cout; a.shift3 = aux3 + 2 * d3.Cout;
     a.out = out_planes; a.out_plane = out_plane;

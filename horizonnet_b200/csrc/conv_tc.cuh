@@ -63,13 +63,13 @@ struct TcPlan {
     int mode;                 // 0: GEMM rows over all halo-NHWC pixels, 1: conv rows
     int M;                    // mode 0: pixel rows, mode 1: B * Ho output rows
     int tw, rows_per_tile, wsegs;          // mode 1: tile columns, output rows per tile, tiles per output row
-    int rowbox, box_rows, box_imgs;        // one TMA box for all rows of a tile: rows of one image x images
+    int box_rows, box_imgs;                // mode 1: the one TMA box of a tile's rows: rows of one image x images
     int dxr, parity;                       // 3x3 dx reuse of one 130-pixel input row; stride 2 along W (parity view)
-    int num_kc, seg;                       // K chunks of 64; chunks per tensor-core accumulation segment
+    int num_kc, seg;                       // K chunks of 64; chunks per tensor-core accumulation segment (SEG)
     int pf;                                // gemm_tc_kernel: L2 prefetch distance in tile rounds, 0 = off
     int n_tiles, num_tiles, grid;          // tiles along Cout, all tiles, CTAs (persistent, min(num_tiles, sms))
 };
-// Reads the HN_TC_* switches; -1 (with hn_last_error set) for a shape conv_tc_supported rejects or a residual with fp32
+// Reads HN_TC_DXR and HN_TC_GEMM; -1 (with hn_last_error set) for a shape conv_tc_supported rejects or a residual with fp32
 // output.  conv_tc_planes launches exactly this plan.
 int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32, bool has_residual, int sms, TcPlan* p);
 // fp32 halo-NHWC in/out convenience wrapper (unit tests): splits, runs the plane kernel, merges the output planes, or with

@@ -1093,7 +1093,8 @@ int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh,
     const Act o = mk(nullptr, B, (H + 2 * ph - kh) / sh + 1, (W + 2 * pw - kw) / sw + 1, Cout, out_halo);
     TcPlan p;
     if (conv_tc_plan(d, a, o, out_f32 != 0, has_residual != 0, sms, &p)) return -1;
-    const int v[18] = {p.gemm_kernel, p.BN, p.mode, p.M, p.tw, p.rows_per_tile, p.wsegs, p.rowbox, p.box_rows, p.box_imgs,
+    const int rowbox = p.mode == 1 && p.rows_per_tile > 1;
+    const int v[18] = {p.gemm_kernel, p.BN, p.mode, p.M, p.tw, p.rows_per_tile, p.wsegs, rowbox, p.box_rows, p.box_imgs,
                        p.dxr, p.parity, p.num_kc, p.seg, p.pf, p.n_tiles, p.num_tiles, p.grid};
     memcpy(plan, v, sizeof(v));
     return 0;

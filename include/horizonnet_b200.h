@@ -262,9 +262,9 @@ int hn_conv2d_dgrad_tc(int B, int H, int W, int Cin, const float* w_oihw, const 
 /* Host-side launch plan of the tensor-core convolution (no GPU work; sms = SM count to plan for) for the conv hn_conv2d
  * impl 1 (out_f32 = 0) or 2 (out_f32 = 1) would run, with or without a residual.  plan[18] = kernel (1 gemm_tc_kernel,
  * 0 conv_tc_kernel), BN, mode (0 GEMM rows, 1 conv rows), M (rows), tile columns, rows per tile, tiles per output row,
- * rowbox, box rows, box images, dx reuse, parity (stride 2 along W), K chunks, chunks per accumulation segment, L2 prefetch
- * distance, tiles along Cout, tiles, CTAs.  Reads the same HN_TC_* switches as the launch.  -1 for a shape the kernel
- * does not take. */
+ * rowbox (1: conv-row tiles of several output rows, which one box per plane loads), box rows, box images, dx reuse,
+ * parity (stride 2 along W), K chunks, chunks per accumulation segment, L2 prefetch distance, tiles along Cout, tiles,
+ * CTAs.  Reads HN_TC_DXR and HN_TC_GEMM like the launch.  -1 for a shape the kernel does not take. */
 int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
                     int out_halo, int out_f32, int has_residual, int sms, int plan[18]);
 int hn_bn_forward_backward(const float* z, int B, int H, int W, int C, const float* gamma, const float* beta,

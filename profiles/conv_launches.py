@@ -129,7 +129,7 @@ def main():
                 raise SystemExit(f'conv_launches.py: launch {i} ({name}) ran {row["kernel"]}, the plan says {want}')
             Ho, Wo = c['H'] // c['stride'][0], c['W'] // c['stride'][1]
             flops = 2.0 * c['B'] * Ho * Wo * c['Cout'] * c['Cin'] * c['k'] * c['k']
-            row.update({f: p[f] for f in ('BN', 'mode', 'dxr', 'rowbox', 'parity', 'num_kc', 'n_tiles', 'num_tiles',
+            row.update({f: p[f] for f in ('BN', 'mode', 'dxr', 'box_rows', 'parity', 'num_kc', 'n_tiles', 'num_tiles',
                                            'grid')})
             row['gflop'] = round(flops / 1e9, 3)
             row['tflops'] = round(flops / (row['us'] * 1e-6) / 1e12, 1)

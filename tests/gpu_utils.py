@@ -115,7 +115,7 @@ CANARY = 12345.5
 
 def run_tc_case(c, dev='cuda:0'):
     """Runs one case of tests/tc_cases.py through hn_conv2d (impl 1, or 2 for fp32 output) and checks it against the fp64
-    reference elementwise.  Returns (worst err / bound, sha1 of the output bytes); raises AssertionError on a violation."""
+    reference elementwise.  Returns worst err / bound; raises AssertionError on a violation."""
     lib = _lib.lib()
     x, w, scale, shift, res = tc_case_inputs(c, dev)
     B, Ci, H, W, Co, k = c['B'], c['Cin'], c['H'], c['W'], c['Cout'], c['k']
@@ -151,9 +151,7 @@ def run_tc_case(c, dev='cuda:0'):
         bound = bound + EPS21
     if res is not None:
         bound = bound + EPS21 * (res.double().abs() + 1.0)
-    ratio = _worst_ratio(y - ref, bound)
-    digest = hashlib.sha1(out.cpu().numpy().tobytes()).hexdigest()
-    return ratio, digest
+    return _worst_ratio(y - ref, bound)
 
 
 def _worst_ratio(diff, bound):

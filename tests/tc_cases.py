@@ -78,14 +78,14 @@ def plan(c, sms=SMS):
 
 def variant_key(c, p):
     """The code paths of conv_tc.cu this launch takes."""
-    return (('gemm_tc' if p['gemm_kernel'] else 'conv_tc'), p['BN'], p['mode'], p['dxr'], p['rowbox'], p['box_imgs'] > 1,
+    return (('gemm_tc' if p['gemm_kernel'] else 'conv_tc'), p['BN'], p['mode'], p['dxr'], p['box_rows'] > 1, p['box_imgs'] > 1,
             p['parity'], c['stride'][0], bool(c['out_f32']), bool(c['residual']),
             p['pf'] > 0 and p['num_tiles'] > p['pf'] * p['grid'],              # the L2 prefetch branch is live
             p['num_kc'] % p['seg'] != 0,                                         # last accumulation segment is short
             p['num_tiles'] > p['grid'])                                          # a CTA runs more than one tile
 
 
-KEY_FIELDS = ('kernel', 'BN', 'mode', 'dxr', 'rowbox', 'whole_images', 'parity', 'sh', 'out_f32', 'residual', 'prefetch',
+KEY_FIELDS = ('kernel', 'BN', 'mode', 'dxr', 'multi_row_box', 'whole_images', 'parity', 'sh', 'out_f32', 'residual', 'prefetch',
               'short_segment', 'multi_tile')
 
 
@@ -117,12 +117,12 @@ CASES = [
     case('dxr_bn64_w2', 2, 16, 256, 64, 64, 3, (1, 1)),                           # layer1 conv2 (wsegs 2)
     case('dxr_bn128_w2', 2, 64, 256, 64, 128, 3, (1, 1)),
     case('dxr_bn64_w1', 1, 16, 128, 128, 128, 3, (1, 1)),
-    # conv rows: rowbox of several rows of one image, and of whole images
+    # conv rows: one box of several rows of one image, and of whole images
     case('rowbox_s1', 2, 16, 32, 256, 256, 3, (1, 1)),                            # layer3 conv2: 4 rows per tile
     case('rowbox_s1_bn128', 8, 16, 32, 256, 256, 3, (1, 1)),
     case('rowbox_s1_k2304', 2, 8, 16, 512, 512, 3, (1, 1)),                       # layer4 conv2: 8 rows per tile
     case('images_s1', 5, 2, 32, 256, 128, 3, (1, 1)),                             # whole images, ragged last tile
-    # stride 2 (first blocks of layers 2-4): parity along W, rowbox2 along H
+    # stride 2 (first blocks of layers 2-4): parity along W, a box of every second input row along H
     case('s2_parity_rowbox2', 2, 32, 64, 128, 128, 3, (2, 2)),                    # layer3.0.conv2 shape family
     case('s2_parity_bn128', 8, 32, 64, 128, 128, 3, (2, 2)),
     case('s2_parity_norowbox', 2, 64, 256, 64, 128, 3, (2, 2)),                   # layer2.0.conv2: 128-wide rows
@@ -186,6 +186,7 @@ MODEL_CASES = [
     case('ghc2.1_raw_b8', 8, 16, 64, 256, 512, 3, (2, 1), out_f32=True),
     case('ghc2.3_dgrad_b1', 1, 4, 64, 64, 256, 3, (1, 1), out_f32=True),
     case('ghc2.3_dgrad_b32', 32, 4, 64, 64, 256, 3, (1, 1), out_f32=True),
+    case('ghc3.2_raw_b1', 1, 4, 32, 256, 512, 3, (2, 1), out_f32=True),
     case('ghc3.3_dgrad_b1', 1, 2, 32, 256, 512, 3, (1, 1), out_f32=True),
     case('ghc3.3_raw_b1', 1, 2, 32, 256, 256, 3, (2, 1), out_f32=True),
     case('layer1.0.conv1_b1', 1, 128, 256, 64, 64, 1, (1, 1)),

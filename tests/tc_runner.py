@@ -1,7 +1,7 @@
 """Runs unit cases of tests/tc_cases.py (or LSTM layers) in a fresh process, so that the HN_TC_* / HN_LSTM_CLUSTER switches,
 which the library reads once per process, take effect.  Prints one JSON line per case.
 
-    python tests/tc_runner.py conv NAME...        -> {"name", "ratio", "digest", "plan"}
+    python tests/tc_runner.py conv NAME...        -> {"name", "ratio", "plan"}
     python tests/tc_runner.py lstm T,B...         -> {"name", "err"}"""
 import json
 import os
@@ -59,9 +59,7 @@ def main(argv):
     for n in names:
         if kind == 'conv':
             c = cases[n]
-            ratio, digest = gu.run_tc_case(c)
-            print(json.dumps({'name': n, 'ratio': ratio, 'digest': digest, 'plan': tc_cases.plan(c, gu.device_sms())}),
-                  flush=True)
+            print(json.dumps({'name': n, 'ratio': gu.run_tc_case(c), 'plan': tc_cases.plan(c, gu.device_sms())}), flush=True)
         else:
             T, B = (int(v) for v in n.split(','))
             print(json.dumps({'name': n, 'err': lstm_error(T, B)}), flush=True)

@@ -27,17 +27,16 @@ def _check(c, p, sms):
     if p['mode'] == 0:                            # GEMM rows: every halo-NHWC pixel once
         assert k == 1 and (sh, sw) == (1, 1) and c['in_halo'] == c['out_halo'], name
         assert p['M'] == B * c['H'] * (c['W'] + 2 * c['in_halo']), name
+        assert not p['rowbox'] and p['box_rows'] == p['box_imgs'] == 1, name
         m_tiles = -(-p['M'] // BM)
     else:                                         # conv rows: B*Ho rows x Wo columns once
         assert p['M'] == B * Ho and p['tw'] * p['rows_per_tile'] == BM and p['wsegs'] * p['tw'] == Wo, name
         m_tiles = -(-p['M'] // p['rows_per_tile']) * p['wsegs']
         assert (m_tiles // p['wsegs'] - 1) * p['rows_per_tile'] < p['M'] <= m_tiles // p['wsegs'] * p['rows_per_tile'], name
         assert p['parity'] == (sw == 2), name
-        if p['rowbox']:
-            assert p['box_rows'] * p['box_imgs'] == p['rows_per_tile'], name
-            assert (p['box_imgs'] == 1 and Ho % p['rows_per_tile'] == 0) or p['box_rows'] == Ho, name
-        else:
-            assert p['box_rows'] == p['box_imgs'] == 1, name
+        assert p['box_rows'] * p['box_imgs'] == p['rows_per_tile'], name     # one TMA box per plane covers the tile
+        assert p['rowbox'] == (p['rows_per_tile'] > 1), name
+        assert (p['box_imgs'] == 1 and Ho % p['rows_per_tile'] == 0) or p['box_rows'] == Ho, name
         if p['dxr']:                              # the 130-pixel input row of the last tile stays inside Wp
             Wp = c['W'] + 2 * c['in_halo']
             assert p['rows_per_tile'] == 1 and k == 3 and sw == 1, name
@@ -103,8 +102,8 @@ def test_unit_cases_include_the_named_variants():
         for ws in (1, 2):
             assert has(lambda c, p: p['dxr'] and p['BN'] == bn and p['wsegs'] == ws)
     assert has(lambda c, p: p['BN'] == 32 and c['stride'] == (2, 1) and c['W'] == 256)
-    assert has(lambda c, p: p['parity'] and p['rowbox'] and c['stride'][0] == 2)
-    assert has(lambda c, p: p['parity'] and not p['rowbox'])
+    assert has(lambda c, p: p['parity'] and p['box_rows'] > 1 and c['stride'][0] == 2)
+    assert has(lambda c, p: p['parity'] and p['box_rows'] == 1)
     assert has(lambda c, p: p['box_imgs'] > 1 and c['B'] in (3, 5) and p['M'] % p['rows_per_tile'] != 0)
     assert has(lambda c, p: p['num_kc'] * 64 == 18432)
     for B in (2, 9):                              # LSTM projection shape, fp32 output
@@ -116,6 +115,8 @@ def test_plan_rejects_what_the_kernel_does_not_take():
     bad = [T.launch('cin48', 2, 16, 32, 48, 64, 3, (1, 1)),                       # Cin % 64
            T.launch('cout96', 2, 16, 32, 64, 96, 3, (1, 1)),                      # Cout > 64, not a multiple of 128
            T.launch('w24', 2, 16, 24, 64, 64, 3, (1, 1)),                         # W = 24: not a power-of-two tile width
+           T.launch('h3_w32', 2, 3, 32, 64, 64, 3, (1, 1)),                       # Ho = 3, 4 rows per tile: not one box
+           T.launch('sh3_w128', 1, 12, 128, 64, 64, 3, (3, 1)),                   # stride 3 along H
            T.launch('f32res', 2, 16, 32, 64, 64, 1, (1, 1), out_f32=True, residual=True)]
     for c in bad:
         assert T.plan(c) is None, c['name']
