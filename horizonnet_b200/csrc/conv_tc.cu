@@ -11,7 +11,9 @@
 //
 // conv_tc_kernel<BN> (persistent, one CTA per SM, 384 threads, launched with programmatic stream serialisation:
 // griddepcontrol.launch_dependents at entry, griddepcontrol.wait after the prologue) runs every convolution of the
-// tensor-core path (3x3 / strided / 1x1, the LSTM input projections, the data gradients of the training step):
+// tensor-core path (3x3 / strided / 1x1, the LSTM input projections, the data gradients of the training step).
+// Like every persistent kernel of this file it takes its tiles one at a time from the stream's tile counter (the
+// producer claims, the other roles read the index from a TileQueue, tc_common.cuh):
 //   warp 0     TMA producer: per 64-channel K chunk it loads A (hi, lo: 128 pixels x 64 ch, 128B swizzle) from the
 //              halo-NHWC planes with ONE box per plane -- {64 ch, tw pixels, R rows} for multi-row tiles (traversal
 //              stride 2 along H for the stride-(2,1) convs, whole images when an image has fewer rows than a tile);
@@ -281,14 +283,13 @@ __device__ __forceinline__ void tile_boxes(const TcArgs& a, const EpiLayout<BN>&
 template <int BN>
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO, const TcArgs a) {
+               const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO, const TcArgs a,
+               unsigned* sched) {
     using S = Smem<BN>;
     constexpr int NST = S::NST;
     constexpr int HALF_TILE = BM * BN * 2;     // one output plane; half an output tile
     static_assert(2 * HALF_TILE <= S::STAGE, "an output tile must fit one ring stage");
     pdl_trigger();
-    const int tile0 = (int)blockIdx.x;
-    const int tstride = (int)gridDim.x;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::BAR_OFF);
@@ -296,6 +297,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint64_t* oready_bar = empty_bar + NST;          // [NST] all 8 consumer warps have written the output tile in that stage
     uint64_t* afull_bar = oready_bar + NST;         // [2] dxr mode: input-row slot filled
     uint64_t* aempty_bar = afull_bar + 2;           // [2] dxr mode: the three taps have read the input-row slot
+    TileQueue* tq = reinterpret_cast<TileQueue*>(smem + S::BAR_OFF + 128);
     // dxr mode re-partitions the operand ring: two input-row slots (hi + lo plane, 136 rows of 128 B each, 130 used)
     // followed by NST weight-tile slots
     constexpr int AX_PLANE = 17 * 1024;
@@ -326,6 +328,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             mbar_init(oready_bar + i, CONS_WARPS);
         }
         for (int i = 0; i < 2; ++i) { mbar_init(afull_bar + i, 1); mbar_init(aempty_bar + i, CONS_WARPS); }
+        tq->init(CONS_WARPS + 1);                    // readers: the consumer warps and the store warp
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     pdl_wait();                                              // everything below reads / writes activations
@@ -339,7 +342,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (lane == 0) {
             int stage = 0, ast = 0;
             uint32_t phase = 0, aph = 0;
-            for (int tile = tile0; tile < a.num_tiles; tile += tstride) {
+            for (int it = 0;; ++it) {
+                const int tile = tq->claim(it, sched);
+                if (tile >= a.num_tiles) { sched_retire(sched); break; }
                 const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
                 int valid_rows = 1, row0 = 0, wo0 = 0;
                 if (a.mode == 1) tile_rows(a, mt, row0, valid_rows, wo0);
@@ -421,7 +426,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         float acc[BN / 2], sum[BN / 2];
         int stage = 0, ast = 0;
         uint32_t phase = 0, aph = 0;
-        for (int tile = tile0; tile < a.num_tiles; tile += tstride) {
+        for (int it = 0;; ++it) {
+            const int tile = tq->next(it);
+            __syncwarp();
+            if (lane == 0) tq->release(it);
+            if (tile >= a.num_tiles) break;
             const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
 #pragma unroll
             for (int j = 0; j < BN / 2; ++j) sum[j] = 0.f;
@@ -525,7 +534,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (lane == 0) {
             int stage = 0;
             uint32_t ophase = 0;                   // bit s: phase of oready_bar[s]
-            for (int tile = tile0; tile < a.num_tiles; tile += tstride) {
+            for (int it = 0;; ++it) {
+                const int tile = tq->next(it);
+                tq->release(it);
+                if (tile >= a.num_tiles) break;
                 const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
                 stage = (stage + a.num_kc) % NST;
                 mbar_wait(oready_bar + stage, (ophase >> stage) & 1);
@@ -579,7 +591,8 @@ __device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* tm, int c0, i
 
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO, const TcArgs a) {
+               const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO, const TcArgs a,
+               unsigned* sched) {
     using S = GSmem;
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
@@ -589,6 +602,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint64_t* rfull_bar = empty_bar + STAGES;       // [2] epilogue buffer holds the residual tile (or is simply free)
     uint64_t* efree_bar = rfull_bar + 2;            // [2] the TMA store has finished reading the epilogue buffer
     uint64_t* oready_bar = efree_bar + 2;           // [2] all 8 consumer warps have written their part of the output tile
+    TileQueue* tq = reinterpret_cast<TileQueue*>(smem + S::BAR_OFF + 128);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const bool has_res = a.res != nullptr;
 
@@ -600,6 +614,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (warp == 1 && lane == 0) {
         for (int i = 0; i < STAGES; ++i) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, CONS_WARPS); }
         for (int i = 0; i < 2; ++i) { mbar_init(rfull_bar + i, 1); mbar_init(efree_bar + i, 1); mbar_init(oready_bar + i, CONS_WARPS); }
+        tq->init(CONS_WARPS + 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // epilogue constants -> shared memory (weights-side data, safe to read before pdl_wait)
@@ -611,11 +626,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (warp == 0) {
         // =============================== TMA producer ===============================
         if (lane == 0) {
-            int stage = 0, it = 0;
+            int stage = 0;
             uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x, ++it) {
+            for (int it = 0;; ++it) {
+                const int tile = tq->claim(it, sched);
+                if (tile >= a.num_tiles) { sched_retire(sched); break; }
                 const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-                if (a.pf > 0) {                  // residual and activation boxes of the tile a.pf rounds ahead -> L2
+                // residual and activation boxes -> L2 of the tile claimed about a.pf rounds ahead (tiles are claimed in
+                // order, about gridDim.x per round)
+                if (a.pf > 0) {
                     const int ta = tile + a.pf * (int)gridDim.x;
                     if (ta < a.num_tiles) {
                         const int mta = ta / a.n_tiles, nta = ta - mta * a.n_tiles;
@@ -658,11 +677,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int wg = (warp - CONS_WARP0) >> 2;
         const uint32_t a_row_off = (uint32_t)(wg * 64 * 128);
         float acc[GBN / 2], sum[GBN / 2];
-        int stage = 0, it = 0;
+        int stage = 0;
         uint32_t phase = 0;
-        for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x, ++it) {
-            const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-            (void)mt;
+        for (int it = 0;; ++it) {
+            const int tile = tq->next(it);
+            __syncwarp();
+            if (lane == 0) tq->release(it);
+            if (tile >= a.num_tiles) break;
+            const int nt = tile % a.n_tiles;
 #pragma unroll
             for (int j = 0; j < GBN / 2; ++j) sum[j] = 0.f;
             int seg_pos = 0;
@@ -695,8 +717,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // one thread hands finished output tiles to the TMA engine and returns the buffer to the producer
         // as soon as the engine has read it, so the residual of tile it+2 is prefetched a whole tile ahead
         if (lane == 0) {
-            int it = 0;
-            for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x, ++it) {
+            for (int it = 0;; ++it) {
+                const int tile = tq->next(it);
+                tq->release(it);
+                if (tile >= a.num_tiles) break;
                 const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
                 const int eb = it & 1;
                 mbar_wait(oready_bar + eb, (it >> 1) & 1);
@@ -811,7 +835,7 @@ __global__ void stem_weight_pad_kernel(const float* __restrict__ w, float* __res
 
 __global__ void __launch_bounds__(NTHREADS, 1)
 stem_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmO, const StemArgs a) {
+               const __grid_constant__ CUtensorMap tmO, const StemArgs a, unsigned* sched) {
     using S = StSmem;
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
@@ -821,6 +845,7 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint64_t* bfull_bar = empty_bar + S::NSTAGE;   // weights resident
     uint64_t* oready_bar = bfull_bar + 1;          // [2] output tile staged by all 8 consumer warps
     uint64_t* efree_bar = oready_bar + 2;          // [2] the TMA store has read the staging buffer
+    TileQueue* tq = reinterpret_cast<TileQueue*>(smem + S::BAR_OFF + 128);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (warp == 0 && lane == 0) {
@@ -832,6 +857,7 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int i = 0; i < S::NSTAGE; ++i) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, CONS_WARPS); }
         mbar_init(bfull_bar, 1);
         for (int i = 0; i < 2; ++i) { mbar_init(oready_bar + i, CONS_WARPS); mbar_init(efree_bar + i, 1); }
+        tq->init(CONS_WARPS + 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -846,7 +872,9 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     tma_load_3d(smem + (pl * 4 + c) * S::B_CHUNK, &tmB, bfull_bar, c * BKC, 0, pl);
             int stage = 0;
             uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+            for (int it = 0;; ++it) {
+                const int tile = tq->claim(it, sched);
+                if (tile >= a.num_tiles) { sched_retire(sched); break; }
                 const int b = tile >> 10, yo = (tile >> 2) & 255, sg = tile & 3;
                 mbar_wait(empty_bar + stage, phase ^ 1);
                 uint8_t* sA = smem + S::A_OFF + stage * S::A_STAGE;
@@ -870,10 +898,14 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
         mbar_wait(bfull_bar, 0);
         const uint32_t sB = smem_u32(smem);
-        int stage = 0, it = 0;
+        int stage = 0;
         uint32_t phase = 0;
         float acc[32];
-        for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x, ++it) {
+        for (int it = 0;; ++it) {
+            const int tile = tq->next(it);
+            __syncwarp();
+            if (lane == 0) tq->release(it);
+            if (tile >= a.num_tiles) break;
             const int eb = it & 1;
             mbar_wait(full_bar + stage, phase);
             const uint32_t sA = smem_u32(smem + S::A_OFF + stage * S::A_STAGE) + (uint32_t)(wg * 64 * 16);
@@ -919,8 +951,10 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
     } else if (warp == 3) {
         if (lane == 0) {
-            int it = 0;
-            for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x, ++it) {
+            for (int it = 0;; ++it) {
+                const int tile = tq->next(it);
+                tq->release(it);
+                if (tile >= a.num_tiles) break;
                 const int b = tile >> 10, yo = (tile >> 2) & 255, sg = tile & 3;
                 const int eb = it & 1;
                 mbar_wait(oready_bar + eb, (it >> 1) & 1);
@@ -982,7 +1016,7 @@ static_assert(BtSmem::T2_OFF % 1024 == 0 && BtSmem::E_OFF % 1024 == 0 && BtSmem:
 __global__ void __launch_bounds__(NTHREADS, 1)
 bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB2,
                const __grid_constant__ CUtensorMap tmB3, const __grid_constant__ CUtensorMap tmR,
-               const __grid_constant__ CUtensorMap tmO, const BottArgs a) {
+               const __grid_constant__ CUtensorMap tmO, const BottArgs a, unsigned* sched) {
     using S = BtSmem;
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
@@ -994,6 +1028,7 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint64_t* rfull_bar = aempty_bar + 2;           // [2] residual tile landed in the epilogue buffer
     uint64_t* oready_bar = rfull_bar + 2;           // [2] output tile complete in the epilogue buffer
     uint64_t* efree_bar = oready_bar + 2;           // [2] TMA store has read the epilogue buffer
+    TileQueue* tq = reinterpret_cast<TileQueue*>(smem + S::BAR_OFF + 128);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (warp == 0 && lane == 0) {
@@ -1009,6 +1044,7 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             mbar_init(afull_bar + i, 1); mbar_init(aempty_bar + i, CONS_WARPS);
             mbar_init(rfull_bar + i, 1); mbar_init(oready_bar + i, CONS_WARPS); mbar_init(efree_bar + i, 1);
         }
+        tq->init(CONS_WARPS + 2);                    // readers: the consumer warps, the residual loader, the store warp
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // epilogue constants -> shared memory (weights-side data, safe to read before pdl_wait)
@@ -1024,7 +1060,9 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (lane == 0) {
             int ast = 0, bst = 0;
             uint32_t aph = 0, bph = 0;
-            for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+            for (int it = 0;; ++it) {
+                const int tile = tq->claim(it, sched);
+                if (tile >= a.num_tiles) { sched_retire(sched); break; }
                 const int rg = tile / a.wsegs;
                 const int wo0 = (tile - rg * a.wsegs) * BM;
                 const int b = rg / a.Ho, ho = rg - b * a.Ho;
@@ -1061,7 +1099,10 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // its own thread, so that the identity tile of n-tile j is requested the moment its epilogue buffer is released
         if (lane == 0) {
             int g3 = 0;
-            for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+            for (int it = 0;; ++it) {
+                const int tile = tq->next(it);
+                tq->release(it);
+                if (tile >= a.num_tiles) break;
                 const int rg = tile / a.wsegs;
                 const int pix0 = rg * a.Wop + 1 + (tile - rg * a.wsegs) * BM;
                 for (int j = 0; j < n3; ++j, ++g3) {
@@ -1078,7 +1119,10 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // =============================== store warp ===============================
         if (lane == 0) {
             int g3 = 0;
-            for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+            for (int it = 0;; ++it) {
+                const int tile = tq->next(it);
+                tq->release(it);
+                if (tile >= a.num_tiles) break;
                 const int rg = tile / a.wsegs;
                 const int pix0 = rg * a.Wop + 1 + (tile - rg * a.wsegs) * BM;
                 for (int j = 0; j < n3; ++j, ++g3) {
@@ -1107,7 +1151,11 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             if (lane == 0) mbar_arrive(empty_bar + bst);
             if (++bst == S::NB) { bst = 0; bph ^= 1; }
         };
-        for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+        for (int it = 0;; ++it) {
+            const int tile = tq->next(it);
+            __syncwarp();
+            if (lane == 0) tq->release(it);
+            if (tile >= a.num_tiles) break;
             const int rg = tile / a.wsegs;
             const int wo0 = (tile - rg * a.wsegs) * BM;
             // ---- conv2 (identical to conv_tc_kernel<64>)

@@ -12,16 +12,20 @@
 //             at a time, lane-contiguous so that every read is conflict-free); per-row power-of-two scale
 //             (11 + 11 significant bits)
 //   step    = D[128 rows x 8 cols] = W[128 x 512] h[512 x 8]: three products Whi*hhi + Whi*hlo + Wlo*hhi with
-//             mma.sync.m16n8k16, K split over the 8 warps, partial sums reduced through shared memory; thread
+//             mma.sync.m16n8k16, K split over the 8 warps, partial sums reduced through shared memory in two halves
+//             of 64 rows (gates i, f, then g, o: the partial-sum block is 17 KB instead of 33 KB); thread
 //             (column = warp, unit = lane) finishes one cell in fp32, writes the fp32 output and the fp16 hi/lo planes
 //             of 256*h into a 1152-byte staging block; one thread then bulk-copies that block into the receive
 //             buffer of all 16 CTAs of the cluster (cp.async.bulk shared::cta -> shared::cluster), each copy
 //             completing on the destination's mbarrier.  Receive / staging buffers are double-buffered by step
 //             parity; a peer can only send h_{t+1} after it has received this CTA's h_t, which makes that safe
 //             without any further handshake.
-//   groups  = one column group of 8 per cluster (the 128 KB of W_lo fragments leave no shared memory for a second
-//             group's exchange buffers); clusters beyond what the device co-schedules run in a later wave.
-//   grid    = 2 directions x ceil(B/8) clusters.
+//   groups  = one or two column groups of 8 per cluster, interleaved step by step (each group has its own exchange
+//             buffers and barriers): while one group's h is in flight between the CTAs the other group's MMAs run.
+//             Two groups per cluster when one group each would not fit in one wave of co-resident clusters (see
+//             lstm_layer_cluster): the batch-32 recurrence then takes 4 clusters = 64 of the 132 SMs and leaves the
+//             rest to the next batch's encoder.  Clusters beyond what the device co-schedules run in a later wave.
+//   grid    = 2 directions x ceil(B/8) clusters, or 2 directions x ceil(B/16) with two groups per cluster.
 #include <cuda_fp16.h>
 #include <cstdlib>
 #include "hn_common.cuh"
@@ -39,18 +43,20 @@ constexpr int NT = 256;                 // 8 warps
 constexpr float H_SCALE = 256.f;        // h planes carry 256*h (|h| < 1): lo stays in fp16's normal range
 constexpr int COLP = 144;               // bytes per column of an exchange block: 64 B hi + 64 B lo + 16 B pad (bank spread)
 constexpr int BLK = NCOL * COLP;        // 1152 B: one CTA's h of one step (32 units x 8 columns, hi + lo)
-constexpr int PCOL = 132;               // floats per column of a partial-sum block: 128 rows + 4 pad (bank spread)
+constexpr int PROWS = 64;               // rows of W_hh per partial-sum half (two gates)
+constexpr int PCOL = PROWS + 4;         // floats per column of a partial-sum block: 64 rows + 4 pad (bank spread)
 
-constexpr int MAXG = 1;                                        // column groups interleaved by one cluster
+constexpr int MAXG = 2;                                        // column groups interleaved by one cluster
 constexpr int SM_RECV = 0;                                     // [MAXG][2 parity][16 source CTAs][BLK]
 constexpr int SM_STAGE = SM_RECV + MAXG * 2 * CL * BLK;        // [MAXG][2 parity][BLK]
-constexpr int SM_PART = SM_STAGE + MAXG * 2 * BLK;             // [8 warps][NCOL][PCOL] fp32 (init: per-row maxima)
+constexpr int SM_PART = SM_STAGE + MAXG * 2 * BLK;             // [8 warps][NCOL][PCOL] fp32 (init: [8 warps][128] row maxima)
 constexpr int SM_WLO = SM_PART + 8 * NCOL * PCOL * 4;          // W_hh lo fragments [8 warps][128 registers][32 lanes]
 constexpr int SM_BAR = SM_WLO + 8 * 128 * 32 * 4;              // full[MAXG][2]
 constexpr int SM_TOTAL = SM_BAR + 64;
 static_assert(SM_RECV % 16 == 0 && SM_STAGE % 16 == 0 && SM_PART % 16 == 0 && SM_WLO % 16 == 0 && SM_BAR % 8 == 0,
               "alignment");
 static_assert(SM_TOTAL <= 227 * 1024, "shared memory per block");
+static_assert(8 * 128 <= 8 * NCOL * PCOL, "init row maxima fit the partial-sum block");
 
 struct ClArgs {
     const float* xproj;      // [T][B][4096]  (dir*2048 + gate*512 + unit), bias already added
@@ -183,64 +189,75 @@ __global__ void __launch_bounds__(NT, 1) lstm_cluster_kernel(const ClArgs a) {
 #pragma unroll
                 for (int g = 0; g < 4; ++g) xp[g] = __ldg(xb + g * HID);
             }
+            float sum[4] = {0.f, 0.f, 0.f, 0.f};
             if (step > 0) {
                 const int par = (step - 1) & 1;
                 mbar_wait(full_bar + g2 * 2 + par, ((step - 1) >> 1) & 1);
                 const uint8_t* rb = smem + SM_RECV + (g2 * 2 + par) * (CL * BLK);
                 float* pw = part + warp * (NCOL * PCOL);
 #pragma unroll
-                for (int mp = 0; mp < 4; ++mp) {                   // two m-tiles per tensor-memory read
-                    uint32_t al[32];
+                for (int hh = 0; hh < 2; ++hh) {                   // rows [64 hh, 64 hh + 64): gates 2 hh, 2 hh + 1
+                    float v[2][2][4];                              // [mp][mm][fragment element]: this warp's partial sums
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) al[i] = wlo[(mp * 32 + i) * 32];
-                    // six independent accumulators (2 m-tiles x 3 products): consecutive MMAs never depend on each other
-                    float d[2][3][4];
+                    for (int mq = 0; mq < 2; ++mq) {               // two m-tiles per tensor-memory read
+                        const int mp = 2 * hh + mq;
+                        uint32_t al[32];
 #pragma unroll
-                    for (int mm = 0; mm < 2; ++mm)
+                        for (int i = 0; i < 32; ++i) al[i] = wlo[(mp * 32 + i) * 32];
+                        // six independent accumulators (2 m-tiles x 3 products): consecutive MMAs never depend on each other
+                        float d[2][3][4];
 #pragma unroll
-                        for (int pr = 0; pr < 3; ++pr)
+                        for (int mm = 0; mm < 2; ++mm)
 #pragma unroll
-                            for (int e = 0; e < 4; ++e) d[mm][pr][e] = 0.f;
+                            for (int pr = 0; pr < 3; ++pr)
 #pragma unroll
-                    for (int kt = 0; kt < 4; ++kt) {
-                        // B fragments: k = 64*warp + 16*kt + 2*tig (+8) -> source CTA k/32, unit k%32; column gid
-                        const uint8_t* hb = rb + (2 * warp + (kt >> 1)) * BLK + gid * COLP + ((kt & 1) * 16 + tig * 2) * 2;
-                        const uint32_t bh0 = *reinterpret_cast<const uint32_t*>(hb);
-                        const uint32_t bh1 = *reinterpret_cast<const uint32_t*>(hb + 16);
-                        const uint32_t bl0 = *reinterpret_cast<const uint32_t*>(hb + 64);
-                        const uint32_t bl1 = *reinterpret_cast<const uint32_t*>(hb + 64 + 16);
+                                for (int e = 0; e < 4; ++e) d[mm][pr][e] = 0.f;
+#pragma unroll
+                        for (int kt = 0; kt < 4; ++kt) {
+                            // B fragments: k = 64*warp + 16*kt + 2*tig (+8) -> source CTA k/32, unit k%32; column gid
+                            const uint8_t* hb = rb + (2 * warp + (kt >> 1)) * BLK + gid * COLP + ((kt & 1) * 16 + tig * 2) * 2;
+                            const uint32_t bh0 = *reinterpret_cast<const uint32_t*>(hb);
+                            const uint32_t bh1 = *reinterpret_cast<const uint32_t*>(hb + 16);
+                            const uint32_t bl0 = *reinterpret_cast<const uint32_t*>(hb + 64);
+                            const uint32_t bl1 = *reinterpret_cast<const uint32_t*>(hb + 64 + 16);
+#pragma unroll
+                            for (int mm = 0; mm < 2; ++mm) {
+                                const int m = mp * 2 + mm;
+                                const uint32_t alo[4] = {al[(mm * 4 + kt) * 4 + 0], al[(mm * 4 + kt) * 4 + 1],
+                                                         al[(mm * 4 + kt) * 4 + 2], al[(mm * 4 + kt) * 4 + 3]};
+                                mma16816(d[mm][0], a_hi[m][kt], bh0, bh1);
+                                mma16816(d[mm][1], a_hi[m][kt], bl0, bl1);
+                                mma16816(d[mm][2], alo, bh0, bh1);
+                            }
+                        }
+#pragma unroll
+                        for (int mm = 0; mm < 2; ++mm)
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) v[mq][mm][e] = d[mm][0][e] + (d[mm][1][e] + d[mm][2][e]);
+                    }
+                    if (hh) __syncthreads();                       // every thread has read the first half
+                    // partial sums of this warp's k-range: part[warp][column][row - 64 hh]
+#pragma unroll
+                    for (int mq = 0; mq < 2; ++mq)
 #pragma unroll
                         for (int mm = 0; mm < 2; ++mm) {
-                            const int m = mp * 2 + mm;
-                            const uint32_t alo[4] = {al[(mm * 4 + kt) * 4 + 0], al[(mm * 4 + kt) * 4 + 1],
-                                                     al[(mm * 4 + kt) * 4 + 2], al[(mm * 4 + kt) * 4 + 3]};
-                            mma16816(d[mm][0], a_hi[m][kt], bh0, bh1);
-                            mma16816(d[mm][1], a_hi[m][kt], bl0, bl1);
-                            mma16816(d[mm][2], alo, bh0, bh1);
+                            const int r = 16 * (2 * mq + mm) + gid;
+                            pw[(tig * 2) * PCOL + r] = v[mq][mm][0];
+                            pw[(tig * 2 + 1) * PCOL + r] = v[mq][mm][1];
+                            pw[(tig * 2) * PCOL + r + 8] = v[mq][mm][2];
+                            pw[(tig * 2 + 1) * PCOL + r + 8] = v[mq][mm][3];
                         }
-                    }
-                    // partial sums of this warp's k-range: part[warp][column][row]
+                    __syncthreads();
+                    // ((p0 + p1) + ...) + p7 over the 8 warps' k-ranges, for the two gates of this half
 #pragma unroll
-                    for (int mm = 0; mm < 2; ++mm) {
-                        const int m = mp * 2 + mm;
-                        pw[(tig * 2) * PCOL + 16 * m + gid] = d[mm][0][0] + (d[mm][1][0] + d[mm][2][0]);
-                        pw[(tig * 2 + 1) * PCOL + 16 * m + gid] = d[mm][0][1] + (d[mm][1][1] + d[mm][2][1]);
-                        pw[(tig * 2) * PCOL + 16 * m + gid + 8] = d[mm][0][2] + (d[mm][1][2] + d[mm][2][2]);
-                        pw[(tig * 2 + 1) * PCOL + 16 * m + gid + 8] = d[mm][0][3] + (d[mm][1][3] + d[mm][2][3]);
-                    }
+                    for (int gq = 0; gq < 2; ++gq)
+#pragma unroll
+                        for (int w8 = 0; w8 < 8; ++w8) sum[2 * hh + gq] += part[(w8 * NCOL + col) * PCOL + gq * 32 + lane];
                 }
-                __syncthreads();
             }
             float pre[4];
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                float sum = 0.f;
-                if (step > 0) {
-#pragma unroll
-                    for (int w8 = 0; w8 < 8; ++w8) sum += part[(w8 * NCOL + col) * PCOL + g * 32 + lane];
-                }
-                pre[g] = fmaf(sum, unscale[g], xp[g]);
-            }
+            for (int g = 0; g < 4; ++g) pre[g] = fmaf(sum[g], unscale[g], xp[g]);
             const float c_new = sigmoidf_(pre[1]) * c_state[g2] + sigmoidf_(pre[0]) * tanhf(pre[2]);
             c_state[g2] = c_new;
             const float h_new = sigmoidf_(pre[3]) * tanhf(c_new);
@@ -306,7 +323,10 @@ int lstm_layer_cluster(const float* xproj, const float* w_hh_fwd, const float* w
     ClArgs a;
     a.xproj = xproj; a.w_hh[0] = w_hh_fwd; a.w_hh[1] = w_hh_bwd; a.out = out;
     a.T = T; a.B = B; a.ngroups = (B + NCOL - 1) / NCOL;
-    // one wave of clusters if possible: a cluster interleaves MAXG column groups when 2 x groups exceeds what fits
+    // One group per cluster when every cluster fits in one wave: a second group makes a cluster about 1.5x slower
+    // (T = 256 on an H100 at 400 W: 2 clusters 1.46 ms with one group each, 2.19 ms with two).  Two groups per
+    // cluster when one group each would need a second wave: batch 32 on the 7 co-resident clusters of that H100 runs
+    // in 2.15 ms on 4 clusters instead of 3.07 ms in two waves, and leaves 68 SMs to the other stream.
     a.gpc = (2 * a.ngroups <= max_clusters) ? 1 : MAXG;
     const int nclusters = 2 * ((a.ngroups + a.gpc - 1) / a.gpc);
     cudaLaunchConfig_t cfg = {};

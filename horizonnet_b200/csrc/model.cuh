@@ -135,8 +135,10 @@ struct hn_model {
     float* bon_slot[2] = {nullptr, nullptr};        // device outputs of the two host-pipeline slots
     float* cor_slot[2] = {nullptr, nullptr};
     // Two-stream schedule of the throughput entry points (hn_model_forward_async, submit/collect): the encoder +
-    // height reduction of batch i+1 run on enc_stream while the bi-LSTM + head of batch i (64 of the 132 SMs,
-    // latency-bound) run on the high-priority rnn_stream.
+    // height reduction of batch i+1 run on enc_stream while the bi-LSTM + head of batch i run on the high-priority
+    // rnn_stream.  The recurrence is latency-bound; at batch 32 on an H100 that co-schedules 7 of its 16-CTA clusters
+    // it takes 4 clusters, 64 of the 132 SMs (lstm_cluster.cu), and the persistent convolution kernels of enc_stream claim their tiles at run time, so the
+    // CTAs resident on the other SMs keep the encoder going meanwhile (tc_common.cuh, TileQueue).
     cudaStream_t enc_stream = nullptr, rnn_stream = nullptr;
     cudaEvent_t ev_in = nullptr, ev_xfree = nullptr, ev_seq = nullptr, ev_rnn_last = nullptr, ev_plain_done = nullptr;
     cudaEvent_t async_done[2] = {nullptr, nullptr}, slot_done[2] = {nullptr, nullptr};

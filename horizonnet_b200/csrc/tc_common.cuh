@@ -5,8 +5,10 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdlib>
+#include <map>
 #include <mutex>
 #include <string>
+#include <utility>
 
 #include "hn_common.cuh"
 #include "ptx.cuh"
@@ -44,6 +46,50 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* tm, ui
 // grid has completed and flushed: the kernel boundaries of a forward stop costing a launch latency + prologue each.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+// Dynamic tile scheduling of the persistent kernels.  A CTA does not own a fixed share of the tiles: its producer
+// thread claims one tile at a time from a global counter (`sched`, see tile_counter) and hands the index to the other
+// roles of the CTA through this queue, in claim order.  CTAs that become resident late -- while the LSTM recurrence of
+// another stream holds part of the GPU -- therefore find less work left, and the launch ends when the tiles run out
+// rather than when the last CTA has worked through a share fixed at launch.  The tile-to-CTA assignment changes no
+// arithmetic: every tile is computed exactly as before.  The producer pushes one index past the last tile as the end
+// marker.  Kept in the barrier area of the kernel's shared memory (80 bytes).
+struct TileQueue {
+    static constexpr int N = 4;
+    uint64_t full[N];         // the index of slot i has been written
+    uint64_t empty[N];        // every reader has taken it
+    int tile[N];
+    __device__ __forceinline__ void init(uint32_t readers) {
+        for (int i = 0; i < N; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, readers); }
+    }
+    // producer, it-th claim: waits for a free slot, claims the next tile of the launch, publishes it
+    __device__ __forceinline__ int claim(int it, unsigned* sched) {
+        const int s = it % N;
+        mbar_wait(empty + s, ((it / N) & 1) ^ 1);
+        const int t = (int)atomicAdd(sched, 1u);
+        tile[s] = t;
+        mbar_arrive(full + s);
+        return t;
+    }
+    // reader, it-th index; every reading warp then calls release(it) once (after __syncwarp)
+    __device__ __forceinline__ int next(int it) {
+        const int s = it % N;
+        mbar_wait(full + s, (it / N) & 1);
+        return *static_cast<volatile int*>(tile + s);
+    }
+    __device__ __forceinline__ void release(int it) { mbar_arrive(empty + it % N); }
+};
+static_assert(sizeof(TileQueue) <= 128, "the kernels keep the queue in the upper 128 bytes of a 256-byte barrier area");
+// The producer of each CTA calls this once, after the claim that returned the end marker.  The last CTA to get
+// there resets the counter for the next launch on the stream, which reads it only after pdl_wait(), i.e. after
+// this grid has completed and flushed.
+__device__ __forceinline__ void sched_retire(unsigned* sched) {
+    __threadfence();          // this CTA's claims come before its retirement
+    if (atomicAdd(sched + 1, 1u) == gridDim.x - 1) {
+        atomicExch(sched, 0u);
+        atomicExch(sched + 1, 0u);
+    }
+}
 
 // 128-byte swizzle shared-memory matrix descriptor of wgmma (sm_90 layout: start address bits [0,14), leading byte
 // offset [16,30), stride byte offset [32,46), layout type [62,64) = 1 for SWIZZLE_128B).  K-major operands: rows of
@@ -149,9 +195,36 @@ inline bool pdl_on() {
     return on;
 }
 
-// launch of a persistent tensor-core kernel with programmatic stream serialisation (see pdl_trigger / pdl_wait)
+// Tile counter (TileQueue::claim, sched_retire) of the persistent kernels launched on stream `st`: two unsigned ints,
+// zero between launches.  One per (device, stream): launches on one stream run one after the other (the next one
+// claims only after pdl_wait), launches on different streams -- the encoder and recurrence streams of the pipelined
+// forward -- may run at the same time and must not share a counter.
+inline cudaError_t tile_counter(cudaStream_t st, unsigned** out) {
+    static std::mutex mu;
+    static std::map<std::pair<int, unsigned long long>, unsigned*> counters;
+    int dev = 0;
+    unsigned long long id = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaStreamGetId(st, &id);
+    if (e != cudaSuccess) return e;
+    std::lock_guard<std::mutex> lock(mu);
+    unsigned*& c = counters[{dev, id}];
+    if (!c) {
+        e = cudaMalloc(reinterpret_cast<void**>(&c), 2 * sizeof(unsigned));
+        if (e == cudaSuccess) e = cudaMemsetAsync(c, 0, 2 * sizeof(unsigned), st);
+        if (e != cudaSuccess) { c = nullptr; return e; }
+    }
+    *out = c;
+    return cudaSuccess;
+}
+
+// launch of a persistent tensor-core kernel with programmatic stream serialisation (see pdl_trigger / pdl_wait); the
+// kernel's last parameter is the stream's tile counter
 template <typename K, typename... Args>
 inline cudaError_t launch_tc(K kernel, int grid, size_t smem_bytes, cudaStream_t st, Args... args) {
+    unsigned* sched = nullptr;
+    const cudaError_t e = tile_counter(st, &sched);
+    if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)grid);
     cfg.blockDim = dim3(NTHREADS);
@@ -162,7 +235,7 @@ inline cudaError_t launch_tc(K kernel, int grid, size_t smem_bytes, cudaStream_t
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at;
     cfg.numAttrs = pdl_on() ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, args...);
+    return cudaLaunchKernelEx(&cfg, kernel, args..., sched);
 }
 
 }  // namespace tc
