@@ -8,7 +8,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libhorizonnet_b200.so')
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 _lib = None
 _lock = threading.Lock()
@@ -52,7 +52,7 @@ SIGNATURES = {
     'hn_bn_forward_backward': (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp,
                                               ctypes.c_double, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp,
                                               vp]),
-    'hn_lstm_layer_backward': (ctypes.c_int, [vp, vp, vp, vp, vp, ctypes.c_int, ctypes.c_int, vp, vp, vp]),
+    'hn_lstm_layer_backward': (ctypes.c_int, [vp, vp, vp, vp, vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp, vp, vp]),
     'hn_train_profile': (ctypes.c_int, [vp, ctypes.POINTER(ctypes.c_double)]),
     'hn_train_profile_units': (ctypes.c_int, [vp, ctypes.POINTER(ctypes.c_double)]),
     'hn_train_debug_unit': (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_int, vp, ctypes.c_longlong, c_int_p, ctypes.c_char_p,

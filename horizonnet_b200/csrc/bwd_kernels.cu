@@ -1145,24 +1145,38 @@ int lstm_cell_scan(float* gates, float* cell, int T, int B, cudaStream_t st) {
     return 0;
 }
 
+// the cooperative kernel for batch B: staged for B <= 16 (dynamic shared memory = one step's dG of one direction)
+static void* lstm_bwd_persistent_for(int B, size_t* smem) {
+    const bool staged = B <= 16;
+    *smem = staged ? (size_t)B * 2048 * sizeof(float) : 0;
+    return staged ? reinterpret_cast<void*>(lstm_bwd_persistent_kernel<true>)
+                  : reinterpret_cast<void*>(lstm_bwd_persistent_kernel<false>);
+}
+
+int lstm_bwd_persistent_fits(int B, bool* fits) {
+    size_t smem = 0;
+    void* kernel = lstm_bwd_persistent_for(B, &smem);
+    int dev = 0, coop = 0, sms = 0, per_sm = 0;
+    HN_CUDA_OK(cudaGetDevice(&dev));
+    HN_CUDA_OK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+    HN_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    if (smem) HN_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    HN_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256, smem));
+    *fits = coop && per_sm * sms >= 128;
+    return 0;
+}
+
 int lstm_bwd_steps(const float* dout, const float* gates, const float* cell, const float* whh_t_f, const float* whh_t_b,
                    float* dgates, float* dc, int T, int B, unsigned int* barrier, int* error_flag, cudaStream_t st) {
     LstmBwdArgs a;
     a.dout = dout; a.gates = gates; a.cell = cell; a.whh_t[0] = whh_t_f; a.whh_t[1] = whh_t_b; a.dgates = dgates; a.dc = dc;
     a.T = T; a.B = B; a.step = 0;
-    int dev = 0, coop = 0, sms = 0, per_sm = 0;
-    HN_CUDA_OK(cudaGetDevice(&dev));
-    HN_CUDA_OK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-    HN_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const bool staged = B <= 16;
-    const size_t smem = staged ? (size_t)B * 2048 * sizeof(float) : 0;
-    void* kernel = staged ? reinterpret_cast<void*>(lstm_bwd_persistent_kernel<true>)
-                          : reinterpret_cast<void*>(lstm_bwd_persistent_kernel<false>);
-    if (staged) HN_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    HN_CUDA_OK(staged ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm_bwd_persistent_kernel<true>, 256, smem)
-                      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm_bwd_persistent_kernel<false>, 256, 0));
-    if (barrier && error_flag && coop && per_sm * sms >= 128) {
+    bool fits = false;
+    if (barrier && error_flag && lstm_bwd_persistent_fits(B, &fits)) return -1;
+    if (fits) {
         // one cooperative launch for the whole sequence (128 co-resident CTAs, grid barrier between the steps)
+        size_t smem = 0;
+        void* kernel = lstm_bwd_persistent_for(B, &smem);
         HN_CUDA_OK(cudaMemsetAsync(barrier, 0, sizeof(unsigned int), st));
         void* args[] = {&a, &barrier, &error_flag};
         HN_CUDA_OK(cudaLaunchCooperativeKernel(kernel, dim3(64, 2), dim3(256), args, smem, st));

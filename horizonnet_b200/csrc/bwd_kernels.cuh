@@ -57,7 +57,10 @@ int lstm_gather(const float* hout, const float* xp, float* hprev, float* xpd, in
 int lstm_cell_scan(float* gates, float* cell, int T, int B, cudaStream_t st);
 // whh_t_*: W_hh transposed, [512][2048] (the same copies the gate GEMM uses)
 // barrier (1 uint) / error_flag (1 int): device scratch of the single cooperative launch (grid barrier between the steps;
-// a barrier time-out sets *error_flag); nullptr: one launch per time step
+// a barrier time-out sets *error_flag); nullptr, or a device that cannot co-schedule that launch
+// (lstm_bwd_persistent_fits): one launch per time step
+// *fits = the device can co-schedule the 128 CTAs of the cooperative launch for batch B
+int lstm_bwd_persistent_fits(int B, bool* fits);
 int lstm_bwd_steps(const float* dout, const float* gates, const float* cell, const float* whh_t_f, const float* whh_t_b,
                    float* dgates, float* dc, int T, int B, unsigned int* barrier, int* error_flag, cudaStream_t st);
 int stem_input_nhwc(const float* x, int in_channels, float* out, int B, cudaStream_t st);

@@ -280,7 +280,7 @@ int conv_bn(hn_model* m, const ConvLayer& c, const Act& in, const Act& out, cons
 extern "C" {
 
 const char* hn_last_error(void) { return g_err.c_str(); }
-int hn_abi_version(void) { return 4; }
+int hn_abi_version(void) { return 5; }
 const char* hn_build_digest(void) { return HN_BUILD_DIGEST; }
 long long hn_kernel_launches(void) { return g_launches.load(); }
 

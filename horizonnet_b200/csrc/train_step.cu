@@ -773,9 +773,9 @@ int hn_bn_forward_backward(const float* z, int B, int H, int W, int C, const flo
 }
 
 // One bidirectional LSTM layer backward from its saved forward tensors: xp [T][B][4096] (input projection + biases),
-// hout [T][B][1024], dout [T][B][1024] -> dgates [2][T][B][2048] (= d xp, per direction).  scratch: floats, see test.
+// hout [T][B][1024], dout [T][B][1024] -> dgates [2][T][B][2048] (= d xp, per direction).  Scratch layout: see the header.
 int hn_lstm_layer_backward(const float* xp, const float* hout, const float* whf, const float* whb, const float* dout, int T,
-                           int B, float* dgates, float* scratch, void* stream) {
+                           int B, int persistent, float* dgates, float* scratch, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     const size_t rows = (size_t)T * B;
     float* hprev = scratch;                         // 2*rows*512
@@ -784,6 +784,15 @@ int hn_lstm_layer_backward(const float* xp, const float* hout, const float* whf,
     float* dc = cell + 2 * rows * 512;              // 2*B*512
     float* wt = dc + (size_t)2 * B * 512;           // 2*512*2048
     float* ones = wt + (size_t)2 * 512 * 2048;      // 4096 + 4096
+    unsigned int* barrier = reinterpret_cast<unsigned int*>(ones + 8192);
+    int* error_flag = reinterpret_cast<int*>(ones + 8193);
+    if (persistent) {
+        bool fits = false;
+        if (lstm_bwd_persistent_fits(B, &fits)) return -1;
+        HN_CHECK(fits, "hn_lstm_layer_backward: cooperative BPTT kernel not supported on this device (its 128 CTAs cannot be "
+                       "co-resident)");
+        HN_CUDA_OK(cudaMemsetAsync(error_flag, 0, sizeof(int), st));
+    }
     if (fill_f32(ones, 4096, 1.f, st) || fill_f32(ones + 4096, 4096, 0.f, st)) return -1;
     if (lstm_gather(hout, xp, hprev, gates, T, B, st)) return -1;
     for (int dir = 0; dir < 2; ++dir) {
@@ -795,8 +804,9 @@ int hn_lstm_layer_backward(const float* xp, const float* hout, const float* whf,
         if (conv_f32(g, a, o, o.p, st)) return -1;
     }
     if (lstm_cell_scan(gates, cell, T, B, st)) return -1;
-    // the unit test covers the one-launch-per-step kernel; the cooperative one is covered by the whole-step tests
-    return lstm_bwd_steps(dout, gates, cell, wt, wt + (size_t)512 * 2048, dgates, dc, T, B, nullptr, nullptr, st);
+    // persistent: the cooperative kernel the training step launches (checked above to fit, so lstm_bwd_steps takes it)
+    return lstm_bwd_steps(dout, gates, cell, wt, wt + (size_t)512 * 2048, dgates, dc, T, B, persistent ? barrier : nullptr,
+                          persistent ? error_flag : nullptr, st);
 }
 
 }  // extern "C"

@@ -271,8 +271,15 @@ int hn_bn_forward_backward(const float* z, int B, int H, int W, int C, const flo
                            float* running_mean, float* running_var, double factor, int train, int relu, const float* res,
                            float* y, const float* dy, float* dz, float* dres, float* dgamma, float* dbeta, float* bn_scratch,
                            double* sums, void* stream);
+/* One bidirectional LSTM layer's gate gradients from its saved forward tensors: xp [T][B][4096] (input projection + biases),
+ * hout [T][B][1024], whf / whb: W_hh [2048][512] per direction, dout [T][B][1024] -> dgates [2][T][B][2048] (d xp).
+ * persistent = 0: BPTT as one launch per time step; 1: the single cooperative launch the training step makes (staged dG in
+ * shared memory for B <= 16), or -1 with "not supported" when the device cannot co-schedule its 128 CTAs (no fallback).
+ * scratch, in 4-byte words, with R = T*B: hprev 2*R*512 | gates 2*R*2048 | cell 2*R*512 | dc carry 2*B*512 |
+ * W_hh^T 2*512*2048 | ones 4096 | zeros 4096 | barrier counter (uint) | error flag (int; zeroed here before a persistent launch,
+ * 1 after a grid-barrier time-out). */
 int hn_lstm_layer_backward(const float* xp, const float* hout, const float* whf, const float* whb, const float* dout, int T,
-                           int B, float* dgates, float* scratch, void* stream);
+                           int B, int persistent, float* dgates, float* scratch, void* stream);
 
 /* One bidirectional LSTM layer recurrence: xproj [T][B][4096] (input projection + both biases,
  * column = dir*2048 + gate*512 + unit), w_hh_* [2048][512] (PyTorch layout), out [T][B][1024]. */

@@ -3,6 +3,7 @@ golden fixtures (minted from the real reference) and size-independent properties
 
 Tolerances: forward outputs 1e-4 max-abs (BASELINE north_star), kernel unit tests relative to the
 output scale; pano_stretch 1.2e-7 (one fp32 ulp in [0,1): 'pixel-exact to bilinear rounding')."""
+import ctypes
 import os
 import numpy as np
 import pytest
@@ -657,7 +658,16 @@ WGRAD_TC_CASES = [
     (5, 64, 2, 16, 128, 3, (2, 1)),        # W = 16: four images per tile, B = 5
     (2, 1024, 4, 32, 512, 3, (2, 1)),      # ghc_lst.3.layer.2: 8 x 4 channel tiles, 9 taps
     (4, 128, 32, 64, 128, 3, (1, 1)),      # 8192 pixels = 128 tiles: more than one pixel slice per work item
+    # the weight gradients of the LSTM and of the MLP head as the training step runs them: GEMM rows, one row of
+    # W = 256 * batch pixels, k = 1 (the training step passes halo-0 rows; this entry point takes halo 1)
+    (1, 1024, 1, 2048, 2048, 1, (1, 1)),   # bi_rnn.weight_ih at batch 8
+    (1, 512, 1, 2048, 2048, 1, (1, 1)),    # bi_rnn.weight_hh at batch 8: pixel slices reduced with red.global.add
+    (1, 512, 1, 4352, 2048, 1, (1, 1)),    # bi_rnn.weight_hh at batch 17
+    (1, 1024, 1, 2048, 512, 1, (1, 1)),    # MLP head W1 at batch 8: pixel slices
 ]
+# cases that must stay split along the pixel axis on an H100, so that the slice reduction stays under test
+WGRAD_TC_MULTI_SLICE = {(1, 512, 1, 2048, 2048, 1, (1, 1)), (1, 1024, 1, 2048, 512, 1, (1, 1)),
+                        (1, 512, 1, 4352, 2048, 1, (1, 1))}
 
 
 @pytest.mark.parametrize('case', WGRAD_TC_CASES)
@@ -665,6 +675,12 @@ def test_conv_wgrad_tc_vs_autograd(case):
     """Weight gradient on the tensor-core kernel (wgrad_tc.cu: pixel-axis GEMM over MN-major plane tiles) against
     torch.autograd in fp64, and against the fp32 CUDA-core kernel on the same inputs."""
     B, Ci, H, W, Co, k, stride = case
+    plan = (ctypes.c_int * 10)()
+    _lib.check(_lib.lib().hn_wgrad_tc_plan(B, H, W, Ci, Co, k, k, stride[0], stride[1], k // 2, k // 2, gu.device_sms(),
+                                           plan), 'hn_wgrad_tc_plan')
+    slices = plan[7]
+    if case in WGRAD_TC_MULTI_SLICE:
+        assert slices > 1, f'planned as {slices} pixel slice(s) on {gu.device_sms()} SMs'
     g = torch.Generator().manual_seed(hash(case) % (2 ** 31))
     x = torch.randn(B, Ci, H, W, generator=g)
     p = k // 2
@@ -690,7 +706,8 @@ def test_conv_wgrad_tc_vs_autograd(case):
     scale = ref.abs().max().item()
     err = (dw.cpu().double() - ref).abs().max().item() / scale
     err32 = (dw32.cpu().double() - ref).abs().max().item() / scale
-    gu.record('wgrad_tc_errors.jsonl', {'case': list(case[:6]) + list(stride), 'err_tc': err, 'err_fp32': err32})
+    gu.record('wgrad_tc_errors.jsonl', {'case': list(case[:6]) + list(stride), 'slices': slices, 'err_tc': err,
+                                        'err_fp32': err32})
     assert err <= 2e-5, (err, err32)
 
 
@@ -774,47 +791,125 @@ def test_batchnorm_forward_backward_vs_autograd(train, relu, res, shape):
         assert torch.equal(rmt.cpu(), rm) and torch.equal(rvt.cpu(), rv)
 
 
-@pytest.mark.parametrize('T,B', [(6, 2), (9, 11)])
-def test_lstm_layer_backward_vs_autograd(T, B):
-    """Gate gradients of one bidirectional layer (recompute of the gates from the saved outputs, cell scan, one launch
-    per time step) against autograd through the oracle's LSTM."""
-    g = torch.Generator().manual_seed(T * 100 + B)
-    x = torch.randn(T, B, 1024, generator=g) * 0.5
-    ws = {}
-    for sfx in ('', '_reverse'):
-        ws['ih' + sfx] = (torch.randn(2048, 1024, generator=g) / 32)
-        ws['hh' + sfx] = (torch.randn(2048, 512, generator=g) / 22)
-        ws['b' + sfx] = torch.randn(2048, generator=g) * 0.1
-    xps, outs = [], []
-    for sfx, rev in (('', False), ('_reverse', True)):
-        xp = (x.double() @ ws['ih' + sfx].double().t() + ws['b' + sfx].double()).requires_grad_()
-        xps.append(xp)
-        # the oracle's recurrence with the input projection made explicit (so that d xp is observable)
+def _bilstm_fp64(xp, whh):
+    """The oracle's bidirectional recurrence with the input projection made explicit (so that d xp is observable):
+    xp [T][B][4096] -> (leaf xp per direction [T][B][2048], hout [T][B][1024]), in fp64."""
+    T, B = xp.shape[:2]
+    xps = [xp[..., :2048].double().clone().requires_grad_(), xp[..., 2048:].double().clone().requires_grad_()]
+    outs = []
+    for d, rev in ((0, False), (1, True)):
         h = torch.zeros(B, 512, dtype=torch.float64)
         c = torch.zeros(B, 512, dtype=torch.float64)
         out = [None] * T
         for t in (range(T - 1, -1, -1) if rev else range(T)):
-            gt = xp[t] + h @ ws['hh' + sfx].double().t()
+            gt = xps[d][t] + h @ whh[d].double().t()
             i, f, gg, o = gt.chunk(4, dim=1)
             c = torch.sigmoid(f) * c + torch.sigmoid(i) * torch.tanh(gg)
             h = torch.sigmoid(o) * torch.tanh(c)
             out[t] = h
         outs.append(torch.stack(out))
-    hout = torch.cat(outs, dim=2)
-    dout = torch.randn(T, B, 1024, generator=g)
-    hout.backward(dout.double())
-    xp_all = torch.cat([xps[0].detach(), xps[1].detach()], dim=2).float().contiguous().to(DEV)
+    return xps, torch.cat(outs, dim=2)
+
+
+# T = 256 (the sequence length of the model) at the batch sizes where the BPTT kernels change shape: the staged cooperative
+# kernel (B <= 16; B = 8 is the benchmark's training batch, 9 a partial 8-column group, 16 the largest staged dG, 128 KB of
+# shared memory), the unstaged one (17, 32).  T = 1: no grid barrier; T = 2, 3: first and last step of a direction meet.
+LSTM_BWD_CASES = [(6, 2), (9, 11)] + [(256, B) for B in (1, 2, 8, 9, 16, 17, 32)] + [(T, B) for T in (1, 2, 3) for B in (5, 17)]
+LSTM_BWD_RELAUNCH = {(256, 8), (256, 17)}          # one case per cooperative variant (staged, unstaged)
+LSTM_BWD_DENSE_BOUND = 5e-5                        # max |err| / max |ref| over a direction (worst measured: 3.1e-7)
+# max |err[t]| / max |ref[t]| per time step; ~4x the worst ratio measured on an H100 SXM (700 W), 1.97e-6 at T = 256, B = 1
+LSTM_BWD_IMPULSE_BOUND = 8e-6
+
+
+@pytest.mark.parametrize('T,B', LSTM_BWD_CASES)
+def test_lstm_layer_backward_vs_autograd(T, B):
+    """Gate gradients of one bidirectional layer (recompute of the gates from the saved outputs, cell scan, BPTT) against
+    autograd through the oracle's LSTM in fp64, with both BPTT kernels on the same inputs: one launch per time step
+    (persistent = 0) and the single cooperative launch the training step makes (persistent = 1, staged for B <= 16).
+    dout patterns: dense (random at every step), and an impulse at the first step each direction processes, with the
+    forget gates biased to ~0.95 so that every later step's dG is pure propagation through the dc carry and the previous
+    step's dG, checked step by step.  Both kernels share lane order, fmaf chain, shuffle tree and cell expressions, so
+    their dgates must agree bit for bit."""
+    g = torch.Generator().manual_seed(T * 100 + B)
+    k = 512 ** -0.5                                                      # nn.LSTM's init: U(-1/sqrt(hidden), 1/sqrt(hidden))
+    uni = lambda *shape: (torch.rand(*shape, generator=g, dtype=torch.float64) * 2 - 1) * k
+    x = torch.randn(T, B, 1024, generator=g, dtype=torch.float64) * 0.5
+    w_ih = [uni(2048, 1024) for _ in range(2)]
+    whh = [uni(2048, 512).float() for _ in range(2)]
+    bias = [uni(2048) + uni(2048) for _ in range(2)]                     # b_ih + b_hh
+    xp_dense = torch.cat([x @ w_ih[d].t() + bias[d] for d in range(2)], dim=2).float()
+    xp_imp = xp_dense.clone()
+    xp_imp.view(T, B, 2, 4, 512)[:, :, :, 1] += 3.0                      # forget gates: sigmoid ~ 0.95
+    dout_dense = torch.randn(T, B, 1024, generator=g)
+    dout_imp = torch.zeros(T, B, 1024)
+    dout_imp[T - 1, :, :512] = torch.randn(B, 512, generator=g)         # forward direction starts its backward at T-1
+    dout_imp[0, :, 512:] = torch.randn(B, 512, generator=g)             # the reverse direction at 0
+
+    lib, st = _lib.lib(), torch.cuda.current_stream().cuda_stream
     rows = T * B
-    scratch = torch.empty(2 * rows * 512 * 2 + 2 * rows * 2048 + 2 * B * 512 + 2 * 512 * 2048 + 8192, device=DEV)
-    dg = torch.full((2, T, B, 2048), float('nan'), device=DEV)
-    hout_d, whf, whb, dout_d = (t.detach().float().contiguous().to(DEV) for t in (hout, ws['hh'], ws['hh_reverse'], dout))
-    _lib.check(_lib.lib().hn_lstm_layer_backward(
-        xp_all.data_ptr(), hout_d.data_ptr(), whf.data_ptr(), whb.data_ptr(), dout_d.data_ptr(), T, B, dg.data_ptr(),
-        scratch.data_ptr(), torch.cuda.current_stream().cuda_stream), 'hn_lstm_layer_backward')
-    torch.cuda.synchronize()
-    for d in range(2):
-        ref = xps[d].grad
-        assert (dg[d].cpu().double() - ref).abs().max().item() <= 5e-5 * ref.abs().max().item(), d
+    n_scratch = 2 * rows * 512 * 2 + 2 * rows * 2048 + 2 * B * 512 + 2 * 512 * 2048 + 8192 + 2
+    scratch = torch.empty(n_scratch, device=DEV)
+    words = scratch[-2:].view(torch.int32)                               # barrier counter, error flag
+    whf, whb = (w.contiguous().to(DEV) for w in whh)
+
+    def run(xp_d, hout_d, dout_d, persistent):
+        words.fill_(-1)
+        dg = torch.full((2, T, B, 2048), float('nan'), device=DEV)
+        rc = lib.hn_lstm_layer_backward(xp_d.data_ptr(), hout_d.data_ptr(), whf.data_ptr(), whb.data_ptr(),
+                                        dout_d.data_ptr(), T, B, persistent, dg.data_ptr(), scratch.data_ptr(), st)
+        if rc != 0:
+            return lib.hn_last_error().decode('utf-8', 'replace'), None
+        torch.cuda.synchronize()
+        barrier, flag = words.tolist()
+        if persistent:
+            assert flag == 0, 'the grid barrier timed out'
+            assert barrier == (T - 1) * 128, barrier                     # every CTA arrived once between each two steps
+        else:
+            assert [barrier, flag] == [-1, -1], 'the per-step kernels touched the barrier words'
+        return None, dg
+
+    refused = None
+    for pattern, xp, dout in (('dense', xp_dense, dout_dense), ('impulse', xp_imp, dout_imp)):
+        xps, hout = _bilstm_fp64(xp, whh)
+        ref = torch.autograd.grad(hout, xps, dout.double())
+        xp_d, hout_d, dout_d = (t.float().contiguous().to(DEV) for t in (xp, hout.detach(), dout))
+        err, dg_step = run(xp_d, hout_d, dout_d, 0)
+        assert err is None, err
+        got = {'step': dg_step}
+        if refused is None:
+            refused, dg_coop = run(xp_d, hout_d, dout_d, 1)
+            if refused is not None:
+                assert 'not supported' in refused, refused
+                assert gu.device_sms() < 128, f'cooperative BPTT kernel refused on a {gu.device_sms()}-SM device: {refused}'
+            else:
+                got['coop'] = dg_coop
+        for d in range(2):
+            r = ref[d]
+            for kern, gd in got.items():
+                diff = (gd[d].cpu().double() - r).abs()
+                if pattern == 'dense':
+                    ratio = diff.max().item() / r.abs().max().item()
+                    gu.record('lstm_bwd_errors.jsonl', {'T': T, 'B': B, 'pattern': pattern, 'dir': d, 'kernel': kern,
+                                                        'ratio': ratio})
+                    assert ratio <= LSTM_BWD_DENSE_BOUND, (pattern, d, kern, ratio)
+                else:
+                    # every step on its own: its dG is propagated from the impulse, a wrong step cannot hide under others
+                    scale = r.abs().flatten(1).max(dim=1).values
+                    assert bool((scale > 1e-30).all()), 'the impulse does not reach every step'
+                    per_t = diff.flatten(1).max(dim=1).values / scale
+                    worst = int(per_t.argmax())
+                    gu.record('lstm_bwd_errors.jsonl', {'T': T, 'B': B, 'pattern': pattern, 'dir': d, 'kernel': kern,
+                                                        'ratio': per_t[worst].item(), 'at_t': worst,
+                                                        'min_scale': scale.min().item()})
+                    assert per_t[worst].item() <= LSTM_BWD_IMPULSE_BOUND, (pattern, d, kern, worst, per_t[worst].item())
+        if 'coop' in got:
+            assert torch.equal(got['coop'], dg_step), f'{pattern}: cooperative and per-step kernels differ'
+            if (T, B) in LSTM_BWD_RELAUNCH and pattern == 'dense':
+                err, again = run(xp_d, hout_d, dout_d, 1)                 # same scratch: the barrier must be re-armed
+                assert err is None, err
+                assert torch.equal(again, got['coop']), 'second cooperative launch on the same scratch differs'
+    if refused is not None:
+        pytest.skip(f'cooperative BPTT kernel not run on this {gu.device_sms()}-SM device: {refused}')
 
 
 @pytest.mark.parametrize('tensor_cores,wgrad_tc', [(True, '1'), (True, '0'), (False, '0')])
