@@ -1,11 +1,10 @@
 // Bidirectional LSTM recurrence on thread-block clusters (reference model.py:222-227 nn.LSTM, h0 = c0 = 0,
 // gate order i,f,g,o; c' = s(f)c + s(i)tanh(g), h' = s(o)tanh(c')).
 //
-// lstm.cu spreads one direction over 64 CTAs that exchange h_t through L2 every step; ncu and the step time
-// (4.9 us, independent of how many sub-batches are pipelined) show that the store -> fence -> flag -> poll -> TMA
-// chain through L2 is the whole cost.  Here one CLUSTER of 16 CTAs owns (direction, 8 batch columns) completely,
-// so the per-step all-to-all stays inside the cluster's distributed shared memory (~0.1 us latency) and clusters
-// never talk to each other:
+// Every step needs h_{t-1} of all 512 units.  Exchanged through L2 between CTAs, the store -> fence -> flag -> poll ->
+// TMA chain costs about 4.9 us per step and is the whole step time (ncu).  Here one CLUSTER of 16 CTAs owns
+// (direction, 8 batch columns) completely, so the per-step all-to-all stays inside the cluster's distributed shared
+// memory (~0.1 us latency) and clusters never talk to each other:
 //   cluster = 16 CTAs x 32 hidden units;  CTA = 32 units x 4 gates = 128 rows of W_hh
 //   W_hh    = fp16 hi plane as mma.sync A fragments in REGISTERS (128 per thread) for the whole sequence,
 //             fp16 lo plane as ready-made fragments in SHARED MEMORY (128 KB, written once, read back 32 registers
@@ -23,7 +22,7 @@
 //   groups  = one or two column groups of 8 per cluster, interleaved step by step (each group has its own exchange
 //             buffers and barriers): while one group's h is in flight between the CTAs the other group's MMAs run.
 //             Two groups per cluster when one group each would not fit in one wave of co-resident clusters (see
-//             lstm_layer_cluster): the batch-32 recurrence then takes 4 clusters = 64 of the 132 SMs and leaves the
+//             lstm_layer): the batch-32 recurrence then takes 4 clusters = 64 of the 132 SMs and leaves the
 //             rest to the next batch's encoder.  Clusters beyond what the device co-schedules run in a later wave.
 //   grid    = 2 directions x ceil(B/8) clusters, or 2 directions x ceil(B/16) with two groups per cluster.
 #include <cuda_fp16.h>
@@ -287,17 +286,20 @@ __global__ void __launch_bounds__(NT, 1) lstm_cluster_kernel(const ClArgs a) {
 
 }  // namespace
 
-// One LSTM layer, both directions, on 16-CTA clusters.  Returns 0 on success, 1 when the device cannot co-schedule
-// such clusters (the caller then uses the L2-exchange kernel of lstm.cu), -1 on error.
-int lstm_layer_cluster(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, float* out, int T, int B,
-                       cudaStream_t st) {
+// One LSTM layer, both directions, on 16-CTA clusters; xproj [T][B][4096], out [T][B][1024].  Returns 0 on success,
+// -1 on error, including a device that cannot co-schedule two such clusters.
+int lstm_layer(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, float* out, int T, int B,
+               cudaStream_t st) {
     // function attributes are per device: set them on every call (cheap); the occupancy answer is cached per device
     int dev = 0;
     HN_CUDA_OK(cudaGetDevice(&dev));
-    const bool attr_ok =
-        cudaFuncSetAttribute(lstm_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL) == cudaSuccess &&
-        cudaFuncSetAttribute(lstm_cluster_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
-    if (!attr_ok) { (void)cudaGetLastError(); return 1; }
+    cudaError_t e = cudaFuncSetAttribute(lstm_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(lstm_cluster_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        return fail("lstm_layer: the 16-CTA recurrence clusters are not supported on device " + std::to_string(dev) + ": " +
+                    cudaGetErrorString(e));
+    }
     static int cached[64];
     static bool cached_init = false;
     if (!cached_init) { for (int i = 0; i < 64; ++i) cached[i] = -1; cached_init = true; }
@@ -319,14 +321,16 @@ int lstm_layer_cluster(const float* xproj, const float* w_hh_fwd, const float* w
         if (const char* e = getenv("HN_LSTM_VERBOSE"))
             if (atoi(e)) fprintf(stderr, "lstm_cluster: device %d: max active 16-CTA clusters = %d\n", dev, max_clusters);
     }
-    if (max_clusters < 2) return 1;
+    if (max_clusters < 2)
+        return fail("lstm_layer: not supported on device " + std::to_string(dev) + ": it co-schedules " +
+                    std::to_string(max_clusters) + " of the recurrence's 16-CTA clusters, 2 are needed");
     ClArgs a;
     a.xproj = xproj; a.w_hh[0] = w_hh_fwd; a.w_hh[1] = w_hh_bwd; a.out = out;
     a.T = T; a.B = B; a.ngroups = (B + NCOL - 1) / NCOL;
-    // One group per cluster when every cluster fits in one wave: a second group makes a cluster about 1.5x slower
-    // (T = 256 on an H100 at 400 W: 2 clusters 1.46 ms with one group each, 2.19 ms with two).  Two groups per
-    // cluster when one group each would need a second wave: batch 32 on the 7 co-resident clusters of that H100 runs
-    // in 2.15 ms on 4 clusters instead of 3.07 ms in two waves, and leaves 68 SMs to the other stream.
+    // One group per cluster when every cluster fits in one wave: a second group makes a cluster about 1.7x slower
+    // (T = 256, kernel time on an H100 at 700 W: 0.71 ms with one group per cluster, 1.20 ms with two).  Two groups
+    // per cluster when one group each would need a second wave: batch 32 on the 7 co-resident clusters of that H100
+    // then runs on 4 clusters in one wave instead of 8 in two, and leaves 68 SMs to the other stream.
     a.gpc = (2 * a.ngroups <= max_clusters) ? 1 : MAXG;
     const int nclusters = 2 * ((a.ngroups + a.gpc - 1) / a.gpc);
     cudaLaunchConfig_t cfg = {};

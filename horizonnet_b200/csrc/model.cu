@@ -337,7 +337,6 @@ int hn_model_create_head(int device, int max_batch, int use_rnn, hn_model** out)
         };
         for (auto& b : rnn_bufs)
             if (m->alloc_t(b.p, b.n)) return -1;
-        if (m->alloc(reinterpret_cast<void**>(&m->counters), lstm_scratch_bytes())) return -1;
     }
     if (m->alloc_t(&m->error_flag, 1)) return -1;
     if (m->alloc_t(&m->tta_ints, 128)) return -1;
@@ -621,9 +620,7 @@ static int forward_rnn(hn_model* m, int B, float* bon, float* cor, cudaStream_t 
         if (run_conv(m, m->xproj[layer], a, xp, nullptr, st, CLS_XPROJ, true)) return -1;
         {
             Scope sc(m, CLS_LSTM, 2.0 * 256 * B * 2 * 2048 * 512, st);
-            if (lstm_layer(m->XP, m->whh[layer][0], m->whh[layer][1], louts[layer], 256, B, m->counters,
-                           m->error_flag, st))
-                return -1;
+            if (lstm_layer(m->XP, m->whh[layer][0], m->whh[layer][1], louts[layer], 256, B, st)) return -1;
         }
         lin = louts[layer];
     }
@@ -787,7 +784,7 @@ int hn_model_profile_read(hn_model* m, double* ms, double* flops, long long* lau
 }
 
 int hn_model_check(hn_model* m) {
-    // surfaces device-side failures (LSTM spin timeout) after a synchronisation point
+    // surfaces device-side failures (grid-barrier time-out of the cooperative BPTT kernel) after a synchronisation point
     HN_CHECK(m, "hn_model_check: NULL model");
     HN_ON_DEVICE(m->device);
     int flag = 0;
@@ -1102,22 +1099,7 @@ int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh,
 
 int hn_lstm_layer(const float* xproj, const float* whf, const float* whb, float* out, int T, int B, void* stream) {
     HN_CHECK(xproj && whf && whb && out && T >= 1 && B >= 1, "hn_lstm_layer: bad argument");
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned int* ctr = nullptr;
-    HN_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&ctr), lstm_scratch_bytes()));
-    int* flag = reinterpret_cast<int*>(ctr + 64);   // counters live in [0, 8), the error flag behind them (first KB of scratch)
-    cudaMemsetAsync(ctr, 0, 1024, st);
-    int rc = lstm_layer(xproj, whf, whb, out, T, B, ctr, flag, st);
-    int h = 0;
-    if (!rc) {
-        if (cudaStreamSynchronize(st) != cudaSuccess) rc = fail("hn_lstm_layer: kernel failed");
-        else {
-            cudaMemcpy(&h, flag, sizeof(int), cudaMemcpyDeviceToHost);
-            if (h) rc = fail("hn_lstm_layer: persistent kernel timed out waiting for a peer CTA");
-        }
-    }
-    cudaFree(ctr);
-    return rc;
+    return lstm_layer(xproj, whf, whb, out, T, B, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -18,8 +18,7 @@ int ghc_to_sequence(const Act ghc[4], float* seq, cudaStream_t st, bool split);
 int linear_head(const float* rnn, const float* w, const float* bias, float* bon, float* cor, int T, int B, int K,
                 cudaStream_t st);
 int lstm_layer(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, float* out, int T, int B,
-               void* scratch, int* error_flag, cudaStream_t st);
-size_t lstm_scratch_bytes();
+               cudaStream_t st);
 int tta_views(const float* x, float* views, int V, const int* modes_dev, const int* shifts_dev, cudaStream_t st);
 int tta_merge(const float* bon, const float* cor, int V, const int* modes_dev, const int* shifts_dev, float* y_bon,
               float* y_cor, cudaStream_t st);
@@ -123,8 +122,7 @@ struct hn_model {
     float* GO[4] = {nullptr, nullptr, nullptr, nullptr};
     float *SEQ = nullptr, *XP = nullptr, *R1 = nullptr, *R2 = nullptr, *R1S = nullptr;
     float *HID = nullptr, *HIDD = nullptr;           // MLP head: hidden layer [T][B][512] after ReLU, and after dropout
-    unsigned int* counters = nullptr;
-    int* error_flag = nullptr;
+    int* error_flag = nullptr;                       // set by a grid-barrier time-out of the cooperative BPTT kernel
     float *x_in = nullptr, *bon_out = nullptr, *cor_out = nullptr;    // for forward_host
     // pipelined host API: 2 input slots, a copy stream and a compute stream (H2D of batch i+1 overlaps forward i)
     float* x_slot[2] = {nullptr, nullptr};

@@ -238,9 +238,7 @@ int walk_forward(hn_model* m, TrainState* ts, const float* x, int B, int in_chan
         Act a = mk(const_cast<float*>(lin), 1, 1, T_STEPS * B, 1024, 0);
         Act xp = mk(ts->xp[layer], 1, 1, T_STEPS * B, 4096, 0);
         if (conv_f32(m->xproj[layer].d, a, xp, nullptr, st)) return -1;
-        if (lstm_layer(ts->xp[layer], m->whh[layer][0], m->whh[layer][1], ts->r[layer], T_STEPS, B, m->counters,
-                       m->error_flag, st))
-            return -1;
+        if (lstm_layer(ts->xp[layer], m->whh[layer][0], m->whh[layer][1], ts->r[layer], T_STEPS, B, st)) return -1;
         // the un-dropped outputs stay on the tape (the backward recomputes the gates from them); rm = what the next
         // consumer sees
         HN_CUDA_OK(cudaMemcpyAsync(ts->rm[layer], ts->r[layer], nseq * sizeof(float), cudaMemcpyDeviceToDevice, st));

@@ -182,7 +182,7 @@ int hn_model_set_option(hn_model* m, const char* name, int value);
 int hn_model_profile_read(hn_model* m, double* ms, double* flops, long long* launches, int reset);
 
 /* Synchronises the device and reports device-side failures recorded by earlier asynchronous
- * forwards (e.g. the persistent LSTM kernel's peer-wait timeout). */
+ * calls (the grid-barrier time-out of the training backward's cooperative LSTM BPTT kernel). */
 int hn_model_check(hn_model* m);
 
 void hn_model_destroy(hn_model* m);
@@ -282,7 +282,9 @@ int hn_lstm_layer_backward(const float* xp, const float* hout, const float* whf,
                            int B, int persistent, float* dgates, float* scratch, void* stream);
 
 /* One bidirectional LSTM layer recurrence: xproj [T][B][4096] (input projection + both biases,
- * column = dir*2048 + gate*512 + unit), w_hh_* [2048][512] (PyTorch layout), out [T][B][1024]. */
+ * column = dir*2048 + gate*512 + unit), w_hh_* [2048][512] (PyTorch layout), out [T][B][1024].
+ * Asynchronous on `stream`, like hn_conv2d; fails with "not supported" on a device that cannot
+ * co-schedule two of the recurrence's 16-CTA clusters. */
 int hn_lstm_layer(const float* xproj_dev, const float* w_hh_fwd_dev, const float* w_hh_bwd_dev,
                   float* out_dev, int T, int B, void* stream);
 

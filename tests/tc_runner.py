@@ -1,8 +1,7 @@
-"""Runs unit cases of tests/tc_cases.py (or LSTM layers) in a fresh process, so that the HN_TC_* / HN_LSTM_CLUSTER switches,
-which the library reads once per process, take effect.  Prints one JSON line per case.
+"""Runs unit cases of tests/tc_cases.py in a fresh process, so that the HN_TC_* switches, which the library reads once per
+process, take effect.  Prints one JSON line per case.  Also holds the LSTM layer check the GPU tests share.
 
-    python tests/tc_runner.py conv NAME...        -> {"name", "ratio", "plan"}
-    python tests/tc_runner.py lstm T,B...         -> {"name", "err"}"""
+    python tests/tc_runner.py conv NAME...        -> {"name", "ratio", "plan"}"""
 import json
 import os
 import sys
@@ -56,13 +55,10 @@ def main(argv):
     entry.build()
     kind, names = argv[0], argv[1:]
     cases = {c['name']: c for c in tc_cases.ALL_CASES}
+    assert kind == 'conv', kind
     for n in names:
-        if kind == 'conv':
-            c = cases[n]
-            print(json.dumps({'name': n, 'ratio': gu.run_tc_case(c), 'plan': tc_cases.plan(c, gu.device_sms())}), flush=True)
-        else:
-            T, B = (int(v) for v in n.split(','))
-            print(json.dumps({'name': n, 'err': lstm_error(T, B)}), flush=True)
+        c = cases[n]
+        print(json.dumps({'name': n, 'ratio': gu.run_tc_case(c), 'plan': tc_cases.plan(c, gu.device_sms())}), flush=True)
 
 
 if __name__ == '__main__':

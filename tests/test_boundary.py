@@ -223,6 +223,6 @@ def test_every_environment_switch_of_the_library_is_documented():
         src = open(f).read()
         names |= set(re.findall(r'getenv\("(HN_[A-Z0-9_]+)"\)', src)) | set(re.findall(r"environ\.get\('(HN_[A-Z0-9_]+)'", src))
     doc = open(os.path.join(root, 'INTEGRATION.md')).read()
-    assert len(names) >= 9
+    assert len(names) >= 8
     missing = sorted(n for n in names if n not in doc)
     assert not missing, missing

@@ -85,7 +85,8 @@ def test_conv_kernel_vs_torch(case, impl):
 @pytest.mark.parametrize('T,B', [(5, 1), (24, 7), (16, 32), (12, 40), (256, 1), (256, 32)])
 def test_lstm_layer_vs_oracle(T, B):
     """One bidirectional layer against an fp64 recurrence of the same input projection, up to the model's T = 256;
-    B = 40 takes two batch-chunk launches.  tc_runner.lstm_error also runs the cooperative kernel (test_tc_kernels.py)."""
+    B = 7 leaves part of an 8-column group empty, and B = 32 and 40 take two column groups per cluster on a card that
+    co-schedules fewer than 8 of the 16-CTA clusters."""
     from tc_runner import lstm_error
     err = lstm_error(T, B, DEV)
     gu.record('lstm_errors.jsonl', {'T': T, 'B': B, 'err': err})

@@ -6,7 +6,8 @@
 - The persistent tensor-core kernels claim their tiles from a per-stream counter at run time; which CTA computes a
   tile must not change it, whether the launch runs alone, next to a recurrence, next to another launch, or right
   after itself under programmatic dependent launch.
-- The pipelined forward (encoder and recurrence on two streams) must equal the plain forward bit for bit."""
+- The pipelined forward (encoder and recurrence on two streams) must equal the plain forward bit for bit.
+- hn_lstm_layer only enqueues the recurrence, so a convolution launched after it on another stream runs beside it."""
 import pytest
 import torch
 
@@ -37,10 +38,25 @@ def _lstm_inputs(T, B, seed):
 def _lstm(xproj_dev, w0, w1, stream=None):
     T, B = xproj_dev.shape[:2]
     out = torch.full((T, B, 1024), float('nan'), device=DEV)
-    st = (stream or torch.cuda.current_stream()).cuda_stream
-    _lib.check(_lib.lib().hn_lstm_layer(xproj_dev.data_ptr(), w0.data_ptr(), w1.data_ptr(), out.data_ptr(), T, B, st),
-               'hn_lstm_layer')
+    stream = stream or torch.cuda.current_stream()
+    stream.wait_stream(torch.cuda.current_stream())        # the call only enqueues: the NaN fill must come first
+    _lib.check(_lib.lib().hn_lstm_layer(xproj_dev.data_ptr(), w0.data_ptr(), w1.data_ptr(), out.data_ptr(), T, B,
+                                        stream.cuda_stream), 'hn_lstm_layer')
     return out
+
+
+def test_lstm_layer_returns_before_the_recurrence_runs():
+    xproj, whh = _lstm_inputs(256, 32, 9)
+    xd, w0, w1 = xproj.to(DEV), whh[0].to(DEV), whh[1].to(DEV)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        torch.cuda._sleep(100_000_000)                      # about 50 ms at the H100's 1980 MHz
+    h = _lstm(xd, w0, w1, s)
+    busy = not s.query()
+    s.synchronize()
+    assert busy, 'hn_lstm_layer returned only after its stream had drained'
+    assert torch.equal(h, _lstm(xd, w0, w1))
 
 
 @pytest.mark.parametrize('B', [16, 24, 32, 40])

@@ -5,8 +5,8 @@
   gpu_utils.run_tc_case: NaN-filled output that must be written everywhere, circular halo columns, a canary behind the
   output;
 * the tensor-core data gradient of the training step (hn_conv2d_dgrad_tc) against torch.autograd in fp64;
-* the HN_TC_* switches that select other code paths, and the cooperative LSTM kernel (HN_LSTM_CLUSTER=0), each in a fresh
-  process (tests/tc_runner.py), since the library reads them once per process.
+* the HN_TC_* switches that select other code paths, each in a fresh process (tests/tc_runner.py), since the library reads
+  them once per process.
 Worst err / bound per case and variant key go to $HN_TEST_RECORD_DIR/tc_errors.jsonl when that variable is set
 (gpu_utils.record)."""
 import json
@@ -115,12 +115,3 @@ def test_switched_off_paths_stay_inside_the_bound():
             gu.record('tc_errors.jsonl', {'test': 'switch', 'switch': sw, 'case': n, 'ratio': r['ratio']})
             assert r['ratio'] <= 1.0, (sw, n, r['ratio'])
             assert base[n]['plan'][field] and not r['plan'][field], (sw, n)           # the switch took the other path
-
-
-def test_cooperative_lstm_kernel_vs_fp64():
-    """HN_LSTM_CLUSTER=0: the cooperative L2-exchange kernel, also the fallback when two 16-CTA clusters cannot be
-    co-scheduled; the model's T = 256, and B = 40 for two batch-chunk launches."""
-    got = _run('lstm', ['256,1', '256,32', '12,40', '256,40'], {'HN_LSTM_CLUSTER': '0'})
-    for n, r in got.items():
-        gu.record('tc_errors.jsonl', {'test': 'lstm_coop', 'case': n, 'err': r['err']})
-    assert len(got) == 4 and all(r['err'] < 2e-6 for r in got.values()), got
