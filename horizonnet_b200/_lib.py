@@ -48,6 +48,9 @@ SIGNATURES = {
     'hn_wgrad_tc_plan': (ctypes.c_int, [ctypes.c_int] * 12 + [c_int_p]),
     'hn_conv2d_dgrad_tc': (ctypes.c_int, [ctypes.c_int] * 4 + [vp, vp] + [ctypes.c_int] * 7 + [vp, vp]),
     'hn_conv_tc_plan': (ctypes.c_int, [ctypes.c_int] * 16 + [c_int_p]),
+    'hn_conv_tc_fold_plan': (ctypes.c_int, [ctypes.c_int] * 8 + [c_int_p]),
+    'hn_conv_tc_fold': (ctypes.c_int, [vp, vp] + [ctypes.c_int] * 7 + [vp, vp, vp, vp]),
+    'hn_bott_tc_fold': (ctypes.c_int, [vp, vp] + [ctypes.c_int] * 3 + [vp] * 5 + [ctypes.c_int, vp, vp]),
     'hn_wgrad_tc_enabled': (ctypes.c_int, []),
     'hn_bn_forward_backward': (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp,
                                               ctypes.c_double, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp,

@@ -22,6 +22,8 @@
 //              3-stage mbarrier ring of 64 KB stages (4 stages of 48 KB for BN <= 64).  After a tile's last K chunk it
 //              claims the next stage as the tile's epilogue slot (one stage holds exactly one output tile, BM x BN x 4 B)
 //              and TMA-loads the residual tile into it, so the residual lands while the last chunks compute.
+//              A block-0 conv3 with its downsample folded in reads two A sources: its K chunks over t2, then its K
+//              chunks over the block input x (1x1, stride 1 or 2 through the parity view), each as the same 128-pixel box.
 //              "dxr" mode (3x3, one 128-pixel row per tile): one 130-pixel box per (dy, chunk) feeds all three dx taps
 //              through wgmma descriptors whose start address is shifted by dx rows (the swizzle is a function of the
 //              absolute shared-memory address), so each input row crosses L2 -> SM once instead of three times.  The
@@ -41,6 +43,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <vector>
 
 #include "hn_common.cuh"
 #include "conv_tc.cuh"
@@ -68,6 +71,10 @@ struct TcArgs {
     int tw, rows_per_tile, wsegs;
     int sh, ph, parity, woff; // parity = 1: stride 2 along W through the [Wp/2][2] view; woff = in_halo - pw
     int kw, kc_per_tap, num_kc;
+    // mode 1, two A sources (a block-0 conv3 with the downsample folded in): chunks [0, k1) come from tmA as described
+    // above, chunks [k1, num_kc) from tmA2, a 1x1 conv without padding with its own row stride, parity and woff.
+    // k1 = num_kc: one source
+    int k1, sh2, parity2, woff2;
     int Bimg;                 // images per plane (plane p of image b sits at index p*Bimg + b of the outer TMA dim)
     int Cout, n_tiles, num_tiles;
     const float* scale;
@@ -282,9 +289,9 @@ __device__ __forceinline__ void tile_boxes(const TcArgs& a, const EpiLayout<BN>&
 
 template <int BN>
 __global__ void __launch_bounds__(NTHREADS, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO, const TcArgs a,
-               unsigned* sched) {
+conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
+               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmR,
+               const __grid_constant__ CUtensorMap tmO, const TcArgs a, unsigned* sched) {
     using S = Smem<BN>;
     constexpr int NST = S::NST;
     constexpr int HALF_TILE = BM * BN * 2;     // one output plane; half an output tile
@@ -318,6 +325,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
     if (warp == 0 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
+        if (a.k1 < a.num_kc) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA2)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmO)) : "memory");
     }
@@ -377,8 +385,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         mbar_wait(empty_bar + stage, phase ^ 1);
                         uint8_t* sA = smem + stage * S::STAGE;
                         uint8_t* sB = sA + 2 * S::A_PLANE;
-                        const int tap = kc / a.kc_per_tap;
-                        const int c0 = (kc - tap * a.kc_per_tap) * BKC;
+                        const bool src2 = kc >= a.k1;
+                        const int tap = src2 ? 0 : kc / a.kc_per_tap;
+                        const int c0 = (src2 ? kc - a.k1 : kc - tap * a.kc_per_tap) * BKC;
                         // one box per plane always delivers the full tile (rows past the end are out-of-bounds zero fill)
                         mbar_expect_tx(full_bar + stage, 2u * S::A_PLANE + 2u * S::B_PLANE);
                         if (a.mode == 0) {
@@ -386,17 +395,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                             tma_load_3d(sA + S::A_PLANE, &tmA, full_bar + stage, c0, mt * BM, 1);
                         } else {
                             // the tile's output rows are consecutive rows of one image, or whole images (conv_tc_plan)
+                            const CUtensorMap* tm = src2 ? &tmA2 : &tmA;
                             const int dy = tap / a.kw, dx = tap - dy * a.kw;
                             const int b = row0 / a.Ho, ho = row0 - b * a.Ho;
-                            const int hin = ho * a.sh + dy - a.ph;
-                            if (a.parity) {
-                                const int p = dx + a.woff;
-                                tma_load_5d(sA, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin, b);
-                                tma_load_5d(sA + S::A_PLANE, &tmA, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin,
+                            const int hin = src2 ? ho * a.sh2 : ho * a.sh + dy - a.ph;
+                            const int woff = src2 ? a.woff2 : a.woff;
+                            if (src2 ? a.parity2 : a.parity) {
+                                const int p = dx + woff;
+                                tma_load_5d(sA, tm, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin, b);
+                                tma_load_5d(sA + S::A_PLANE, tm, full_bar + stage, c0, p & 1, wo0 + (p >> 1), hin,
                                             a.Bimg + b);
                             } else {
-                                tma_load_4d(sA, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin, b);
-                                tma_load_4d(sA + S::A_PLANE, &tmA, full_bar + stage, c0, wo0 + dx + a.woff, hin, a.Bimg + b);
+                                tma_load_4d(sA, tm, full_bar + stage, c0, wo0 + dx + woff, hin, b);
+                                tma_load_4d(sA + S::A_PLANE, tm, full_bar + stage, c0, wo0 + dx + woff, hin, a.Bimg + b);
                             }
                         }
                         tma_load_3d(sB, &tmB, full_bar + stage, kc * BKC, nt * BN, 0);
@@ -984,13 +995,18 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // The 64-channel intermediate never visits HBM, and the TMA engine streams the residual and the output of one
 // conv3 tile while the next one computes.  Results are bit-identical to the unfused kernels (same products, same
 // accumulator structure, same epilogue arithmetic); HN_TC_FUSE=0 selects the unfused path.
-//   warp 0      TMA producer (input rows, then the conv2 and conv3 weight tiles of the tile through one ring)
+// With the downsample folded in (`fold`, layer1.0) conv3 has no residual: the producer loads the tile's 128 pixels of
+// the block input x once, into the next input-row slot, and every conv3 n-tile accumulates two K chunks, t2 and that x
+// tile, against the folded weights [s3 W3 ; sd Wd] -- the same products in the same order as conv_tc_kernel's two-source
+// conv3, so the result stays bit-identical to the unfused path.
+//   warp 0      TMA producer (input rows, the x tile, then the conv2 and conv3 weight tiles of the tile through one ring)
 //   warp 2      residual-tile loader          warp 3   TMA store          warps 4-11   two consumer warpgroups
 struct BottArgs {
     int Ho, Wo, Wop, wsegs, Bimg;
     int num_tiles;
     int n3;                              // conv3 n-tiles of 64 channels (Cout3 / 64)
     int C3;                              // conv3 output channels
+    int fold;                            // 1: conv3 K = [t2 | x] (downsample folded in), no residual
     const float* scale2; const float* shift2;     // conv2: accumulator -> plane units, shift in plane units
     const float* scale3; const float* shift3;     // conv3
     unsigned short* out; size_t out_plane;        // output planes (halo-column stores)
@@ -1016,7 +1032,8 @@ static_assert(BtSmem::T2_OFF % 1024 == 0 && BtSmem::E_OFF % 1024 == 0 && BtSmem:
 __global__ void __launch_bounds__(NTHREADS, 1)
 bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB2,
                const __grid_constant__ CUtensorMap tmB3, const __grid_constant__ CUtensorMap tmR,
-               const __grid_constant__ CUtensorMap tmO, const BottArgs a, unsigned* sched) {
+               const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmO, const BottArgs a,
+               unsigned* sched) {
     using S = BtSmem;
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
@@ -1035,7 +1052,7 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB2)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB3)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmR)) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(a.fold ? &tmX : &tmR)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmO)) : "memory");
     }
     if (warp == 1 && lane == 0) {
@@ -1084,13 +1101,24 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         if (++bst == S::NB) { bst = 0; bph ^= 1; }
                     }
                 }
+                if (a.fold) {                           // the tile's 128 pixels of x, read by every conv3 n-tile
+                    mbar_wait(aempty_bar + ast, aph ^ 1);
+                    uint8_t* sX = smem + ast * S::AX_SLOT;
+                    const int pix0 = rg * a.Wop + 1 + wo0;
+                    mbar_expect_tx(afull_bar + ast, 2u * BM * 128u);
+                    tma_load_3d(sX, &tmX, afull_bar + ast, 0, pix0, 0);
+                    tma_load_3d(sX + S::AX_PLANE, &tmX, afull_bar + ast, 0, pix0, 1);
+                    if (++ast == 2) { ast = 0; aph ^= 1; }
+                }
                 for (int j = 0; j < n3; ++j) {          // conv3 weight tiles (the same for every tile: L2 hits)
-                    mbar_wait(empty_bar + bst, bph ^ 1);
-                    uint8_t* sB = smem + S::B_OFF + bst * S::B_STAGE;
-                    mbar_expect_tx(full_bar + bst, (uint32_t)S::B_STAGE);
-                    tma_load_3d(sB, &tmB3, full_bar + bst, 0, j * 64, 0);
-                    tma_load_3d(sB + S::B_PLANE, &tmB3, full_bar + bst, 0, j * 64, 1);
-                    if (++bst == S::NB) { bst = 0; bph ^= 1; }
+                    for (int kc = 0; kc <= a.fold; ++kc) {
+                        mbar_wait(empty_bar + bst, bph ^ 1);
+                        uint8_t* sB = smem + S::B_OFF + bst * S::B_STAGE;
+                        mbar_expect_tx(full_bar + bst, (uint32_t)S::B_STAGE);
+                        tma_load_3d(sB, &tmB3, full_bar + bst, kc * BKC, j * 64, 0);
+                        tma_load_3d(sB + S::B_PLANE, &tmB3, full_bar + bst, kc * BKC, j * 64, 1);
+                        if (++bst == S::NB) { bst = 0; bph ^= 1; }
+                    }
                 }
             }
         }
@@ -1108,6 +1136,7 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 for (int j = 0; j < n3; ++j, ++g3) {
                     const int eb = g3 & 1;
                     mbar_wait(efree_bar + eb, ((g3 >> 1) & 1) ^ 1);
+                    if (a.fold) { mbar_arrive(rfull_bar + eb); continue; }      // no residual: the buffer is just free
                     uint8_t* ebuf = smem + S::E_OFF + eb * S::EBUF;
                     mbar_expect_tx(rfull_bar + eb, 2u * S::E_PLANE);
                     tma_load_3d(ebuf, &tmR, rfull_bar + eb, j * 64, pix0, 0);
@@ -1204,11 +1233,25 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
             for (int h = 0; h < 2; ++h)
                 halo.pix[h] = halo_pixel(frag_row(wg, warp, lane, h), (long long)rg * a.Wop, a.Wop, BM, 1, wo0, a.Wo);
+            uint32_t x_hi = 0;
+            if (a.fold) {
+                mbar_wait(afull_bar + ast, aph);
+                x_hi = smem_u32(smem + ast * S::AX_SLOT) + a_row_off;
+            }
             for (int j = 0; j < n3; ++j, ++g3) {
                 mbar_wait(full_bar + bst, bph);
                 const uint32_t sB = smem_u32(smem + S::B_OFF + bst * S::B_STAGE);
-                chunk_mma(acc, t_hi + a_row_off, t_lo + a_row_off, sB, sB + S::B_PLANE, true);
+                chunk_issue(acc, t_hi + a_row_off, t_lo + a_row_off, sB, sB + S::B_PLANE, true);
+                if (a.fold) {                         // + the x chunk against the next weight tile, one segment
+                    const int b1 = bst + 1 == S::NB ? 0 : bst + 1;
+                    mbar_wait(full_bar + b1, b1 == 0 ? bph ^ 1 : bph);
+                    const uint32_t sB1 = smem_u32(smem + S::B_OFF + b1 * S::B_STAGE);
+                    chunk_issue(acc, x_hi, x_hi + S::AX_PLANE, sB1, sB1 + S::B_PLANE, false);
+                }
+                wgmma_wait0();
+                reg_fence(acc);
                 release_b();
+                if (a.fold) release_b();
 #pragma unroll
                 for (int q = 0; q < 32; ++q) sum[q] = 0.f + acc[q];      // as gemm_tc_kernel's single segment
                 const int eb = g3 & 1;
@@ -1216,11 +1259,16 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 const uint32_t e_hi = smem_u32(smem + S::E_OFF + eb * S::EBUF);
                 HaloStore hj = halo;
                 hj.n0 = j * 64;
-                epi_inplace<64>(sum, cst + 128 + j * 64, cst + 128 + a.C3 + j * 64, e_hi, e_hi + S::E_PLANE, true, true, wg,
-                              warp, lane, &hj);
+                epi_inplace<64>(sum, cst + 128 + j * 64, cst + 128 + a.C3 + j * 64, e_hi, e_hi + S::E_PLANE, !a.fold, true,
+                                wg, warp, lane, &hj);
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                 __syncwarp();
                 if (lane == 0) mbar_arrive(oready_bar + eb);
+            }
+            if (a.fold) {                             // every n-tile has read the x tile
+                __syncwarp();
+                if (lane == 0) mbar_arrive(aempty_bar + ast);
+                if (++ast == 2) { ast = 0; aph ^= 1; }
             }
         }
     }
@@ -1228,14 +1276,44 @@ bott_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
 // -------------------------------------------------------------------------------- host side
 template <int BN>
-int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO, const TcArgs& a,
-           int grid, cudaStream_t st) {
+int launch(const CUtensorMap& tmA, const CUtensorMap& tmA2, const CUtensorMap& tmB, const CUtensorMap& tmR,
+           const CUtensorMap& tmO, const TcArgs& a, int grid, cudaStream_t st) {
     const int bytes = conv_smem_bytes<BN>(a.Cout);
     HN_CHECK(bytes <= MAX_SMEM, "conv_tc: too many output channels for the epilogue constants in shared memory");
     HN_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    HN_CUDA_OK(launch_tc(conv_tc_kernel<BN>, grid, bytes, st, tmA, tmB, tmR, tmO, a));
+    HN_CUDA_OK(launch_tc(conv_tc_kernel<BN>, grid, bytes, st, tmA, tmA2, tmB, tmR, tmO, a));
     HN_LAUNCH_OK();
     return 0;
+}
+
+int launch_bn(int BN, const CUtensorMap& tmA, const CUtensorMap& tmA2, const CUtensorMap& tmB, const CUtensorMap& tmR,
+              const CUtensorMap& tmO, const TcArgs& a, int grid, cudaStream_t st) {
+    switch (BN) {
+        case 128: return launch<128>(tmA, tmA2, tmB, tmR, tmO, a, grid, st);
+        case 64: return launch<64>(tmA, tmA2, tmB, tmR, tmO, a, grid, st);
+        default: return launch<32>(tmA, tmA2, tmB, tmR, tmO, a, grid, st);
+    }
+}
+
+// Conv-row (mode 1) A operand map of a 1x1 or kxk conv over `in` for the tiles of plan pl: {C, Wp, H, 2B} (or with
+// stride 2 along W the parity view {C, 2, Wp/2, H, 2B}), one box per plane of a tile's 128 pixels x 64 channels
+int conv_rows_map(CUtensorMap* tm, const unsigned short* in_planes, const Act& in, int Cin, int sh, bool parity,
+                  bool dxr, const TcPlan& pl) {
+    // stride 2 along H (height-reduction convs): a box of several rows spans 2*rows input rows and takes every second
+    // one; a one-row tile reads its input row without a traversal stride
+    const int hs = pl.rows_per_tile > 1 ? sh : 1;
+    const cuuint32_t boxrows = (cuuint32_t)(pl.box_rows * hs);
+    const cuuint64_t C2 = (cuuint64_t)Cin * 2, Wp = in.Wp();
+    if (!parity) {
+        cuuint64_t dims[4] = {(cuuint64_t)Cin, Wp, (cuuint64_t)in.H, (cuuint64_t)2 * in.B};
+        cuuint64_t str[3] = {C2, C2 * Wp, C2 * Wp * in.H};
+        cuuint32_t box[4] = {BKC, dxr ? 130u : (cuuint32_t)pl.tw, boxrows, (cuuint32_t)pl.box_imgs};
+        return make_map(tm, in_planes, 4, dims, str, box, 2, hs);
+    }
+    cuuint64_t dims[5] = {(cuuint64_t)Cin, 2, Wp / 2, (cuuint64_t)in.H, (cuuint64_t)2 * in.B};
+    cuuint64_t str[4] = {C2, 2 * C2, C2 * Wp, C2 * Wp * in.H};
+    cuuint32_t box[5] = {BKC, 1, (cuuint32_t)pl.tw, boxrows, (cuuint32_t)pl.box_imgs};
+    return make_map(tm, in_planes, 5, dims, str, box, 3, hs);
 }
 
 // Tensor map of an output-geometry tensor (output or residual) as the epilogue of a tile with BN channels moves it (see
@@ -1263,13 +1341,16 @@ int conv_tc_map(CUtensorMap* tm, const void* base, const TcPlan& pl, const Act& 
 
 }  // namespace
 
-bool conv_tc_supported(const ConvDesc& d, const Act& in, const Act& out) {
+// channel and padding limits of both modes
+static bool conv_channels_supported(const ConvDesc& d, const Act& in) {
     if (d.Cin % 64 != 0 || d.Cout % 32 != 0) return false;
     if (d.Cout > 64 && d.Cout % 128 != 0) return false;
     if (d.Cout < 64 && d.Cout != 32) return false;
-    if (d.pw > in.halo) return false;
-    const bool gemm = (d.kh == 1 && d.kw == 1 && d.sh == 1 && d.sw == 1 && in.halo == out.halo);
-    if (gemm) return true;
+    return d.pw <= in.halo;
+}
+
+// the conv-row (mode 1) tiling
+static bool conv_rows_supported(const ConvDesc& d, const Act& in, const Act& out) {
     if (d.sw != 1 && d.sw != 2) return false;
     if (d.sw == 2 && (in.Wp() % 2) != 0) return false;
     const int tw = out.W < 128 ? out.W : 128;
@@ -1281,18 +1362,49 @@ bool conv_tc_supported(const ConvDesc& d, const Act& in, const Act& out) {
     return out.H % rows_per_tile == 0 || rows_per_tile % out.H == 0;
 }
 
+bool conv_tc_supported(const ConvDesc& d, const Act& in, const Act& out) {
+    if (!conv_channels_supported(d, in)) return false;
+    const bool gemm = (d.kh == 1 && d.kw == 1 && d.sh == 1 && d.sw == 1 && in.halo == out.halo);
+    return gemm || conv_rows_supported(d, in, out);
+}
+
+// output channels per tile for `rows` output pixels
+static int tile_bn(int Cout, long long rows) {
+    const int BN = Cout >= 128 ? 128 : Cout;
+    // layers with too few 128x128 tiles to fill the SMs (the tail of the height-reduction convs): halve the tile width
+    const long long tiles128 = ((rows + BM - 1) / BM) * (Cout / 128 > 0 ? Cout / 128 : 1);
+    return (BN == 128 && tiles128 < 110) ? 64 : BN;
+}
+
+// conv-row (mode 1) fields of the plan; returns the number of M tiles
+static long long plan_rows(const ConvDesc& d, const Act& in, const Act& out, bool out_f32, TcPlan* p) {
+    p->mode = 1;
+    p->M = out.B * out.H;
+    p->tw = out.W < 128 ? out.W : 128;
+    p->rows_per_tile = BM / p->tw;
+    p->wsegs = out.W / p->tw;
+    p->parity = (d.sw == 2);
+    // one box for all rows of a tile: consecutive output rows of one image, or whole images when an image has fewer
+    // output rows than a tile (the last height-reduction convs) -- the box then spans R / Ho consecutive images
+    p->box_rows = p->box_imgs = 1;
+    if (out.H % p->rows_per_tile == 0) p->box_rows = p->rows_per_tile;
+    else { p->box_rows = out.H; p->box_imgs = p->rows_per_tile / out.H; }
+    // dx reuse (HN_TC_DXR=0 disables).  Its epilogue slot is two weight slots, each half an output tile: a plane, or
+    // half of the fp32 boxes -- which needs two of them (BN >= 64)
+    static const int dxr_mode = [] { const char* e = getenv("HN_TC_DXR"); return e ? atoi(e) : 1; }();
+    p->dxr = (dxr_mode != 0 && !p->parity && d.kw == 3 && p->rows_per_tile == 1 && p->tw == BM &&
+              !(out_f32 && p->BN < 64) &&
+              (long long)p->wsegs * BM + (in.halo - d.pw) + 2 <= (long long)in.Wp()) ? 1 : 0;
+    return (long long)((p->M + p->rows_per_tile - 1) / p->rows_per_tile) * p->wsegs;
+}
+
 int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32, bool has_residual, int sms, TcPlan* p) {
     HN_CHECK(conv_tc_supported(d, in, out), "conv_tc: unsupported shape");
     HN_CHECK(!(out_f32 && has_residual), "conv_tc: residual with fp32 output is not supported");
     HN_CHECK(sms >= 1, "conv_tc_plan: sms must be positive");
     memset(p, 0, sizeof(*p));
     const bool gemm = (d.kh == 1 && d.kw == 1 && d.sh == 1 && d.sw == 1 && in.halo == out.halo);
-    int BN = d.Cout >= 128 ? 128 : d.Cout;
-    {   // layers with too few 128x128 tiles to fill the SMs (the tail of the height-reduction convs): halve the tile width
-        const long long rows = gemm ? (long long)in.B * in.H * in.Wp() : (long long)out.B * out.H * out.W;
-        const long long tiles128 = ((rows + BM - 1) / BM) * (d.Cout / 128 > 0 ? d.Cout / 128 : 1);
-        if (BN == 128 && tiles128 < 110) BN = 64;
-    }
+    const int BN = tile_bn(d.Cout, gemm ? (long long)in.B * in.H * in.Wp() : (long long)out.B * out.H * out.W);
     p->num_kc = d.kh * d.kw * (d.Cin / BKC);
     p->seg = SEG;
     p->box_rows = p->box_imgs = 1;
@@ -1316,23 +1428,7 @@ int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32,
         m_tiles = ((long long)p->M + BM - 1) / BM;
     } else {
         p->BN = BN;
-        p->mode = 1;
-        p->M = out.B * out.H;
-        p->tw = out.W < 128 ? out.W : 128;
-        p->rows_per_tile = BM / p->tw;
-        p->wsegs = out.W / p->tw;
-        p->parity = (d.sw == 2);
-        // one box for all rows of a tile: consecutive output rows of one image, or whole images when an image has fewer
-        // output rows than a tile (the last height-reduction convs) -- the box then spans R / Ho consecutive images
-        if (out.H % p->rows_per_tile == 0) p->box_rows = p->rows_per_tile;
-        else { p->box_rows = out.H; p->box_imgs = p->rows_per_tile / out.H; }
-        // dx reuse (HN_TC_DXR=0 disables).  Its epilogue slot is two weight slots, each half an output tile: a plane, or
-        // half of the fp32 boxes -- which needs two of them (BN >= 64)
-        static const int dxr_mode = [] { const char* e = getenv("HN_TC_DXR"); return e ? atoi(e) : 1; }();
-        p->dxr = (dxr_mode != 0 && !p->parity && d.kw == 3 && p->rows_per_tile == 1 && p->tw == BM &&
-                  !(out_f32 && BN < 64) &&
-                  (long long)p->wsegs * BM + (in.halo - d.pw) + 2 <= (long long)in.Wp()) ? 1 : 0;
-        m_tiles = (long long)((p->M + p->rows_per_tile - 1) / p->rows_per_tile) * p->wsegs;
+        m_tiles = plan_rows(d, in, out, out_f32, p);
     }
     p->n_tiles = d.Cout / p->BN;
     HN_CHECK(m_tiles * p->n_tiles < (1ll << 31), "conv_tc: too many tiles");
@@ -1389,6 +1485,7 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
         HN_LAUNCH_OK();
         return 0;
     }
+    a.k1 = a.num_kc;
     if (pl.mode == 0) {
         cuuint64_t dims[3] = {(cuuint64_t)d.Cin, (cuuint64_t)pl.M, 2};
         cuuint64_t str[2] = {(cuuint64_t)d.Cin * 2, (cuuint64_t)in_plane * 2};
@@ -1402,22 +1499,7 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
         a.sh = d.sh; a.ph = d.ph; a.woff = in.halo - d.pw;
         a.parity = pl.parity;
         a.dxr = pl.dxr;
-        // stride 2 along H (height-reduction convs): a box of several rows spans 2*rows input rows and takes every second
-        // one; a one-row tile reads its input row without a traversal stride
-        const int hs = pl.rows_per_tile > 1 ? d.sh : 1;
-        const cuuint32_t boxrows = (cuuint32_t)(pl.box_rows * hs);
-        const cuuint64_t C2 = (cuuint64_t)d.Cin * 2, Wp = in.Wp();
-        if (!a.parity) {
-            cuuint64_t dims[4] = {(cuuint64_t)d.Cin, Wp, (cuuint64_t)in.H, (cuuint64_t)2 * in.B};
-            cuuint64_t str[3] = {C2, C2 * Wp, C2 * Wp * in.H};
-            cuuint32_t box[4] = {BKC, a.dxr ? 130u : (cuuint32_t)a.tw, boxrows, (cuuint32_t)pl.box_imgs};
-            if (make_map(&tmA, in_planes, 4, dims, str, box, 2, hs)) return -1;
-        } else {
-            cuuint64_t dims[5] = {(cuuint64_t)d.Cin, 2, Wp / 2, (cuuint64_t)in.H, (cuuint64_t)2 * in.B};
-            cuuint64_t str[4] = {C2, 2 * C2, C2 * Wp, C2 * Wp * in.H};
-            cuuint32_t box[5] = {BKC, 1, (cuuint32_t)a.tw, boxrows, (cuuint32_t)pl.box_imgs};
-            if (make_map(&tmA, in_planes, 5, dims, str, box, 3, hs)) return -1;
-        }
+        if (conv_rows_map(&tmA, in_planes, in, d.Cin, d.sh, a.parity != 0, a.dxr != 0, pl)) return -1;
     }
     if (a.num_tiles == 0) return 0;
     CUtensorMap tmR, tmO;
@@ -1425,11 +1507,65 @@ int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_
     const void* obase = f32 ? static_cast<const void*>(out_f32) : static_cast<const void*>(out_planes);
     if (conv_tc_map(&tmO, obase, pl, out, d.Cout, f32)) return -1;
     if (conv_tc_map(&tmR, res_planes ? static_cast<const void*>(res_planes) : obase, pl, out, d.Cout, f32)) return -1;
-    switch (BN) {
-        case 128: return launch<128>(tmA, tmB, tmR, tmO, a, pl.grid, st);
-        case 64: return launch<64>(tmA, tmB, tmR, tmO, a, pl.grid, st);
-        default: return launch<32>(tmA, tmB, tmR, tmO, a, pl.grid, st);
+    return launch_bn(BN, tmA, tmA, tmB, tmR, tmO, a, pl.grid, st);
+}
+
+// ---------------------------------------------------------------------- block-0 conv3 with the downsample folded in
+// Plan of conv_tc_fold_planes: conv rows over the output geometry (the downsample's plan, stride 1 or 2), K chunks of t2
+// then of x
+int conv_tc_fold_plan(const Act& t2, const Act& x, int stride, const Act& out, int sms, TcPlan* p) {
+    ConvDesc dd;
+    memset(&dd, 0, sizeof(dd));
+    dd.Cin = x.C; dd.Cout = out.C; dd.kh = dd.kw = 1; dd.sh = dd.sw = stride;
+    HN_CHECK(stride == 1 || stride == 2, "conv_tc_fold: stride must be 1 or 2");
+    HN_CHECK(t2.B == out.B && t2.H == out.H && t2.W == out.W && t2.halo == out.halo && x.B == out.B &&
+             x.H == out.H * stride && x.W == out.W * stride && t2.C % 64 == 0,
+             "conv_tc_fold: t2 must have the output geometry and x stride times its size");
+    HN_CHECK(conv_channels_supported(dd, x) && conv_rows_supported(dd, x, out), "conv_tc_fold: unsupported shape");
+    HN_CHECK(sms >= 1, "conv_tc_fold_plan: sms must be positive");
+    memset(p, 0, sizeof(*p));
+    p->BN = tile_bn(out.C, (long long)out.B * out.H * out.W);
+    p->num_kc = (t2.C + x.C) / BKC;
+    p->seg = SEG;
+    const long long m_tiles = plan_rows(dd, x, out, false, p);
+    p->n_tiles = out.C / p->BN;
+    HN_CHECK(m_tiles * p->n_tiles < (1ll << 31), "conv_tc: too many tiles");
+    p->num_tiles = (int)(m_tiles * p->n_tiles);
+    p->grid = p->num_tiles < sms ? p->num_tiles : sms;
+    return 0;
+}
+
+int conv_tc_fold_planes(const unsigned short* wq, const float* tc_aux, const Act& t2, const unsigned short* t2_planes,
+                        const Act& x, const unsigned short* x_planes, int stride, const Act& out, unsigned short* out_planes,
+                        cudaStream_t st) {
+    TcPlan pl;
+    if (conv_tc_fold_plan(t2, x, stride, out, num_sms(), &pl)) return -1;
+    const int K = t2.C + x.C, Cout = out.C;
+    TcArgs a;
+    memset(&a, 0, sizeof(a));
+    CUtensorMap tmA, tmA2, tmB, tmR, tmO;
+    {   // folded weights: {K, Cout, 2}
+        cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)Cout, 2};
+        cuuint64_t str[2] = {(cuuint64_t)K * 2, (cuuint64_t)K * Cout * 2};
+        cuuint32_t box[3] = {BKC, (cuuint32_t)pl.BN, 1};
+        if (make_map(&tmB, wq, 3, dims, str, box)) return -1;
     }
+    a.mode = 1; a.M = pl.M;
+    a.Cout = Cout; a.n_tiles = pl.n_tiles; a.num_tiles = pl.num_tiles;
+    a.kw = 1; a.kc_per_tap = t2.C / BKC; a.num_kc = pl.num_kc; a.k1 = t2.C / BKC;
+    a.scale = tc_aux + Cout; a.shift = tc_aux + 2 * Cout;                // plane units
+    a.out = out_planes; a.out_plane = out.numel(); a.relu = 1;
+    a.Bimg = out.B;
+    a.Ho = out.H; a.Wo = out.W; a.Wop = out.Wp(); a.out_halo = out.halo;
+    a.tw = pl.tw; a.rows_per_tile = pl.rows_per_tile; a.wsegs = pl.wsegs;
+    a.sh = 1; a.ph = 0; a.parity = 0; a.woff = t2.halo;
+    a.sh2 = stride; a.parity2 = pl.parity; a.woff2 = x.halo;
+    if (conv_rows_map(&tmA, t2_planes, t2, t2.C, 1, false, false, pl)) return -1;
+    if (conv_rows_map(&tmA2, x_planes, x, x.C, stride, pl.parity != 0, false, pl)) return -1;
+    if (a.num_tiles == 0) return 0;
+    if (conv_tc_map(&tmO, out_planes, pl, out, Cout, false)) return -1;
+    if (conv_tc_map(&tmR, out_planes, pl, out, Cout, false)) return -1;
+    return launch_bn(pl.BN, tmA, tmA2, tmB, tmR, tmO, a, pl.grid, st);
 }
 
 
@@ -1444,21 +1580,25 @@ bool bott_tc_supported(const ConvDesc& d2, const ConvDesc& d3, const Act& in, co
 }
 
 // in: conv2 input planes [B][H][W+2][64]; res / out: [B][H][W+2][C3] planes (res = the block's identity); wq2 / aux2, wq3 / aux3
-// as produced by pack_weight_tc for the two convolutions.
+// as produced by pack_weight_tc for the two convolutions.  Folded downsample instead of an identity (res_planes null):
+// x_planes = the block input, in `in`'s geometry, and wq3 / aux3 the folded pack [2][C3][64 + 64] (conv_tc_fold_planes).
 int bott_tc_planes(const ConvDesc& d2, const unsigned short* wq2, const float* aux2, const ConvDesc& d3,
                    const unsigned short* wq3, const float* aux3, const Act& in, const unsigned short* in_planes, const Act& out,
-                   unsigned short* out_planes, const unsigned short* res_planes, cudaStream_t st) {
+                   unsigned short* out_planes, const unsigned short* res_planes, const unsigned short* x_planes,
+                   cudaStream_t st) {
     HN_CHECK(bott_tc_supported(d2, d3, in, out), "bott_tc: unsupported shape");
-    HN_CHECK(res_planes != nullptr, "bott_tc: the fused kernel expects the block's identity");
+    HN_CHECK((res_planes != nullptr) != (x_planes != nullptr),
+             "bott_tc: the fused kernel takes the block's identity or, folded, its input");
+    const int fold = x_planes != nullptr;
+    const int K3 = 64 * (1 + fold);
     const size_t in_plane = in.numel(), out_plane = out.numel();
     const cuuint64_t Wp = in.Wp();
-    CUtensorMap tmA, tmB2, tmB3, tmR, tmO;
+    CUtensorMap tmA, tmB2, tmB3, tmR, tmX, tmO;
     {
         cuuint64_t dims[4] = {64, Wp, (cuuint64_t)in.H, (cuuint64_t)2 * in.B};
         cuuint64_t str[3] = {128, 128 * Wp, 128 * Wp * in.H};
         cuuint32_t box[4] = {BKC, 130, 1, 1};
         if (make_map(&tmA, in_planes, 4, dims, str, box)) return -1;
-        (void)in_plane;
     }
     {
         cuuint64_t dims[3] = {576, 64, 2};
@@ -1467,8 +1607,8 @@ int bott_tc_planes(const ConvDesc& d2, const unsigned short* wq2, const float* a
         if (make_map(&tmB2, wq2, 3, dims, str, box)) return -1;
     }
     {
-        cuuint64_t dims[3] = {64, (cuuint64_t)d3.Cout, 2};
-        cuuint64_t str[2] = {64 * 2, (cuuint64_t)64 * d3.Cout * 2};
+        cuuint64_t dims[3] = {(cuuint64_t)K3, (cuuint64_t)d3.Cout, 2};
+        cuuint64_t str[2] = {(cuuint64_t)K3 * 2, (cuuint64_t)K3 * d3.Cout * 2};
         cuuint32_t box[3] = {BKC, 64, 1};
         if (make_map(&tmB3, wq3, 3, dims, str, box)) return -1;
     }
@@ -1478,7 +1618,10 @@ int bott_tc_planes(const ConvDesc& d2, const unsigned short* wq2, const float* a
         cuuint64_t str[2] = {(cuuint64_t)d3.Cout * 2, (cuuint64_t)out_plane * 2};
         cuuint32_t box[3] = {64, BM, 1};
         if (make_map(&tmO, out_planes, 3, dims, str, box)) return -1;
-        if (make_map(&tmR, res_planes, 3, dims, str, box)) return -1;
+        if (make_map(&tmR, fold ? out_planes : res_planes, 3, dims, str, box)) return -1;
+        cuuint64_t xdims[3] = {64, Mtot, 2};
+        cuuint64_t xstr[2] = {128, (cuuint64_t)in_plane * 2};
+        if (make_map(&tmX, fold ? x_planes : in_planes, 3, xdims, xstr, box)) return -1;
     }
     BottArgs a;
     memset(&a, 0, sizeof(a));
@@ -1487,6 +1630,7 @@ int bott_tc_planes(const ConvDesc& d2, const unsigned short* wq2, const float* a
     HN_CHECK(tiles < (1ll << 31) && (long long)out.B * out.H * out.Wp() < (1ll << 31), "bott_tc: too many tiles");
     a.num_tiles = (int)tiles;
     a.n3 = d3.Cout / 64; a.C3 = d3.Cout;
+    a.fold = fold;
     a.scale2 = aux2 + 64; a.shift2 = aux2 + 2 * 64;                        // plane units (conv_tc.cuh: tc_aux)
     a.scale3 = aux3 + d3.Cout; a.shift3 = aux3 + 2 * d3.Cout;
     a.out = out_planes; a.out_plane = out_plane;
@@ -1495,7 +1639,8 @@ int bott_tc_planes(const ConvDesc& d2, const unsigned short* wq2, const float* a
     int dev = 0, sms = 0;
     HN_CUDA_OK(cudaGetDevice(&dev));
     HN_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    HN_CUDA_OK(launch_tc(bott_tc_kernel, a.num_tiles < sms ? a.num_tiles : sms, BtSmem::TOTAL, st, tmA, tmB2, tmB3, tmR, tmO, a));
+    HN_CUDA_OK(launch_tc(bott_tc_kernel, a.num_tiles < sms ? a.num_tiles : sms, BtSmem::TOTAL, st, tmA, tmB2, tmB3, tmR, tmX,
+                         tmO, a));
     HN_LAUNCH_OK();
     return 0;
 }
@@ -1695,6 +1840,64 @@ int conv_tc(const ConvDesc& d, const Act& in, const Act& out, const float* resid
     if (pout) cudaFreeAsync(pout, st);
     if (pres) cudaFreeAsync(pres, st);
     return rc;
+}
+
+// Unit-test conveniences of the folded conv3 and of the fused layer1.0 bottleneck: fp32 halo-NHWC tensors in and out,
+// planes and packed weights built on the fly.  `bufs` holds the device allocations, freed on every path.
+namespace {
+struct DevBufs {
+    cudaStream_t st;
+    std::vector<void*> p;
+    template <typename T>
+    T* get(size_t n) {
+        void* q = nullptr;
+        if (cudaMallocAsync(&q, n * sizeof(T), st) != cudaSuccess) return nullptr;
+        p.push_back(q);
+        return static_cast<T*>(q);
+    }
+    ~DevBufs() { for (void* q : p) cudaFreeAsync(q, st); }
+};
+}  // namespace
+
+int conv_tc_fold(const float* w, const float* shift, const Act& t2, const Act& x, int stride, const Act& out,
+                 cudaStream_t st) {
+    TcPlan pl;
+    if (conv_tc_fold_plan(t2, x, stride, out, 1, &pl)) return -1;
+    const int K = t2.C + x.C;
+    DevBufs b{st, {}};
+    unsigned short *pt = b.get<unsigned short>(2 * t2.numel()), *px = b.get<unsigned short>(2 * x.numel());
+    unsigned short *po = b.get<unsigned short>(2 * out.numel()), *pw = b.get<unsigned short>((size_t)2 * K * out.C);
+    float* aux = b.get<float>(3 * out.C + 1);
+    HN_CHECK(pt && px && po && pw && aux, "conv_tc_fold: out of device memory");
+    HN_CUDA_OK(cudaMemsetAsync(po, 0xff, out.numel() * 4, st));     // NaN: an element the kernel leaves unwritten
+    if (split_planes(t2.p, pt, t2.numel(), st) || split_planes(x.p, px, x.numel(), st)) return -1;
+    if (pack_weight_impl<true>(w, pw, nullptr, shift, aux, aux + 3 * out.C, out.C, K, 1, 1, st)) return -1;
+    if (conv_tc_fold_planes(pw, aux, t2, pt, x, px, stride, out, po, st)) return -1;
+    return merge_planes(po, out.p, out.numel(), st);
+}
+
+int bott_tc_fold(const float* w2, const float* scale2, const float* shift2, const float* w3, const float* shift3,
+                 const Act& in, const Act& x, const Act& out, cudaStream_t st) {
+    ConvDesc d2, d3;
+    memset(&d2, 0, sizeof(d2));
+    d2.Cin = d2.Cout = 64; d2.kh = d2.kw = 3; d2.sh = d2.sw = 1; d2.ph = d2.pw = 1; d2.relu = 1;
+    d3 = d2;
+    d3.Cout = out.C; d3.kh = d3.kw = 1; d3.ph = d3.pw = 0;
+    HN_CHECK(bott_tc_supported(d2, d3, in, out), "bott_tc_fold: unsupported shape");
+    HN_CHECK(x.B == in.B && x.H == in.H && x.W == in.W && x.C == 64 && x.halo == in.halo,
+             "bott_tc_fold: x must have the conv2 input's geometry");
+    DevBufs b{st, {}};
+    unsigned short *pi = b.get<unsigned short>(2 * in.numel()), *px = b.get<unsigned short>(2 * x.numel());
+    unsigned short *po = b.get<unsigned short>(2 * out.numel());
+    unsigned short *pw2 = b.get<unsigned short>(2 * 64 * 576), *pw3 = b.get<unsigned short>((size_t)2 * out.C * 128);
+    float *aux2 = b.get<float>(3 * 64 + 1), *aux3 = b.get<float>(3 * out.C + 1);
+    HN_CHECK(pi && px && po && pw2 && pw3 && aux2 && aux3, "bott_tc_fold: out of device memory");
+    HN_CUDA_OK(cudaMemsetAsync(po, 0xff, out.numel() * 4, st));
+    if (split_planes(in.p, pi, in.numel(), st) || split_planes(x.p, px, x.numel(), st)) return -1;
+    if (pack_weight_impl<true>(w2, pw2, scale2, shift2, aux2, aux2 + 3 * 64, 64, 64, 3, 3, st)) return -1;
+    if (pack_weight_impl<true>(w3, pw3, nullptr, shift3, aux3, aux3 + 3 * out.C, out.C, 128, 1, 1, st)) return -1;
+    if (bott_tc_planes(d2, pw2, aux2, d3, pw3, aux3, in, pi, out, po, nullptr, px, st)) return -1;
+    return merge_planes(po, out.p, out.numel(), st);
 }
 
 }  // namespace hn

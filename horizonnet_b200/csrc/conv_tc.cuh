@@ -82,12 +82,30 @@ int conv_tc(const ConvDesc& d, const Act& in, const Act& out, const float* resid
 int conv_tc_planes(const ConvDesc& d, const unsigned short* wq, const float* tc_aux, const Act& in,
                    const unsigned short* in_planes, const Act& out, unsigned short* out_planes, float* out_f32,
                    const unsigned short* res_planes, cudaStream_t st);
+// Eval-mode conv3 of a bottleneck's block 0 with its downsample folded in: out = relu([t2 | x↓] . wq + shift), one GEMM
+// with K = t2.C + x.C and no residual.  x↓ = x at every stride-th pixel (the 1x1 downsample), t2 has the output geometry.
+// wq: [2][Cout][K] planes of [s3 W3 ; sd Wd] (both BN scales folded into the weights), tc_aux from pack_weight_tc with
+// scale 1 and shift f3 + fd.  Plan: conv rows (mode 1) of conv_tc_kernel, the first t2.C / 64 K chunks from t2.
+int conv_tc_fold_plan(const Act& t2, const Act& x, int stride, const Act& out, int sms, TcPlan* p);
+int conv_tc_fold_planes(const unsigned short* wq, const float* tc_aux, const Act& t2, const unsigned short* t2_planes,
+                        const Act& x, const unsigned short* x_planes, int stride, const Act& out, unsigned short* out_planes,
+                        cudaStream_t st);
+// fp32 halo-NHWC convenience wrapper (unit tests): w = the folded fp32 weights [Cout][K], shift [Cout]
+int conv_tc_fold(const float* w, const float* shift, const Act& t2, const Act& x, int stride, const Act& out,
+                 cudaStream_t st);
 // conv2 (3x3 s1, 64 -> 64) + BN + ReLU fused with conv3 (1x1, 64 -> C3) + BN + identity + ReLU of a layer1 bottleneck
-// (conv_tc.cu: bott_tc_kernel); bit-identical to running conv_tc_planes twice; HN_TC_FUSE=0 disables it.
+// (conv_tc.cu: bott_tc_kernel); bit-identical to running conv_tc_planes twice; HN_TC_FUSE=0 disables it.  With the
+// downsample folded in (res_planes null, x_planes the block input in `in`'s geometry, wq3 / aux3 the folded pack of
+// conv_tc_fold_planes) it is bit-identical to conv_tc_planes + conv_tc_fold_planes.
 bool bott_tc_supported(const ConvDesc& d2, const ConvDesc& d3, const Act& in, const Act& out);
 int bott_tc_planes(const ConvDesc& d2, const unsigned short* wq2, const float* aux2, const ConvDesc& d3,
                    const unsigned short* wq3, const float* aux3, const Act& in, const unsigned short* in_planes, const Act& out,
-                   unsigned short* out_planes, const unsigned short* res_planes, cudaStream_t st);
+                   unsigned short* out_planes, const unsigned short* res_planes, const unsigned short* x_planes,
+                   cudaStream_t st);
+// fp32 convenience wrapper of the folded bott_tc_planes (unit tests): w2 OIHW [64][64][3][3] with BN scale2 / shift2,
+// w3 the folded fp32 weights [C3][128] with shift3; in / x / out fp32 halo-NHWC
+int bott_tc_fold(const float* w2, const float* scale2, const float* shift2, const float* w3, const float* shift3,
+                 const Act& in, const Act& x, const Act& out, cudaStream_t st);
 // 7x7 stride-2 stem on wgmma (conv_tc.cu: stem_tc_kernel): NCHW fp32 input -> fp32 halo-NHWC [B][256][514][64]
 // (interior columns only).  wq [2][64][224] / tc_aux [3*64+1] come from stem_tc_pack_weights (pad_scratch: 64*224 floats);
 // scratch: stem_tc_scratch_bytes(B) bytes of packed input planes.

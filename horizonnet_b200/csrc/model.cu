@@ -55,6 +55,20 @@ __global__ void fold_bn_kernel(const float* __restrict__ gamma, const float* __r
     shift[i] = (float)((double)beta[i] + (b - (double)mean[i]) * s);
 }
 
+// block 0: [s3 W3 | sd Wd] per output channel n (1x1 OIHW weights [Cout][Cmid], [Cout][Cin]) and f3 + fd.  Both scales go
+// into the weights (not their ratio: a BN scale can be near 0)
+__global__ void fold_downsample_kernel(const float* __restrict__ w3, const float* __restrict__ s3, const float* __restrict__ f3,
+                                       const float* __restrict__ wd, const float* __restrict__ sd,
+                                       const float* __restrict__ fd, float* __restrict__ w, float* __restrict__ shift,
+                                       int Cout, int Cmid, int Cin) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int K = Cmid + Cin;
+    if (i >= (size_t)Cout * K) return;
+    const int n = (int)(i / K), k = (int)(i - (size_t)n * K);
+    w[i] = k < Cmid ? s3[n] * w3[(size_t)n * Cmid + k] : sd[n] * wd[(size_t)n * Cin + (k - Cmid)];
+    if (k == 0) shift[n] = f3[n] + fd[n];
+}
+
 __global__ void lstm_bias_kernel(const float* __restrict__ bih_f, const float* __restrict__ bhh_f,
                                  const float* __restrict__ bih_b, const float* __restrict__ bhh_b,
                                  float* __restrict__ scale, float* __restrict__ shift) {
@@ -211,6 +225,27 @@ int pack_conv(hn_model* m, ConvLayer& c, cudaStream_t st) {
     return 0;
 }
 
+// Folded conv3 + downsample pack of a block 0 (hn_model::Block::fold) from the eval-mode BN constants of both; built by
+// the first eval forward that uses it after hn_model_finalize or refold_bn (hn_model::fold_stale)
+int alloc_fold(hn_model* m, hn_model::Block& b) {
+    ConvLayer& f = b.fold;
+    const int Cout = b.c3.d.Cout;
+    const size_t nw = (size_t)Cout * (b.c3.d.Cin + b.ds.d.Cin);
+    if (f.w) return 0;
+    return (m->alloc_t(&f.w, nw) || m->alloc_t(&f.shift, Cout) || m->alloc_t(&f.wq, 2 * nw) ||
+            m->alloc_t(&f.tc_scale, 3 * Cout + 1)) ? -1 : 0;
+}
+
+int pack_fold(hn_model* m, hn_model::Block& b, cudaStream_t st) {
+    ConvLayer& f = b.fold;
+    const int Cout = b.c3.d.Cout, Cmid = b.c3.d.Cin, Cin = b.ds.d.Cin, K = Cmid + Cin;
+    const size_t nw = (size_t)Cout * K;
+    fold_downsample_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, st>>>(m->T(b.c3.wkey), b.c3.scale, b.c3.shift,
+                                                                         m->T(b.ds.wkey), b.ds.scale, b.ds.shift, f.w,
+                                                                         f.shift, Cout, Cmid, Cin);
+    HN_LAUNCH_OK();
+    return pack_weight_tc(f.w, f.wq, nullptr, f.shift, f.tc_scale, f.tc_scale + 3 * Cout, Cout, K, 1, 1, st);
+}
 
 
 int run_conv(hn_model* m, const ConvLayer& c, const Act& in, const Act& out, const float* res, cudaStream_t st,
@@ -244,6 +279,7 @@ int refold_bn(hn_model* m, cudaStream_t st) {
         HN_LAUNCH_OK();
         if (c->tc_scale && tc_aux_update(c->scale, c->shift, c->tc_scale + 3 * C, c->tc_scale, C, st)) return -1;
     }
+    m->fold_stale = true;                            // the folded packs carry the BN scales in their weights
     if (tc_aux_update(m->stem.scale, m->stem.shift, m->stem_aux + 3 * 64, m->stem_aux, 64, st)) return -1;
     m->bn_stale = false;
     return 0;
@@ -404,6 +440,7 @@ int hn_model_set_option(hn_model* m, const char* name, int value) {
     if (std::strcmp(name, "profile") == 0) { m->profile = value; return 0; }
     if (std::strcmp(name, "stem_tc") == 0) { m->stem_tc_on = value; return 0; }
     if (std::strcmp(name, "fuse_bottleneck") == 0) { m->fuse_on = value; return 0; }
+    if (std::strcmp(name, "fold_downsample") == 0) { m->fold_on = value; return 0; }
     return fail(std::string("hn_model_set_option: unknown option '") + name + "'");
 }
 
@@ -419,8 +456,9 @@ int hn_model_finalize(hn_model* m) {
     for (int l = 0; l < 4; ++l)
         for (auto& b : m->blocks[l]) {
             if (pack_conv(m, b.c1, st) || pack_conv(m, b.c2, st) || pack_conv(m, b.c3, st)) return -1;
-            if (b.has_ds && pack_conv(m, b.ds, st)) return -1;
+            if (b.has_ds && (pack_conv(m, b.ds, st) || alloc_fold(m, b))) return -1;
         }
+    m->fold_stale = true;
     for (int s = 0; s < 4; ++s)
         for (int j = 0; j < 4; ++j)
             if (pack_conv(m, m->ghc[s][j], st)) return -1;
@@ -485,6 +523,12 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
         for (size_t i = 0; tr && i < m->bn_names.size(); ++i) need = need || !tr->bn_train[i];
         if (need && refold_bn(m, st)) return -1;
     }
+    if (!tr && m->use_tc && m->fold_on && m->fold_stale) {
+        for (int l = 0; l < 4; ++l)
+            for (auto& b : m->blocks[l])
+                if (b.has_ds && pack_fold(m, b, st)) return -1;
+        m->fold_stale = false;
+    }
     // model.py:248-252 + :73-76: normalise, stem conv/BN/ReLU, max-pool
     Act s0 = mk(m->S0, B, 256, 512, 64);
     {
@@ -533,23 +577,35 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
             Act t2 = mk(m->T2, B, Ho, Wo, blk.c2.d.Cout);
             Act y = mk(b == nb - 1 ? m->F[l] : m->X[b & 1], B, Ho, Wo, blk.c3.d.Cout);
             if (conv_bn(m, blk.c1, cur, t1, nullptr, st, CLS_ENC_CONV, tr)) return -1;
+            // eval forward on the tensor cores: the downsample runs inside conv3, one GEMM over [t2 | x] (no identity tensor)
+            const bool fold = blk.has_ds && !tr && m->use_tc && m->fold_on;
             const float* idn = cur.p;
-            if (blk.has_ds) {
+            if (blk.has_ds && !fold) {
                 Act d = mk(m->IDN, B, Ho, Wo, blk.ds.d.Cout);
                 if (conv_bn(m, blk.ds, cur, d, nullptr, st, CLS_ENC_CONV, tr)) return -1;
                 idn = d.p;
             }
-            if (!tr && m->use_tc && m->fuse_on && blk.c2.wq && blk.c3.wq && bott_tc_supported(blk.c2.d, blk.c3.d, t1, y)) {
+            const double conv3_k = blk.c3.d.Cin + (fold ? (double)blk.ds.d.Cin : 0.0);
+            if (!tr && m->use_tc && m->fuse_on && blk.c2.wq && blk.c3.wq && bott_tc_supported(blk.c2.d, blk.c3.d, t1, y) &&
+                (!fold || (cur.C == 64 && cur.H == t1.H && cur.W == t1.W))) {
                 // layer1: conv2 + conv3 in one kernel, the 64-channel intermediate stays in shared memory (conv_tc.cu)
-                const double flops = 2.0 * (double)B * Ho * Wo * (64.0 * 9 * 64 + (double)blk.c3.d.Cout * 64);
+                const double flops = 2.0 * (double)B * Ho * Wo * (64.0 * 9 * 64 + (double)blk.c3.d.Cout * conv3_k);
                 Scope sc(m, CLS_ENC_CONV, flops, st);
-                if (bott_tc_planes(blk.c2.d, blk.c2.wq, blk.c2.tc_scale, blk.c3.d, blk.c3.wq, blk.c3.tc_scale, t1,
+                const ConvLayer& c3 = fold ? blk.fold : blk.c3;
+                const unsigned short* idn_planes = reinterpret_cast<const unsigned short*>(idn);
+                if (bott_tc_planes(blk.c2.d, blk.c2.wq, blk.c2.tc_scale, blk.c3.d, c3.wq, c3.tc_scale, t1,
                                    reinterpret_cast<const unsigned short*>(t1.p), y, reinterpret_cast<unsigned short*>(y.p),
-                                   reinterpret_cast<const unsigned short*>(idn), st))
+                                   fold ? nullptr : idn_planes, fold ? idn_planes : nullptr, st))
                     return -1;
             } else {
                 if (conv_bn(m, blk.c2, t1, t2, nullptr, st, CLS_ENC_CONV, tr)) return -1;
-                if (conv_bn(m, blk.c3, t2, y, idn, st, CLS_ENC_CONV, tr)) return -1;   // + identity, ReLU
+                if (fold) {
+                    Scope sc(m, CLS_ENC_CONV, 2.0 * (double)B * Ho * Wo * blk.c3.d.Cout * conv3_k, st);
+                    if (conv_tc_fold_planes(blk.fold.wq, blk.fold.tc_scale, t2, reinterpret_cast<const unsigned short*>(t2.p),
+                                            cur, reinterpret_cast<const unsigned short*>(cur.p), s, y,
+                                            reinterpret_cast<unsigned short*>(y.p), st))
+                        return -1;
+                } else if (conv_bn(m, blk.c3, t2, y, idn, st, CLS_ENC_CONV, tr)) return -1;   // + identity, ReLU
             }
             cur = y;
         }
@@ -1095,6 +1151,39 @@ int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh,
                        p.dxr, p.parity, p.num_kc, p.seg, p.pf, p.n_tiles, p.num_tiles, p.grid};
     memcpy(plan, v, sizeof(v));
     return 0;
+}
+
+int hn_conv_tc_fold_plan(int B, int H, int W, int Cin, int Cmid, int Cout, int stride, int sms, int plan[18]) {
+    HN_CHECK(plan, "hn_conv_tc_fold_plan: NULL argument");
+    HN_CHECK(B >= 1 && H >= 1 && W >= 1 && (stride == 1 || stride == 2) && H % stride == 0 && W % stride == 0,
+             "hn_conv_tc_fold_plan: bad geometry");
+    const Act x = mk(nullptr, B, H, W, Cin), t2 = mk(nullptr, B, H / stride, W / stride, Cmid);
+    const Act o = mk(nullptr, B, H / stride, W / stride, Cout);
+    TcPlan p;
+    if (conv_tc_fold_plan(t2, x, stride, o, sms, &p)) return -1;
+    const int v[18] = {p.gemm_kernel, p.BN, p.mode, p.M, p.tw, p.rows_per_tile, p.wsegs, p.rows_per_tile > 1, p.box_rows,
+                       p.box_imgs, p.dxr, p.parity, p.num_kc, p.seg, p.pf, p.n_tiles, p.num_tiles, p.grid};
+    memcpy(plan, v, sizeof(v));
+    return 0;
+}
+
+int hn_conv_tc_fold(const float* t2, const float* x, int B, int H, int W, int Cin, int Cmid, int Cout, int stride,
+                    const float* w, const float* shift, float* out, void* stream) {
+    HN_CHECK(t2 && x && w && shift && out, "hn_conv_tc_fold: NULL argument");
+    HN_CHECK(B >= 1 && H >= 1 && W >= 1 && (stride == 1 || stride == 2) && H % stride == 0 && W % stride == 0,
+             "hn_conv_tc_fold: bad geometry");
+    const Act xa = mk(const_cast<float*>(x), B, H, W, Cin);
+    const Act ta = mk(const_cast<float*>(t2), B, H / stride, W / stride, Cmid);
+    const Act oa = mk(out, B, H / stride, W / stride, Cout);
+    return conv_tc_fold(w, shift, ta, xa, stride, oa, (cudaStream_t)stream);
+}
+
+int hn_bott_tc_fold(const float* in, const float* x, int B, int H, int W, const float* w2, const float* scale2,
+                    const float* shift2, const float* w3, const float* shift3, int C3, float* out, void* stream) {
+    HN_CHECK(in && x && w2 && scale2 && shift2 && w3 && shift3 && out, "hn_bott_tc_fold: NULL argument");
+    HN_CHECK(B >= 1 && H >= 1 && W >= 1 && C3 >= 64, "hn_bott_tc_fold: bad geometry");
+    return bott_tc_fold(w2, scale2, shift2, w3, shift3, mk(const_cast<float*>(in), B, H, W, 64),
+                        mk(const_cast<float*>(x), B, H, W, 64), mk(out, B, H, W, C3), (cudaStream_t)stream);
 }
 
 int hn_lstm_layer(const float* xproj, const float* whf, const float* whb, float* out, int T, int B, void* stream) {

@@ -95,7 +95,9 @@ struct hn_model {
 
     // graph
     ConvLayer stem;                                  // weights packed [147][64]
-    struct Block { ConvLayer c1, c2, c3, ds; bool has_ds = false; };
+    // fold (block 0, eval): conv3 + downsample as one 1x1 conv over [t2 | x]: w = [s3 W3 ; sd Wd] fp32 [Cout][K], shift =
+    // f3 + fd, wq / tc_scale their planes (conv_tc_fold_planes)
+    struct Block { ConvLayer c1, c2, c3, ds, fold; bool has_ds = false; };
     std::vector<Block> blocks[4];
     ConvLayer ghc[4][4];
     int use_rnn = 1;                                 // 0: per-column MLP head instead of the bi-LSTM (model.py:234-243)
@@ -109,9 +111,11 @@ struct hn_model {
     float* stem_aux = nullptr;                       // 3*64 + 1 epilogue constants
     int stem_tc_on = 1;                              // option "stem_tc" / HN_TC_STEM=0: fp32 CUDA-core stem inside the TC path
     int fuse_on = 1;                                 // option "fuse_bottleneck": fused conv2+conv3 kernel for layer1 (bit-identical)
+    int fold_on = 1;                                 // option "fold_downsample": block-0 downsample inside conv3 (eval, TC)
     // train-mode scratch (one layer at a time, stream ordered): batch sums, scale/shift, tensor-core epilogue constants
     std::shared_ptr<void> train_state;               // tape + gradient buffers of the training step (train_step.cu)
     bool bn_stale = false;     // running statistics moved (train forward) since the eval-mode constants were folded
+    bool fold_stale = true;    // weights or eval-mode BN constants changed since the folded block-0 packs were built
     double* trn_sums = nullptr;
     float *trn_scale = nullptr, *trn_shift = nullptr, *trn_aux = nullptr;
 

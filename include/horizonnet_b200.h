@@ -171,6 +171,9 @@ int hn_model_stage(hn_model* m, const char* stage, float* out_dev, long long cap
  * through the split-fp16 tensor-core path (default), 0 = exact fp32 CUDA-core kernels everywhere;
  * "stem_tc" = 1 (default; env HN_TC_STEM) runs the 7x7 stem on wgmma when "tensor_cores" is on, 0 = fp32 CUDA-core stem;
  * "fuse_bottleneck" = 1 (default; env HN_TC_FUSE) runs conv2 + conv3 of the layer1 bottlenecks as one kernel (bit-identical results);
+ * "fold_downsample" = 1 (default) runs the downsample of each layer's block 0 inside its conv3 in the eval forward on
+ * the tensor cores (one GEMM over [t2 | x] with both BN scales folded into the weights, no identity tensor), 0 = a
+ * launch of its own and conv3 with a residual;
  * "profile" = 1 turns on per-launch CUDA-event timing (see hn_model_profile_read). */
 int hn_model_set_option(hn_model* m, const char* name, int value);
 
@@ -267,6 +270,19 @@ int hn_conv2d_dgrad_tc(int B, int H, int W, int Cin, const float* w_oihw, const 
  * CTAs.  Reads HN_TC_DXR and HN_TC_GEMM like the launch.  -1 for a shape the kernel does not take. */
 int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
                     int out_halo, int out_f32, int has_residual, int sms, int plan[18]);
+/* The same plan (same 18 fields) for the eval-mode conv3 of a bottleneck's block 0 with its downsample folded in:
+ * relu([t2 | x at every stride-th pixel] . W + shift), x [B][H][W][Cin] (halo 1), t2 and the output [B][H/s][W/s][Cmid],
+ * [Cout]; K chunks = (Cmid + Cin) / 64, the first Cmid / 64 over t2.  -1 for a shape the kernel does not take. */
+int hn_conv_tc_fold_plan(int B, int H, int W, int Cin, int Cmid, int Cout, int stride, int sms, int plan[18]);
+/* That convolution on the tensor cores with fp32 tensors (unit tests): t2 / x / out halo-1 NHWC fp32 with circular halo
+ * columns in the geometry above, w the folded weights [Cout][Cmid + Cin], shift [Cout]. */
+int hn_conv_tc_fold(const float* t2, const float* x, int B, int H, int W, int Cin, int Cmid, int Cout, int stride,
+                    const float* w, const float* shift, float* out, void* stream);
+/* The fused layer1.0 bottleneck kernel with the downsample folded in (unit tests): in = conv1 output and x = block input,
+ * both [B][H][W][64] halo-1 NHWC fp32; w2 OIHW [64][64][3][3] with BN scale2 / shift2; w3 the folded conv3 weights
+ * [C3][64 + 64] with shift3; out [B][H][W][C3]. */
+int hn_bott_tc_fold(const float* in, const float* x, int B, int H, int W, const float* w2, const float* scale2,
+                    const float* shift2, const float* w3, const float* shift3, int C3, float* out, void* stream);
 int hn_bn_forward_backward(const float* z, int B, int H, int W, int C, const float* gamma, const float* beta,
                            float* running_mean, float* running_var, double factor, int train, int relu, const float* res,
                            float* y, const float* dy, float* dz, float* dres, float* dgamma, float* dbeta, float* bn_scratch,

@@ -1,13 +1,13 @@
 """Per-launch time of every convolution of the plain resnet50_rnn forward (batch 32, 512 x 1024), from torch.profiler.
 
 The tensor-core convolution kernels (conv_tc_kernel, gemm_tc_kernel, bott_tc_kernel) run in a fixed order per forward:
-the units of tests/tc_cases.resnet50_rnn_convs (layer1's conv2 + conv3 fused into one bott_tc_kernel), then the two LSTM
-input projections.  Each launch is listed with its plan (hn_conv_tc_plan), its algorithmic FLOPs and a model of the
+the units of tests/tc_cases.resnet50_rnn_convs (layer1's conv2 + conv3 fused into one bott_tc_kernel; with the model option
+fold_downsample, the default, each block-0 downsample inside its conv3), then the two LSTM input projections.  Each launch is listed with its plan (hn_conv_tc_plan), its algorithmic FLOPs and a model of the
 operand bytes it pulls from L2 into shared memory.  The HN_TC_* switches in the environment apply, so run one process
 per setting; with programmatic dependent launch on (the default) a kernel's duration includes the time it waits for
 its predecessor, HN_TC_PDL=0 gives the clean attribution.
 
-    python profiles/conv_launches.py --out table.json [--reps 5]
+    python profiles/conv_launches.py --out table.json [--reps 5] [--fold-downsample 0]
 """
 import argparse
 import json
@@ -25,20 +25,45 @@ B = 32
 CONV_KERNELS = ('conv_tc_kernel', 'gemm_tc_kernel', 'bott_tc_kernel')
 
 
-def expected_launches():
-    """(name, launch dict or None for the fused layer1 bottleneck) in forward order."""
+def expected_launches(fold=False):
+    """(name, launch dict or None for the fused layer1 bottleneck) in forward order.  fold: the model option
+    fold_downsample (on by default) -- no downsample launches; the block-0 conv3 of layers 2-4 runs as one two-source
+    launch over [t2 | x] (a 'fold' launch dict, plan_of), layer1.0's inside bott_tc_kernel."""
     import tc_cases as T
+    convs = T.resnet50_rnn_convs()
+    ds = {n.rsplit('.', 1)[0]: (H, W, Ci, st[0]) for n, H, W, Ci, Co, k, st in convs if n.endswith('downsample')}
     out = []
-    for name, H, W, Ci, Co, k, st in T.resnet50_rnn_convs():
+    for name, H, W, Ci, Co, k, st in convs:
+        blk = name.rsplit('.', 1)[0]
+        if fold and name.endswith('downsample'):
+            continue
         if name.startswith('layer1') and name.endswith('conv3'):
             continue
         if name.startswith('layer1') and name.endswith('conv2'):
             out.append((name[:-1] + '2+conv3', None))
             continue
+        if fold and name.endswith('conv3') and blk in ds:
+            Hx, Wx, Cx, s = ds[blk]
+            out.append((name + '+downsample', dict(name=name + '+downsample', fold=True, B=B, H=Hx, W=Wx, Cin=Cx, Cmid=Ci,
+                                                   Cout=Co, k=1, stride=(s, s))))
+            continue
         out.append((name, T.launch(name, B, H, W, Ci, Co, k, st, residual=name.endswith('conv3'))))
     for layer in range(2):
         out.append((f'xproj{layer}', T.launch(f'xproj{layer}', 1, 1, 256 * B, 1024, 4096, 1, (1, 1), 0, 0, out_f32=True)))
     return out
+
+
+def plan_of(c):
+    """hn_conv_tc_plan of a launch dict, or hn_conv_tc_fold_plan of a fold launch."""
+    import ctypes
+    import tc_cases as T
+    from horizonnet_b200 import _lib
+    if not c.get('fold'):
+        return T.plan(c)
+    out = (ctypes.c_int * len(T.PLAN_FIELDS))()
+    rc = _lib.lib().hn_conv_tc_fold_plan(c['B'], c['H'], c['W'], c['Cin'], c['Cmid'], c['Cout'], c['stride'][0], T.SMS,
+                                         out)
+    return dict(zip(T.PLAN_FIELDS, out)) if rc == 0 else None
 
 
 def model_bytes(c, p):
@@ -80,6 +105,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', required=True)
     ap.add_argument('--reps', type=int, default=5)
+    ap.add_argument('--fold-downsample', type=int, choices=(0, 1), default=1, help='model option fold_downsample')
     args = ap.parse_args()
 
     import torch
@@ -96,6 +122,8 @@ def main():
     net = net.to(dev)
     x = synthetic_panoramas(B, seed=1000).to(dev)
     with torch.no_grad():
+        net(x)                                      # creates the handle the option applies to
+        net.set_option('fold_downsample', args.fold_downsample)
         for _ in range(3):
             net(x)
     torch.cuda.synchronize()
@@ -107,7 +135,7 @@ def main():
     kern = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
             and any(k in e.name for k in CONV_KERNELS)]
     kern.sort(key=lambda e: e.time_range.start)
-    exp = expected_launches()
+    exp = expected_launches(fold=bool(args.fold_downsample))
     if len(kern) != args.reps * len(exp):
         with open(args.out, 'w') as f:
             json.dump({'error': 'launch count', 'kernels': [e.name for e in kern]}, f, indent=1)
@@ -121,14 +149,14 @@ def main():
                'us': us[len(us) // 2],
                'us_min': us[0], 'us_max': us[-1]}
         if c is not None:
-            p = T.plan(c)
+            p = plan_of(c)
             if p is None:
                 raise SystemExit(f'conv_launches.py: no plan for {name}')
             want = 'gemm_tc_kernel' if p['gemm_kernel'] else f'conv_tc_kernel<{p["BN"]}>'
             if want not in row['kernel']:
                 raise SystemExit(f'conv_launches.py: launch {i} ({name}) ran {row["kernel"]}, the plan says {want}')
             Ho, Wo = c['H'] // c['stride'][0], c['W'] // c['stride'][1]
-            flops = 2.0 * c['B'] * Ho * Wo * c['Cout'] * c['Cin'] * c['k'] * c['k']
+            flops = 2.0 * c['B'] * Ho * Wo * c['Cout'] * (c['Cin'] * c['k'] * c['k'] + c.get('Cmid', 0))
             row.update({f: p[f] for f in ('BN', 'mode', 'dxr', 'box_rows', 'parity', 'num_kc', 'n_tiles', 'num_tiles',
                                            'grid')})
             row['gflop'] = round(flops / 1e9, 3)
@@ -141,7 +169,7 @@ def main():
     for r in rows:
         f = r['name'].split('.')[0]
         fam[f] = round(fam.get(f, 0.0) + r['us'] / 1e3, 3)
-    res = {'card': card(), 'batch': B, 'reps': args.reps, 'env': env,
+    res = {'card': card(), 'batch': B, 'reps': args.reps, 'env': env, 'options': {'fold_downsample': args.fold_downsample},
            'what': 'median device duration over the reps of each convolution launch of the plain forward (torch.profiler)',
            'family_ms': fam, 'conv_tc_kernel_ms': round(sum(r['us'] for r in rows if 'conv_tc_kernel' in r['kernel']) / 1e3, 3),
            'total_ms': round(sum(r['us'] for r in rows) / 1e3, 3),
