@@ -8,7 +8,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libhorizonnet_b200.so')
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 _lib = None
 _lock = threading.Lock()
@@ -26,6 +26,7 @@ SIGNATURES = {
     'hn_kernel_launches': (ctypes.c_longlong, []),
     'hn_model_create': (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.POINTER(vp)]),
     'hn_model_create_head': (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(vp)]),
+    'hn_model_create_arch': (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(vp)]),
     'hn_model_num_tensors': (ctypes.c_int, [vp]),
     'hn_model_tensor_info': (ctypes.c_int, [vp, ctypes.c_int, ctypes.POINTER(ctypes.c_char_p),
                                             ctypes.POINTER(ctypes.c_longlong)]),

@@ -499,16 +499,17 @@ __global__ void maxpool_bwd_kernel(const float* __restrict__ x, const float* __r
 struct GhcDst {
     float* p[4];
     int H[4], W[4], C[4], chan_off[4];
+    int lg;                   // log2 of the sequence width (1024 or 256)
 };
 
 // adjoint of ghc_to_sequence_kernel (tail.cu): scatter d seq[t][b][ch] to the two source columns it interpolated
 __global__ void ghc_to_sequence_bwd_kernel(const float* __restrict__ dseq, const GhcDst s, int B) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t total = (size_t)256 * B * 1024;
+    const size_t total = ((size_t)256 * B) << s.lg;
     if (i >= total) return;
-    const int ch = (int)(i & 1023);
-    const int b = (int)((i >> 10) % B);
-    const int t = (int)((i >> 10) / B);
+    const int ch = (int)(i & ((1u << s.lg) - 1));
+    const int b = (int)((i >> s.lg) % B);
+    const int t = (int)((i >> s.lg) / B);
     int sc = 3;
     if (ch < s.chan_off[1]) sc = 0; else if (ch < s.chan_off[2]) sc = 1; else if (ch < s.chan_off[3]) sc = 2;
     const int H = s.H[sc], W = s.W[sc], C = s.C[sc];
@@ -1091,8 +1092,9 @@ int ghc_to_sequence_bwd(const float* dseq, const Act dghc[4], cudaStream_t st) {
         s.p[i] = dghc[i].p; s.H[i] = dghc[i].H; s.W[i] = dghc[i].W; s.C[i] = dghc[i].C; s.chan_off[i] = off;
         off += dghc[i].C * dghc[i].H;
     }
-    HN_CHECK(off == 1024, "ghc_to_sequence_bwd: the 4 scales must flatten to 1024 channels");
-    const size_t total = (size_t)256 * dghc[0].B * 1024;
+    HN_CHECK((off == 1024 || off == 256), "ghc_to_sequence_bwd: the 4 scales must flatten to 1024 or 256 channels");
+    s.lg = off == 1024 ? 10 : 8;
+    const size_t total = (size_t)256 * dghc[0].B * off;
     ghc_to_sequence_bwd_kernel<<<blocks_for(total), 256, 0, st>>>(dseq, s, dghc[0].B);
     HN_LAUNCH_OK();
     return 0;

@@ -1,5 +1,5 @@
 // hn_model: weight registry (reference checkpoint layout, misc/utils.py:49-65), BN folding and
-// weight packing, activation workspace, and the forward schedule of HorizonNet('resnet50', rnn)
+// weight packing, activation workspace, and the forward schedule of HorizonNet('resnet50' or 'resnet18', rnn)
 // (reference model.py:254-281), plus the C ABI (include/horizonnet_b200.h).
 #include <algorithm>
 #include <cstring>
@@ -112,15 +112,15 @@ __global__ void rows_to_batch_major_kernel(const float* __restrict__ in, float* 
     out[i] = in[((size_t)t * B + b) * C + c];
 }
 
-// seq [T][B][1024] -> feature [B][1024][T]
-__global__ void seq_to_feature_kernel(const float* __restrict__ seq, float* __restrict__ out, int T, int B) {
+// seq [T][B][C] -> feature [B][C][T]
+__global__ void seq_to_feature_kernel(const float* __restrict__ seq, float* __restrict__ out, int T, int B, int C) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t total = (size_t)T * B * 1024;
+    const size_t total = (size_t)T * B * C;
     if (i >= total) return;
     const int t = (int)(i % T);
-    const int ch = (int)((i / T) % 1024);
-    const int b = (int)(i / T / 1024);
-    out[i] = seq[((size_t)t * B + b) * 1024 + ch];
+    const int ch = (int)((i / T) % C);
+    const int b = (int)(i / T / C);
+    out[i] = seq[((size_t)t * B + b) * C + ch];
 }
 
 }  // namespace
@@ -145,31 +145,47 @@ ConvLayer make_conv(hn_model* m, const std::string& wkey, const std::string& bn,
     return c;
 }
 
-// Builds the key list in the reference's own order (tests/golden/state_dict_keys.json) and the graph.
-void build_graph(hn_model* m) {
+// The encoders the library builds (torchvision resnet.py): block kind, blocks per layer, channel expansion
+struct Arch {
+    const char* name;
+    hn_model::Kind kind;
+    int nblk[4];
+    int expansion;
+};
+const Arch ARCHS[] = {{"resnet50", hn_model::BOTTLENECK, {3, 4, 6, 3}, 4}, {"resnet18", hn_model::BASIC, {2, 2, 2, 2}, 1}};
+
+int block_out_channels(const hn_model::Block& b) { return b.kind == hn_model::BASIC ? b.c2.d.Cout : b.c3.d.Cout; }
+
+// Builds the key list in the reference's own order (tests/golden/state_dict_keys*.json) and the graph.
+void build_graph(hn_model* m, const Arch& arch) {
     const std::string enc = "feature_extractor.encoder.";
     m->stem = make_conv(m, enc + "conv1.1.weight", enc + "bn1", "", 3, 64, 7, 2, 2, 1);
-    const int nblk[4] = {3, 4, 6, 3};
     const int planes[4] = {64, 128, 256, 512};
     int inpl = 64;
     for (int l = 0; l < 4; ++l) {
-        for (int b = 0; b < nblk[l]; ++b) {
+        const int cout = planes[l] * arch.expansion;
+        for (int b = 0; b < arch.nblk[l]; ++b) {
             const std::string p = enc + "layer" + std::to_string(l + 1) + "." + std::to_string(b) + ".";
             const int stride = (b == 0 && l > 0) ? 2 : 1;
             hn_model::Block blk;
-            blk.c1 = make_conv(m, p + "conv1.weight", p + "bn1", "", inpl, planes[l], 1, 1, 1, 1);
-            blk.c2 = make_conv(m, p + "conv2.1.weight", p + "bn2", "", planes[l], planes[l], 3, stride, stride, 1);
-            blk.c3 = make_conv(m, p + "conv3.weight", p + "bn3", "", planes[l], planes[l] * 4, 1, 1, 1, 1);
-            blk.has_ds = (b == 0);
+            blk.kind = arch.kind;
+            if (arch.kind == hn_model::BOTTLENECK) {
+                blk.c1 = make_conv(m, p + "conv1.weight", p + "bn1", "", inpl, planes[l], 1, 1, 1, 1);
+                blk.c2 = make_conv(m, p + "conv2.1.weight", p + "bn2", "", planes[l], planes[l], 3, stride, stride, 1);
+                blk.c3 = make_conv(m, p + "conv3.weight", p + "bn3", "", planes[l], cout, 1, 1, 1, 1);
+            } else {       // BasicBlock: conv1 3x3 carries the stride, conv2 3x3 + identity
+                blk.c1 = make_conv(m, p + "conv1.1.weight", p + "bn1", "", inpl, planes[l], 3, stride, stride, 1);
+                blk.c2 = make_conv(m, p + "conv2.1.weight", p + "bn2", "", planes[l], cout, 3, 1, 1, 1);
+            }
+            blk.has_ds = (b == 0) && (stride != 1 || inpl != cout);
             if (blk.has_ds)
-                blk.ds = make_conv(m, p + "downsample.0.weight", p + "downsample.1", "", inpl, planes[l] * 4, 1, stride,
-                                   stride, 0);
-            inpl = planes[l] * 4;
+                blk.ds = make_conv(m, p + "downsample.0.weight", p + "downsample.1", "", inpl, cout, 1, stride, stride, 0);
+            inpl = cout;
             m->blocks[l].push_back(blk);
         }
     }
     for (int s = 0; s < 4; ++s) {
-        const int c = planes[s] * 4;
+        const int c = planes[s] * arch.expansion;
         const int ch[5] = {c, c / 2, c / 2, c / 4, c / 8};
         for (int j = 0; j < 4; ++j) {
             const std::string p =
@@ -177,21 +193,24 @@ void build_graph(hn_model* m) {
             m->ghc[s][j] = make_conv(m, p + "0.1.weight", p + "1", p + "0.1.bias", ch[j], ch[j + 1], 3, 2, 1, 1);
         }
     }
+    m->c_last = 0;                                   // model.py:175-178: C/8 channels at H = 8, 4, 2, 1 per scale
+    for (int s = 0; s < 4; ++s) m->c_last += m->ghc[s][3].d.Cout * (8 >> s);
+    const int K0 = m->c_last;
     if (!m->use_rnn) {
-        // model.py:234-243: Linear(1024, 512), ReLU, Dropout, Linear(512, 12)
-        m->add_slot("linear.0.weight", 512ll * 1024);
+        // model.py:234-243: Linear(c_last, 512), ReLU, Dropout, Linear(512, 12)
+        m->add_slot("linear.0.weight", 512ll * K0);
         m->add_slot("linear.0.bias", 512);
         m->add_slot("linear.3.weight", 12 * 512);
         m->add_slot("linear.3.bias", 12);
         ConvLayer& c = m->mlp1;
-        c.d.Cin = 1024; c.d.Cout = 512; c.d.kh = c.d.kw = 1; c.d.sh = c.d.sw = 1; c.d.ph = c.d.pw = 0; c.d.relu = 1;
+        c.d.Cin = K0; c.d.Cout = 512; c.d.kh = c.d.kw = 1; c.d.sh = c.d.sw = 1; c.d.ph = c.d.pw = 0; c.d.relu = 1;
         c.wkey = "linear.0.weight"; c.biaskey = "linear.0.bias";
         return;
     }
     for (int layer = 0; layer < 2; ++layer)
         for (int dir = 0; dir < 2; ++dir) {
             const std::string sfx = "_l" + std::to_string(layer) + (dir ? "_reverse" : "");
-            m->add_slot("bi_rnn.weight_ih" + sfx, 2048ll * 1024);
+            m->add_slot("bi_rnn.weight_ih" + sfx, 2048ll * (layer == 0 ? K0 : 1024));
             m->add_slot("bi_rnn.weight_hh" + sfx, 2048ll * 512);
             m->add_slot("bi_rnn.bias_ih" + sfx, 2048);
             m->add_slot("bi_rnn.bias_hh" + sfx, 2048);
@@ -200,7 +219,8 @@ void build_graph(hn_model* m) {
     m->add_slot("linear.bias", 12);
     for (int layer = 0; layer < 2; ++layer) {
         ConvLayer& c = m->xproj[layer];
-        c.d.Cin = 1024; c.d.Cout = 4096; c.d.kh = c.d.kw = 1; c.d.sh = c.d.sw = 1; c.d.ph = c.d.pw = 0; c.d.relu = 0;
+        c.d.Cin = layer == 0 ? K0 : 1024; c.d.Cout = 4096; c.d.kh = c.d.kw = 1; c.d.sh = c.d.sw = 1; c.d.ph = c.d.pw = 0;
+        c.d.relu = 0;
     }
 }
 
@@ -254,8 +274,13 @@ int run_conv(hn_model* m, const ConvLayer& c, const Act& in, const Act& out, con
     Scope sc(m, cls, flops, st);
     if (!m->use_tc) return conv_f32(c.d, in, out, res, st);
     // tensor-core path: every activation buffer holds fp16 hi/lo planes (same bytes as fp32)
-    if (!c.wq || !conv_tc_supported(c.d, in, out))
+    if (!c.wq || !conv_tc_supported(c.d, in, out)) {
+        // resnet18's narrow height-reduction convs (Cin 16 / 32): fp32 CUDA-core kernel on the same planes (conv_narrow.cu)
+        if (!res && !out_f32 && conv_narrow_supported(c.d, in, out))
+            return conv_narrow_planes(c.d, in, reinterpret_cast<const unsigned short*>(in.p), out,
+                                      reinterpret_cast<unsigned short*>(out.p), st);
         return fail("hn_model_forward: a convolution of the graph is not covered by the tensor-core kernel");
+    }
     return conv_tc_planes(c.d, c.wq, c.tc_scale, in, reinterpret_cast<const unsigned short*>(in.p), out,
                           out_f32 ? nullptr : reinterpret_cast<unsigned short*>(out.p), out_f32 ? out.p : nullptr,
                           reinterpret_cast<const unsigned short*>(res), st);
@@ -266,7 +291,8 @@ int refold_bn(hn_model* m, cudaStream_t st) {
     std::vector<ConvLayer*> all{&m->stem};
     for (int l = 0; l < 4; ++l)
         for (auto& b : m->blocks[l]) {
-            all.push_back(&b.c1); all.push_back(&b.c2); all.push_back(&b.c3);
+            all.push_back(&b.c1); all.push_back(&b.c2);
+            if (b.kind == hn_model::BOTTLENECK) all.push_back(&b.c3);
             if (b.has_ds) all.push_back(&b.ds);
         }
     for (int s = 0; s < 4; ++s)
@@ -297,7 +323,8 @@ int conv_bn(hn_model* m, const ConvLayer& c, const Act& in, const Act& out, cons
     ConvLayer t = c;
     t.d.relu = 0; t.d.scale = m->trn_scale; t.d.shift = m->trn_shift; t.tc_scale = m->trn_aux;
     if (bn_identity_constants(bias, m->trn_scale, m->trn_shift, C, st)) return -1;
-    if (m->use_tc && tc_aux_update(m->trn_scale, m->trn_shift, c.tc_scale + 3 * C, m->trn_aux, C, st)) return -1;
+    // (the narrow convs have no weight planes: their kernel reads trn_scale / trn_shift directly)
+    if (m->use_tc && c.tc_scale && tc_aux_update(m->trn_scale, m->trn_shift, c.tc_scale + 3 * C, m->trn_aux, C, st)) return -1;
     if (run_conv(m, t, in, out, nullptr, st, cls)) return -1;
     if (bn_batch_stats(out, m->use_tc != 0, m->trn_sums, st)) return -1;
     if (bn_train_finalize(m->trn_sums, (long long)out.B * out.H * out.W, m->T(c.bnprefix + ".weight"),
@@ -305,7 +332,7 @@ int conv_bn(hn_model* m, const ConvLayer& c, const Act& in, const Act& out, cons
                           const_cast<float*>(m->T(c.bnprefix + ".running_var")), tr->bn_factor[c.bn_index],
                           m->trn_scale, m->trn_shift, C, st))
         return -1;
-    if (m->use_tc && tc_aux_update(m->trn_scale, m->trn_shift, c.tc_scale + 3 * C, m->trn_aux, C, st)) return -1;
+    if (m->use_tc && c.tc_scale && tc_aux_update(m->trn_scale, m->trn_shift, c.tc_scale + 3 * C, m->trn_aux, C, st)) return -1;
     t.d.relu = c.d.relu;
     return run_conv(m, t, in, out, res, st, cls);
 }
@@ -316,16 +343,24 @@ int conv_bn(hn_model* m, const ConvLayer& c, const Act& in, const Act& out, cons
 extern "C" {
 
 const char* hn_last_error(void) { return g_err.c_str(); }
-int hn_abi_version(void) { return 5; }
+int hn_abi_version(void) { return 6; }
 const char* hn_build_digest(void) { return HN_BUILD_DIGEST; }
 long long hn_kernel_launches(void) { return g_launches.load(); }
 
-int hn_model_create(int device, int max_batch, hn_model** out) { return hn_model_create_head(device, max_batch, 1, out); }
+int hn_model_create(int device, int max_batch, hn_model** out) { return hn_model_create_arch(device, max_batch, "resnet50", 1, out); }
 
 int hn_model_create_head(int device, int max_batch, int use_rnn, hn_model** out) {
-    HN_CHECK(out != nullptr, "hn_model_create: out is NULL");
+    return hn_model_create_arch(device, max_batch, "resnet50", use_rnn, out);
+}
+
+int hn_model_create_arch(int device, int max_batch, const char* backbone, int use_rnn, hn_model** out) {
+    HN_CHECK(out != nullptr && backbone != nullptr, "hn_model_create: NULL argument");
     HN_CHECK(max_batch >= 1 && max_batch <= 1024, "hn_model_create: max_batch must be in 1..1024");
     HN_CHECK(use_rnn == 0 || use_rnn == 1, "hn_model_create_head: use_rnn must be 0 or 1");
+    const Arch* arch = nullptr;
+    for (const Arch& a : ARCHS)
+        if (std::strcmp(a.name, backbone) == 0) arch = &a;
+    if (!arch) return fail(std::string("hn_model_create_arch: unsupported backbone '") + backbone + "' (resnet50, resnet18)");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return fail("hn_model_create: no CUDA device -- libhorizonnet_b200 has no CPU path");
@@ -339,27 +374,59 @@ int hn_model_create_head(int device, int max_batch, int use_rnn, hn_model** out)
     m->max_batch = max_batch;
     m->use_rnn = use_rnn;
     if (const char* e = getenv("HN_TC_STEM")) m->stem_tc_on = atoi(e);
-    build_graph(m.get());
+    build_graph(m.get(), *arch);
     for (auto& s : m->slots)
         if (!s.ignored && m->alloc_t(&s.dev, (size_t)s.numel)) return -1;
     const size_t B = (size_t)max_batch;
+    const size_t CL = (size_t)m->c_last;
+    // encoder workspace from the graph, per image: X block outputs, F stage outputs, T1 / T2 the intermediates of a
+    // block, IDN its downsample, G / GO the height reduction (halo-NHWC: H x (W + 2) x C)
+    size_t x_img = 0, t1_img = 0, t2_img = 0, idn_img = 0, f_img[4] = {0, 0, 0, 0}, g_img = 0, go_img[4] = {0, 0, 0, 0};
+    {
+        auto px = [](int h, int w, int c) { return (size_t)h * (w + 2) * c; };
+        int H = 128, W = 256;                              // after the stem and the max-pool
+        for (int l = 0; l < 4; ++l) {
+            const int nb = (int)m->blocks[l].size();
+            for (int b = 0; b < nb; ++b) {
+                const hn_model::Block& blk = m->blocks[l][b];
+                const bool basic = blk.kind == hn_model::BASIC;
+                const int s = basic ? blk.c1.d.sh : blk.c2.d.sh, Ho = H / s, Wo = W / s;
+                t1_img = std::max(t1_img, basic ? px(Ho, Wo, blk.c1.d.Cout) : px(H, W, blk.c1.d.Cout));
+                if (!basic) t2_img = std::max(t2_img, px(Ho, Wo, blk.c2.d.Cout));
+                if (blk.has_ds) idn_img = std::max(idn_img, px(Ho, Wo, blk.ds.d.Cout));
+                const size_t y = px(Ho, Wo, block_out_channels(blk));
+                if (b == nb - 1) f_img[l] = y; else x_img = std::max(x_img, y);
+                H = Ho; W = Wo;
+            }
+            int h = H;
+            for (int j = 0; j < 4; ++j) {
+                h /= 2;
+                const size_t o = px(h, W, m->ghc[l][j].d.Cout);
+                if (j == 3) go_img[l] = o; else g_img = std::max(g_img, o);
+            }
+        }
+    }
+    // X[0] is also the stem's packed-input scratch (stem_tc) and the plane-merge scratch of hn_model_stage("layerN")
+    const size_t x0 = std::max({x_img * B, (stem_tc_scratch_bytes((int)B) + 3) / 4, f_img[0] * B, f_img[1] * B,
+                                f_img[2] * B, f_img[3] * B});
+    m->x0_cap = x0;
     if (!use_rnn) {
         // MLP head: no projections / recurrence buffers.  XP stays as scratch: stem weight packing at finalize and the
         // plane merge of the "feature" test stage.
         struct { float** p; size_t n; } head_bufs[] = {
-            {&m->XP, std::max((size_t)256 * B * 1024, (size_t)4096 * 1024)},
+            {&m->XP, std::max((size_t)256 * B * CL, (size_t)4096 * 1024)},
             {&m->HID, 256 * B * 512}, {&m->HIDD, 256 * B * 512},
         };
         for (auto& b : head_bufs)
             if (m->alloc_t(b.p, b.n)) return -1;
     }
     struct { float** p; size_t n; } bufs[] = {
-        {&m->S0, B * 256 * 514 * 64},   {&m->S1, B * 128 * 258 * 64},  {&m->X[0], B * 128 * 258 * 256},
-        {&m->X[1], B * 128 * 258 * 256}, {&m->IDN, B * 128 * 258 * 256}, {&m->T1, B * 128 * 258 * 128},
-        {&m->T2, B * 128 * 258 * 64},   {&m->F[0], B * 128 * 258 * 256}, {&m->F[1], B * 64 * 130 * 512},
-        {&m->F[2], B * 32 * 66 * 1024}, {&m->F[3], B * 16 * 34 * 2048}, {&m->G[0], B * 64 * 258 * 128},
-        {&m->G[1], B * 64 * 258 * 128}, {&m->GO[0], B * 8 * 258 * 32},  {&m->GO[1], B * 4 * 130 * 64},
-        {&m->GO[2], B * 2 * 66 * 128},  {&m->GO[3], B * 1 * 34 * 256},  {&m->SEQ, 256 * B * 1024},
+        {&m->S0, B * 256 * 514 * 64},   {&m->S1, B * 128 * 258 * 64},  {&m->X[0], x0},
+        {&m->X[1], B * x_img},          {&m->IDN, B * idn_img},        {&m->T1, B * t1_img},
+        {&m->T2, B * t2_img},           {&m->F[0], B * f_img[0]},      {&m->F[1], B * f_img[1]},
+        {&m->F[2], B * f_img[2]},       {&m->F[3], B * f_img[3]},      {&m->G[0], B * g_img},
+        {&m->G[1], B * g_img},          {&m->GO[0], B * go_img[0]},    {&m->GO[1], B * go_img[1]},
+        {&m->GO[2], B * go_img[2]},     {&m->GO[3], B * go_img[3]},    {&m->SEQ, 256 * B * CL},
         {&m->x_in, B * 3 * 512 * 1024}, {&m->bon_out, B * 2 * 1024},    {&m->cor_out, B * 1024},
         {&m->x_slot[1], B * 3 * 512 * 1024},
         {&m->bon_slot[1], B * 2 * 1024},  {&m->cor_slot[1], B * 1024},
@@ -455,25 +522,28 @@ int hn_model_finalize(hn_model* m) {
     if (stem_tc_pack_weights(m->T(m->stem.wkey), m->XP, m->stem_wq, m->stem.scale, m->stem.shift, m->stem_aux, st)) return -1;
     for (int l = 0; l < 4; ++l)
         for (auto& b : m->blocks[l]) {
-            if (pack_conv(m, b.c1, st) || pack_conv(m, b.c2, st) || pack_conv(m, b.c3, st)) return -1;
-            if (b.has_ds && (pack_conv(m, b.ds, st) || alloc_fold(m, b))) return -1;
+            if (pack_conv(m, b.c1, st) || pack_conv(m, b.c2, st)) return -1;
+            if (b.kind == hn_model::BOTTLENECK && pack_conv(m, b.c3, st)) return -1;
+            if (b.has_ds && pack_conv(m, b.ds, st)) return -1;
+            if (b.has_ds && b.kind == hn_model::BOTTLENECK && alloc_fold(m, b)) return -1;
         }
     m->fold_stale = true;
     for (int s = 0; s < 4; ++s)
         for (int j = 0; j < 4; ++j)
             if (pack_conv(m, m->ghc[s][j], st)) return -1;
     if (!m->use_rnn) {
-        // MLP layer 1: OIHW [512][1024] -> [K=1024][N=512], epilogue 1 * acc + linear.0.bias, ReLU in the kernel
+        // MLP layer 1: OIHW [512][K] -> [K][N=512] (K = c_last), epilogue 1 * acc + linear.0.bias, ReLU in the kernel
         ConvLayer& c = m->mlp1;
+        const int K = m->c_last;
         if (!c.w) {
-            if (m->alloc_t(&c.w, (size_t)512 * 1024) || m->alloc_t(&c.scale, 512) || m->alloc_t(&c.shift, 512)) return -1;
-            if (m->alloc_t(&c.wq, (size_t)2 * 512 * 1024) || m->alloc_t(&c.tc_scale, 3 * 512 + 1)) return -1;
+            if (m->alloc_t(&c.w, (size_t)512 * K) || m->alloc_t(&c.scale, 512) || m->alloc_t(&c.shift, 512)) return -1;
+            if (m->alloc_t(&c.wq, (size_t)2 * 512 * K) || m->alloc_t(&c.tc_scale, 3 * 512 + 1)) return -1;
         }
-        pack_oihw_kernel<<<(512 * 1024 + 255) / 256, 256, 0, st>>>(m->T(c.wkey), c.w, 512, 1024, 1, 1);
+        pack_oihw_kernel<<<(512 * K + 255) / 256, 256, 0, st>>>(m->T(c.wkey), c.w, 512, K, 1, 1);
         HN_LAUNCH_OK();
         bias_constants_kernel<<<2, 256, 0, st>>>(m->T(c.biaskey), c.scale, c.shift, 512);
         HN_LAUNCH_OK();
-        if (pack_weight_tc(m->T(c.wkey), c.wq, c.scale, c.shift, c.tc_scale, c.tc_scale + 3 * 512, 512, 1024, 1, 1, st)) return -1;
+        if (pack_weight_tc(m->T(c.wkey), c.wq, c.scale, c.shift, c.tc_scale, c.tc_scale + 3 * 512, 512, K, 1, 1, st)) return -1;
         c.d.w = c.w; c.d.scale = c.scale; c.d.shift = c.shift;
         HN_CUDA_OK(cudaMemcpyAsync(m->head_w, m->T("linear.3.weight"), 12 * 512 * sizeof(float), cudaMemcpyDeviceToDevice, st));
         HN_CUDA_OK(cudaMemcpyAsync(m->head_b, m->T("linear.3.bias"), 12 * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -484,26 +554,27 @@ int hn_model_finalize(hn_model* m) {
     }
     for (int layer = 0; layer < 2; ++layer) {
         ConvLayer& c = m->xproj[layer];
+        const int K = c.d.Cin;                       // c_last for layer 0, 1024 for layer 1
         if (!c.w) {
-            if (m->alloc_t(&c.w, (size_t)4096 * 1024) || m->alloc_t(&c.scale, 4096) || m->alloc_t(&c.shift, 4096)) return -1;
-            if (m->alloc_t(&c.wq, (size_t)2 * 4096 * 1024) || m->alloc_t(&c.tc_scale, 3 * 4096 + 1)) return -1;
+            if (m->alloc_t(&c.w, (size_t)4096 * K) || m->alloc_t(&c.scale, 4096) || m->alloc_t(&c.shift, 4096)) return -1;
+            if (m->alloc_t(&c.wq, (size_t)2 * 4096 * K) || m->alloc_t(&c.tc_scale, 3 * 4096 + 1)) return -1;
         }
         const std::string l = "_l" + std::to_string(layer);
-        // [4096][1024] (fwd rows then reverse rows) -> [K=1024][N=4096]
+        // [4096][K] (fwd rows then reverse rows) -> [K][N=4096]
         for (int dir = 0; dir < 2; ++dir) {
             const float* w = m->T("bi_rnn.weight_ih" + l + (dir ? "_reverse" : ""));
-            HN_CUDA_OK(cudaMemcpyAsync(m->XP + (size_t)dir * 2048 * 1024, w, (size_t)2048 * 1024 * sizeof(float),
+            HN_CUDA_OK(cudaMemcpyAsync(m->XP + (size_t)dir * 2048 * K, w, (size_t)2048 * K * sizeof(float),
                                        cudaMemcpyDeviceToDevice, st));
             m->whh[layer][dir] = m->T("bi_rnn.weight_hh" + l + (dir ? "_reverse" : ""));
         }
-        pack_oihw_kernel<<<(4096 * 1024 + 255) / 256, 256, 0, st>>>(m->XP, c.w, 4096, 1024, 1, 1);
+        pack_oihw_kernel<<<(4096 * K + 255) / 256, 256, 0, st>>>(m->XP, c.w, 4096, K, 1, 1);
         HN_LAUNCH_OK();
 
         lstm_bias_kernel<<<16, 256, 0, st>>>(m->T("bi_rnn.bias_ih" + l), m->T("bi_rnn.bias_hh" + l),
                                              m->T("bi_rnn.bias_ih" + l + "_reverse"),
                                              m->T("bi_rnn.bias_hh" + l + "_reverse"), c.scale, c.shift);
         HN_LAUNCH_OK();
-        if (pack_weight_tc(m->XP, c.wq, c.scale, c.shift, c.tc_scale, c.tc_scale + 3 * 4096, 4096, 1024, 1, 1, st)) return -1;
+        if (pack_weight_tc(m->XP, c.wq, c.scale, c.shift, c.tc_scale, c.tc_scale + 3 * 4096, 4096, K, 1, 1, st)) return -1;
         c.d.w = c.w; c.d.scale = c.scale; c.d.shift = c.shift;
     }
     HN_CUDA_OK(cudaMemcpyAsync(m->head_w, m->T("linear.weight"), 12 * 1024 * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -526,7 +597,7 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
     if (!tr && m->use_tc && m->fold_on && m->fold_stale) {
         for (int l = 0; l < 4; ++l)
             for (auto& b : m->blocks[l])
-                if (b.has_ds && pack_fold(m, b, st)) return -1;
+                if (b.has_ds && b.kind == hn_model::BOTTLENECK && pack_fold(m, b, st)) return -1;
         m->fold_stale = false;
     }
     // model.py:248-252 + :73-76: normalise, stem conv/BN/ReLU, max-pool
@@ -565,12 +636,29 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
         if (maxpool3x3s2(s0, cur, st, m->use_tc != 0)) return -1;
     }
 
-    // model.py:78-81: layer1..layer4 (torchvision Bottleneck v1.5)
+    // model.py:78-81: layer1..layer4 (torchvision Bottleneck v1.5, or BasicBlock)
     Act feats[4];
     for (int l = 0; l < 4; ++l) {
         const int nb = (int)m->blocks[l].size();
         for (int b = 0; b < nb; ++b) {
             const hn_model::Block& blk = m->blocks[l][b];
+            if (blk.kind == hn_model::BASIC) {
+                // conv1 3x3 (stride) + BN + ReLU; the downsample (block 0 of layers 2-4) as its own launch; conv2 3x3 + BN +
+                // identity + ReLU.  No fold / fused kernel for this block kind: the options change nothing here
+                const int s = blk.c1.d.sh;
+                Act t1 = mk(m->T1, B, cur.H / s, cur.W / s, blk.c1.d.Cout);
+                Act y = mk(b == nb - 1 ? m->F[l] : m->X[b & 1], B, t1.H, t1.W, blk.c2.d.Cout);
+                if (conv_bn(m, blk.c1, cur, t1, nullptr, st, CLS_ENC_CONV, tr)) return -1;
+                const float* idn = cur.p;
+                if (blk.has_ds) {
+                    Act d = mk(m->IDN, B, t1.H, t1.W, blk.ds.d.Cout);
+                    if (conv_bn(m, blk.ds, cur, d, nullptr, st, CLS_ENC_CONV, tr)) return -1;
+                    idn = d.p;
+                }
+                if (conv_bn(m, blk.c2, t1, y, idn, st, CLS_ENC_CONV, tr)) return -1;
+                cur = y;
+                continue;
+            }
             const int s = blk.c2.d.sh;
             const int Ho = cur.H / s, Wo = cur.W / s;
             Act t1 = mk(m->T1, B, cur.H, cur.W, blk.c1.d.Cout);
@@ -626,17 +714,17 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
     return 0;
 }
 
-// (2) model.py:152-155 + :175-178 + :263: upsample + flatten + concat + permute -> SEQ [T=256][B][1024]
+// (2) model.py:152-155 + :175-178 + :263: upsample + flatten + concat + permute -> SEQ [T=256][B][c_last]
 static int forward_sequence(hn_model* m, const Act gout[4], cudaStream_t st) {
     Scope sc(m, CLS_TAIL, 0.0, st);
     return ghc_to_sequence(gout, m->SEQ, st, m->use_tc != 0);
 }
 
-// (3') model.py:270-279 (use_rnn=False): per-column MLP over the rows of SEQ.  Layer 1 (1024 -> 512, bias, ReLU) is the
+// (3') model.py:270-279 (use_rnn=False): per-column MLP over the rows of SEQ.  Layer 1 (c_last -> 512, bias, ReLU) is the
 // same GEMM-row convolution as the LSTM projections; dropout (train mode) on the hidden layer; layer 2 + the scatter.
 static int forward_mlp(hn_model* m, int B, float* bon, float* cor, cudaStream_t st, const TrainCtx* tr) {
     const size_t nh = (size_t)256 * B * 512;
-    const Act a = mk(m->SEQ, 1, 1, 256 * B, 1024, 0);
+    const Act a = mk(m->SEQ, 1, 1, 256 * B, m->c_last, 0);
     const Act h = mk(m->HID, 1, 1, 256 * B, 512, 0);
     if (run_conv(m, m->mlp1, a, h, nullptr, st, CLS_HEAD, true)) return -1;
     const float* head_in = m->HID;
@@ -658,7 +746,7 @@ static int forward_rnn(hn_model* m, int B, float* bon, float* cor, cudaStream_t 
     const float* lin = m->SEQ;
     float* louts[2] = {m->R1, m->R2};
     for (int layer = 0; layer < 2; ++layer) {
-        Act a = mk(const_cast<float*>(lin), 1, 1, 256 * B, 1024, 0);
+        Act a = mk(const_cast<float*>(lin), 1, 1, 256 * B, m->xproj[layer].d.Cin, 0);
         Act xp = mk(m->XP, 1, 1, 256 * B, 4096, 0);
         if (tr && layer == 1 && tr->rnn_p > 0.0) {
             // train mode: nn.LSTM(dropout=p) zeroes layer-1 outputs on their way into layer 2 (model.py:226)
@@ -946,14 +1034,14 @@ int hn_model_stage(hn_model* m, const char* stage, float* out, long long capacit
     const std::string s(stage);
     for (int l = 0; l < 4; ++l)
         if (s == "layer" + std::to_string(l + 1)) {
-            const int C = 256 << l, H = 128 >> l, W = 256 >> l;
+            const int C = block_out_channels(m->blocks[l].back()), H = 128 >> l, W = 256 >> l;
             const size_t total = (size_t)B * C * H * W;
             HN_CHECK((long long)total <= capacity, "hn_model_stage: output buffer too small");
             const float* src = m->F[l];
             if (m->use_tc) {       // F[l] holds fp16 hi/lo planes: merge into X[0] (free after the forward)
                 const size_t n = (size_t)B * H * (W + 2) * C;
                 float* tmp = m->X[0];
-                HN_CHECK(n <= (size_t)m->max_batch * 128 * 258 * 256, "hn_model_stage: scratch buffer too small");
+                HN_CHECK(n <= m->x0_cap, "hn_model_stage: scratch buffer too small");
                 if (merge_planes(reinterpret_cast<const unsigned short*>(m->F[l]), tmp, n, st)) return -1;
                 src = tmp;
             }
@@ -973,14 +1061,15 @@ int hn_model_stage(hn_model* m, const char* stage, float* out, long long capacit
     const size_t total = (size_t)256 * B * 1024;
     HN_CHECK((long long)total <= capacity, "hn_model_stage: output buffer too small");
     if (s == "feature") {
+        const size_t n = (size_t)256 * B * m->c_last;
         const float* seq = m->SEQ;
         if (m->use_tc) {      // SEQ holds fp16 hi/lo planes; XP is dead after the forward and large enough
-            if (merge_planes(reinterpret_cast<const unsigned short*>(m->SEQ), m->XP, total, st)) return -1;
+            if (merge_planes(reinterpret_cast<const unsigned short*>(m->SEQ), m->XP, n, st)) return -1;
             seq = m->XP;
         }
-        seq_to_feature_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(seq, out, 256, B);
+        seq_to_feature_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seq, out, 256, B, m->c_last);
         HN_LAUNCH_OK();
-        dims[0] = B; dims[1] = 1024; dims[2] = 256; dims[3] = 0;
+        dims[0] = B; dims[1] = m->c_last; dims[2] = 256; dims[3] = 0;
         return 0;
     }
     if (s == "mlp_hidden") {      // post-ReLU, pre-dropout hidden layer -> [B][256][512] (reference linear[1], model.py:272)
@@ -1130,7 +1219,18 @@ int hn_conv2d(const float* in, int B, int H, int W, int Cin, int in_halo, const 
         if (impl == 2 && residual) return fail("hn_conv2d: the fp32-output tensor-core epilogue takes no residual");
         return conv_tc(d, a, o, residual, impl == 2, (cudaStream_t)stream);
     }
-    HN_CHECK(impl == 0, "hn_conv2d: impl must be 0, 1 or 2");
+    if (impl == 3) {              // the narrow height-reduction kernel, through split planes of in / out
+        if (!conv_narrow_supported(d, a, o) || residual) return fail("hn_conv2d: shape not supported by the narrow kernel");
+        cudaStream_t st = (cudaStream_t)stream;
+        unsigned short *ip = nullptr, *op = nullptr;
+        HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&ip), a.numel() * 2 * sizeof(unsigned short), st));
+        HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&op), o.numel() * 2 * sizeof(unsigned short), st));
+        int rc = split_planes(in, ip, a.numel(), st) || conv_narrow_planes(d, a, ip, o, op, st) ||
+                 merge_planes(op, out, o.numel(), st);
+        cudaFreeAsync(ip, st); cudaFreeAsync(op, st);
+        return rc ? -1 : 0;
+    }
+    HN_CHECK(impl == 0, "hn_conv2d: impl must be 0, 1, 2 or 3");
     return conv_f32(d, a, o, residual, (cudaStream_t)stream);
 }
 

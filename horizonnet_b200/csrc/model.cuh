@@ -13,7 +13,13 @@
 
 namespace hn {
 
+// seq [T=256][B][C], C = the four scales' C*H summed (c_last: 1024 or 256, a power of two)
 int ghc_to_sequence(const Act ghc[4], float* seq, cudaStream_t st, bool split);
+// 3x3, stride (2, 1), circular-W conv + scale/shift (+ ReLU) for Cin or Cout below the tensor-core kernel's 64 / 32
+// (conv_narrow.cu): split-plane input and output, fp32 weights [K][Cout] and fp32 accumulation
+bool conv_narrow_supported(const ConvDesc& d, const Act& in, const Act& out);
+int conv_narrow_planes(const ConvDesc& d, const Act& in, const unsigned short* in_planes, const Act& out,
+                       unsigned short* out_planes, cudaStream_t st);
 // K = 1024: the bi-LSTM head (rnn [T][B][1024]); K = 512: the last layer of the MLP head (hidden [T][B][512])
 int linear_head(const float* rnn, const float* w, const float* bias, float* bon, float* cor, int T, int B, int K,
                 cudaStream_t st);
@@ -97,8 +103,13 @@ struct hn_model {
     ConvLayer stem;                                  // weights packed [147][64]
     // fold (block 0, eval): conv3 + downsample as one 1x1 conv over [t2 | x]: w = [s3 W3 ; sd Wd] fp32 [Cout][K], shift =
     // f3 + fd, wq / tc_scale their planes (conv_tc_fold_planes)
-    struct Block { ConvLayer c1, c2, c3, ds, fold; bool has_ds = false; };
+    // kind BOTTLENECK (resnet50): conv1 1x1, conv2 3x3 (stride), conv3 1x1 + identity.  BASIC (resnet18): c1 3x3 (stride),
+    // c2 3x3 + identity; c3 and fold stay empty
+    enum Kind { BOTTLENECK = 0, BASIC = 1 };
+    struct Block { ConvLayer c1, c2, c3, ds, fold; bool has_ds = false; Kind kind = BOTTLENECK; };
     std::vector<Block> blocks[4];
+    int c_last = 1024;                               // feature-sequence width: 1024 (resnet50), 256 (resnet18)
+    size_t x0_cap = 0;                               // floats in X[0] (also scratch of the stem and of hn_model_stage)
     ConvLayer ghc[4][4];
     int use_rnn = 1;                                 // 0: per-column MLP head instead of the bi-LSTM (model.py:234-243)
     ConvLayer xproj[2];                              // LSTM input projections as 1x1 convs, N = 4096

@@ -2,7 +2,7 @@
 //
 // ghc_to_sequence: reference model.py:152-155 (circular pad by 1, bilinear W-upsample to 256+2f
 //   columns, crop f) + model.py:175-178 (reshape (C,H)->C*H, concat 4 scales) + model.py:263
-//   (permute to [T=256, B, 1024]) in one pass.  Because (W+2)*f == 256+2f the interpolate scale is
+//   (permute to [T=256, B, c_last], c_last = 1024 resnet50 / 256 resnet18) in one pass.  Because (W+2)*f == 256+2f the interpolate scale is
 //   exactly 1/f, so out[col] = (1-l)*x[i0] + l*x[i0+1] with s = (col+0.5)/f + 0.5 in halo
 //   coordinates, i0 = floor(s), l = s - i0 (all exactly representable in fp32; f=1 is the identity).
 // head_kernel<K>: model.py:266-269, Linear(K -> 12) + the [T,B,3,4] -> [B,3,T*4] scatter;
@@ -18,17 +18,18 @@ namespace {
 struct GhcSrc {
     const float* p[4];
     int H[4], W[4], C[4], chan_off[4];
+    int lg;                   // log2 of the sequence width (1024 or 256)
 };
 
 template <bool SPLIT>
 __global__ void __launch_bounds__(256) ghc_to_sequence_kernel(const GhcSrc s, float* __restrict__ seq, int B) {
     // seq[t][b][ch], ch = chan_off[s] + c*H + h ; one thread per (t, b, ch), ch fastest
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t total = (size_t)256 * B * 1024;
+    const size_t total = ((size_t)256 * B) << s.lg;
     if (i >= total) return;
-    const int ch = (int)(i & 1023);
-    const int b = (int)((i >> 10) % B);
-    const int t = (int)((i >> 10) / B);
+    const int ch = (int)(i & ((1u << s.lg) - 1));
+    const int b = (int)((i >> s.lg) % B);
+    const int t = (int)((i >> s.lg) / B);
     int sc = 3;
     if (ch < s.chan_off[1]) sc = 0; else if (ch < s.chan_off[2]) sc = 1; else if (ch < s.chan_off[3]) sc = 2;
     const int H = s.H[sc], W = s.W[sc], C = s.C[sc];
@@ -112,8 +113,10 @@ int ghc_to_sequence(const Act ghc[4], float* seq, cudaStream_t st, bool split) {
         s.p[i] = ghc[i].p; s.H[i] = ghc[i].H; s.W[i] = ghc[i].W; s.C[i] = ghc[i].C; s.chan_off[i] = off;
         off += ghc[i].C * ghc[i].H;
     }
-    HN_CHECK(off == 1024, "ghc_to_sequence: the 4 scales must flatten to 1024 channels (model.py:218)");
-    const size_t total = (size_t)256 * ghc[0].B * 1024;
+    HN_CHECK((off == 1024 || off == 256),
+             "ghc_to_sequence: the 4 scales must flatten to 1024 (resnet50) or 256 (resnet18) channels (model.py:218)");
+    s.lg = off == 1024 ? 10 : 8;
+    const size_t total = (size_t)256 * ghc[0].B * off;
     if (split)
         ghc_to_sequence_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(s, seq, ghc[0].B);
     else

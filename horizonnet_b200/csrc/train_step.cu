@@ -1,4 +1,4 @@
-// Training step of HorizonNet('resnet50', rnn): forward with a tape + backward (SURVEY 8 row f1; reference
+// Training step of HorizonNet('resnet50' or 'resnet18', rnn): forward with a tape + backward (SURVEY 8 row f1; reference
 // train.py:44-58 feed_forward and :272-281 loss.backward()).  The losses and the optimizer stay in PyTorch (they are
 // elementwise on [B,3,1024] outputs and on the parameters): the boundary is an autograd.Function whose forward is
 // hn_train_forward and whose backward hands d(bon), d(cor) to hn_train_backward and reads one gradient per
@@ -122,7 +122,8 @@ int unit_forward(hn_model* m, TrainState* ts, Bump& Y, Bump& Z, Bump& BN, const 
     u.y.p = Y.take(u.y.numel());
     u.bn = BN.take((size_t)4 * c.d.Cout);
     ts->dz_max = std::max(ts->dz_max, u.z.numel());
-    if (c.d.sh != 1 || c.d.sw != 1) ts->dil_max = std::max(ts->dil_max, (size_t)in.B * in.H * in.Wp() * c.d.Cout);
+    // (the fp32 data gradient pads Cout to a multiple of 16, see walk_backward)
+    if (c.d.sh != 1 || c.d.sw != 1) ts->dil_max = std::max(ts->dil_max, (size_t)in.B * in.H * in.Wp() * ((c.d.Cout + 15) / 16 * 16));
     ts->w_max = std::max(ts->w_max, (size_t)c.d.Cout * c.d.Cin * c.d.kh * c.d.kw);
     ts->din_max = std::max(ts->din_max, in.numel());
     if (run) {
@@ -188,12 +189,23 @@ int walk_forward(hn_model* m, TrainState* ts, const float* x, int B, int in_chan
     if (run && maxpool3x3s2(ts->stem_y, ts->pool_y, st, false)) return -1;
     if (run && m->use_tc && split_planes(ts->pool_y.p, planes_of(ts, ts->pool_y), ts->pool_y.numel(), st)) return -1;
 
-    // ---- layer1..4 (model.py:78-81, torchvision Bottleneck v1.5)
+    // ---- layer1..4 (model.py:78-81, torchvision Bottleneck v1.5 or BasicBlock)
     Act cur = ts->pool_y, feats[4];
     for (int l = 0; l < 4; ++l) {
         for (size_t b = 0; b < m->blocks[l].size(); ++b) {
             const hn_model::Block& blk = m->blocks[l][b];
             Act t1, t2, y, dsy;
+            if (blk.kind == hn_model::BASIC) {       // units conv1, downsample, conv2 (+ identity: its gradient goes to idn)
+                if (unit_forward(m, ts, Y, Z, BN, blk.c1, cur, nullptr, tr, st, run, &t1)) return -1;
+                const float* idn = cur.p;
+                if (blk.has_ds) {
+                    if (unit_forward(m, ts, Y, Z, BN, blk.ds, cur, nullptr, tr, st, run, &dsy)) return -1;
+                    idn = dsy.p;
+                }
+                if (unit_forward(m, ts, Y, Z, BN, blk.c2, t1, idn, tr, st, run, &y)) return -1;
+                cur = y;
+                continue;
+            }
             if (unit_forward(m, ts, Y, Z, BN, blk.c1, cur, nullptr, tr, st, run, &t1)) return -1;
             const float* idn = cur.p;
             if (blk.has_ds) {
@@ -221,7 +233,7 @@ int walk_forward(hn_model* m, TrainState* ts, const float* x, int B, int in_chan
     if (!m->use_rnn) {
         // model.py:270-275: MLP per row, layer 1 on the exact fp32 kernel; both hidden layers stay on the tape
         const size_t nh = (size_t)T_STEPS * B * 512;
-        const Act a = mk(ts->seq, 1, 1, T_STEPS * B, 1024, 0);
+        const Act a = mk(ts->seq, 1, 1, T_STEPS * B, m->c_last, 0);
         const Act h = mk(ts->mh, 1, 1, T_STEPS * B, 512, 0);
         if (conv_f32(m->mlp1.d, a, h, nullptr, st)) return -1;
         HN_CUDA_OK(cudaMemcpyAsync(ts->mhd, ts->mh, nh * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -235,7 +247,7 @@ int walk_forward(hn_model* m, TrainState* ts, const float* x, int B, int in_chan
     const size_t nseq = (size_t)T_STEPS * B * 1024;
     const float* lin = ts->seq;
     for (int layer = 0; layer < 2; ++layer) {
-        Act a = mk(const_cast<float*>(lin), 1, 1, T_STEPS * B, 1024, 0);
+        Act a = mk(const_cast<float*>(lin), 1, 1, T_STEPS * B, m->xproj[layer].d.Cin, 0);
         Act xp = mk(ts->xp[layer], 1, 1, T_STEPS * B, 4096, 0);
         if (conv_f32(m->xproj[layer].d, a, xp, nullptr, st)) return -1;
         if (lstm_layer(ts->xp[layer], m->whh[layer][0], m->whh[layer][1], ts->r[layer], T_STEPS, B, st)) return -1;
@@ -275,7 +287,9 @@ int ensure_buffers(hn_model* m, TrainState* ts, int B, const TrainCtx& tr) {
     if (fill_f32(ts->ones, 4096, 1.f, 0) || fill_f32(ts->zeros, 4096, 0.f, 0)) return -1;
     if (ts->alloc_t(&ts->stem_in, (size_t)B * 512 * 1030 * 3)) return -1;
     const size_t rows = (size_t)T_STEPS * B;
-    if (ts->alloc_t(&ts->seq, rows * 1024) || ts->alloc_t(&ts->da, rows * 1024) || ts->alloc_t(&ts->db, rows * 1024)) return -1;
+    // da / db: gradients of the LSTM outputs (1024 wide) and of the sequence (c_last <= 1024)
+    if (ts->alloc_t(&ts->seq, rows * m->c_last) || ts->alloc_t(&ts->da, rows * 1024) || ts->alloc_t(&ts->db, rows * 1024))
+        return -1;
     if (!m->use_rnn) {
         if (ts->alloc_t(&ts->mh, rows * 512) || ts->alloc_t(&ts->mhd, rows * 512)) return -1;
         HN_CUDA_OK(cudaStreamSynchronize(0));
@@ -374,19 +388,20 @@ int mlp_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dc
     if (relu_bwd_inplace(dh, ts->mh, nh, st)) return -1;
     if (col_sum(dh, rows, 512, GRAD("linear.0.bias"), st)) return -1;
     // dW1 = dH^T SEQ: the weight gradient of a 1x1 "convolution" over the T*B rows, like W_ih of the LSTM
-    const Act xa = mk(ts->seq, 1, 1, (int)rows, 1024, 0);
+    const int CL = m->c_last;
+    const Act xa = mk(ts->seq, 1, 1, (int)rows, CL, 0);
     const Act dg = mk(dh, 1, 1, (int)rows, 512, 0);
-    ConvDesc wi; wi.Cin = 1024; wi.Cout = 512;
+    ConvDesc wi; wi.Cin = CL; wi.Cout = 512;
     if (m->use_tc && wgrad_tc_on() && conv_wgrad_tc_supported(wi, xa, dg)) {
         unsigned short* xpl = reinterpret_cast<unsigned short*>(ts->pl_scratch);
         unsigned short* gpl = reinterpret_cast<unsigned short*>(ts->pl_scratch + rows * 1024);
         float* gmax = ts->aux_tmp + 3 * 4096 + 1;
-        if (split_planes(ts->seq, xpl, rows * 1024, st) || split_planes_pow2(dh, gpl, nh, gmax, st)) return -1;
+        if (split_planes(ts->seq, xpl, rows * CL, st) || split_planes_pow2(dh, gpl, nh, gmax, st)) return -1;
         if (conv_wgrad_tc(wi, xa, xpl, dg, gpl, gmax, GRAD("linear.0.weight"), st)) return -1;
     } else if (conv_wgrad_f32(wi, xa, dg, GRAD("linear.0.weight"), st)) return -1;
-    // d(sequence) = dH W1      (W1 [512][1024] is already conv_f32's [K][N] packing)
-    ConvDesc di; di.Cin = 512; di.Cout = 1024; di.w = m->T("linear.0.weight"); di.scale = ts->ones; di.shift = ts->zeros;
-    if (conv_f32(di, dg, mk(ts->db, 1, 1, (int)rows, 1024, 0), nullptr, st)) return -1;
+    // d(sequence) = dH W1      (W1 [512][c_last] is already conv_f32's [K][N] packing)
+    ConvDesc di; di.Cin = 512; di.Cout = CL; di.w = m->T("linear.0.weight"); di.scale = ts->ones; di.shift = ts->zeros;
+    if (conv_f32(di, dg, mk(ts->db, 1, 1, (int)rows, CL, 0), nullptr, st)) return -1;
     *dseq = ts->db;
     HN_CUDA_OK(cudaEventRecord(ts->ev[1], st));
     HN_CUDA_OK(cudaEventRecord(ts->ev[2], st));          // no recurrence: the bi-LSTM phase is empty
@@ -412,6 +427,7 @@ int rnn_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dc
     for (int layer = 1; layer >= 0; --layer) {
         const std::string l = "_l" + std::to_string(layer);
         const float* X = layer == 0 ? ts->seq : ts->rm[0];
+        const int K = m->xproj[layer].d.Cin;             // layer input width: c_last, then 1024
         if (lstm_gather(ts->r[layer], ts->xp[layer], ts->hprev, ts->gates, T_STEPS, B, st)) return -1;
         for (int dir = 0; dir < 2; ++dir) {
             // gate pre-activations of every step at once: XP + H_prev * W_hh^T
@@ -427,8 +443,8 @@ int rnn_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dc
                            ts->barrier, m->error_flag, st))
             return -1;
         // weight gradients = 1x1 "convolutions" over the T*B rows: dW_ih = dG^T X, dW_hh = dG^T H_prev
-        const Act xa = mk(const_cast<float*>(X), 1, 1, (int)rows, 1024, 0);
-        ConvDesc wi; wi.Cin = 1024; wi.Cout = 2048;
+        const Act xa = mk(const_cast<float*>(X), 1, 1, (int)rows, K, 0);
+        ConvDesc wi; wi.Cin = K; wi.Cout = 2048;
         ConvDesc wh; wh.Cin = 512; wh.Cout = 2048;
         const bool lstm_wg_tc = m->use_tc && wgrad_tc_on() &&
                                 conv_wgrad_tc_supported(wi, xa, mk(ts->dgates, 1, 1, (int)rows, 2048, 0)) &&
@@ -438,7 +454,7 @@ int rnn_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dc
         unsigned short* hpl = reinterpret_cast<unsigned short*>(ts->pl_scratch + rows * 1024);
         unsigned short* gpl = reinterpret_cast<unsigned short*>(ts->pl_scratch + rows * 1536);
         float* gmax = ts->aux_tmp + 3 * 4096 + 1;
-        if (lstm_wg_tc && split_planes(X, xpl, rows * 1024, st)) return -1;
+        if (lstm_wg_tc && split_planes(X, xpl, rows * K, st)) return -1;
         for (int dir = 0; dir < 2; ++dir) {
             const std::string sfx = l + (dir ? "_reverse" : "");
             Act dg = mk(ts->dgates + dir * rows * 2048, 1, 1, (int)rows, 2048, 0);
@@ -454,10 +470,10 @@ int rnn_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dc
             float* bi = GRAD("bi_rnn.bias_ih" + sfx);
             if (col_sum(dg.p, rows, 2048, bi, st)) return -1;
             HN_CUDA_OK(cudaMemcpyAsync(GRAD("bi_rnn.bias_hh" + sfx), bi, 2048 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-            // d(layer input) (+)= dG * W_ih      (W_ih [2048][1024] is already conv_f32's [K][N] packing)
-            ConvDesc di; di.Cin = 2048; di.Cout = 1024; di.w = m->T("bi_rnn.weight_ih" + sfx); di.scale = ts->ones;
+            // d(layer input) (+)= dG * W_ih      (W_ih [2048][K] is already conv_f32's [K][N] packing)
+            ConvDesc di; di.Cin = 2048; di.Cout = K; di.w = m->T("bi_rnn.weight_ih" + sfx); di.scale = ts->ones;
             di.shift = ts->zeros;
-            Act dx = mk(dnext, 1, 1, (int)rows, 1024, 0);
+            Act dx = mk(dnext, 1, 1, (int)rows, K, 0);
             if (conv_f32(di, dg, dx, dir ? dnext : nullptr, st)) return -1;
         }
         if (layer == 1 && tr.rnn_p > 0.0 && (tr.mask[0] ? multiply_inplace(dnext, tr.mask[0], nseq, st)
@@ -527,6 +543,22 @@ int walk_backward(hn_model* m, TrainState* ts, const float* dbon, const float* d
             const DgradScratch s = {ts->dil_scratch, ts->dtmp, sp, ts->dw_scratch,
                                     reinterpret_cast<unsigned short*>(ts->wd_scratch), ts->aux_tmp, amax, ts->zeros};
             if (dgrad_tc(u.d, m->T(c.wkey), dz, din, s, sp_is_dz, st)) return -1;
+        } else if (u.d.Cout % 16 != 0) {
+            // resnet18's ghc0.3 (16 -> 8): conv_dgrad_f32 takes Cout in steps of 16, so dz and the weights get zero channels
+            // up to 16 (OIHW: the extra output channels are zero rows after the real ones).  dw_scratch and pl2_scratch are
+            // free here: the weight gradient is already in its OIHW buffer and took the fp32 kernel
+            ConvDesc dp = u.d;
+            dp.Cout = (u.d.Cout + 15) / 16 * 16;
+            Act dzp = dz;
+            dzp.C = dp.Cout; dzp.p = ts->pl2_scratch;
+            const size_t nw = (size_t)u.d.Cout * u.d.Cin * u.d.kh * u.d.kw, nwp = (size_t)dp.Cout * u.d.Cin * u.d.kh * u.d.kw;
+            HN_CUDA_OK(cudaMemsetAsync(ts->dw_scratch, 0, nwp * sizeof(float), st));
+            HN_CUDA_OK(cudaMemcpyAsync(ts->dw_scratch, m->T(c.wkey), nw * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            HN_CUDA_OK(cudaMemsetAsync(dzp.p, 0, dzp.numel() * sizeof(float), st));
+            HN_CUDA_OK(cudaMemcpy2DAsync(dzp.p, dp.Cout * sizeof(float), dz.p, u.d.Cout * sizeof(float), u.d.Cout * sizeof(float),
+                                         dz.numel() / u.d.Cout, cudaMemcpyDeviceToDevice, st));
+            if (pack_dgrad_weight(ts->dw_scratch, ts->wd_scratch, dp.Cout, u.d.Cin, u.d.kh, u.d.kw, st)) return -1;
+            if (conv_dgrad_f32(dp, ts->wd_scratch, dzp, din, true, ts->dil_scratch, ts->ones, ts->zeros, st)) return -1;
         } else {
             if (pack_dgrad_weight(m->T(c.wkey), ts->wd_scratch, u.d.Cout, u.d.Cin, u.d.kh, u.d.kw, st)) return -1;
             if (conv_dgrad_f32(u.d, ts->wd_scratch, dz, din, true, ts->dil_scratch, ts->ones, ts->zeros, st)) return -1;

@@ -8,7 +8,8 @@ Boundary kept from the reference (SURVEY 8b):
     ``NotImplementedError`` for any other H x W (model.py:255-256);
   * ``.backbone``, ``.use_rnn``, ``.feature_extractor.list_blocks()``, ``.x_mean``, ``.x_std``.
 Built: ``backbone='resnet50'`` with ``use_rnn=True`` (the path BASELINE.json names) or ``use_rnn=False`` (the
-per-column MLP head of model.py:234-243, what the reference's ``train.py --no_rnn`` trains), inference
+per-column MLP head of model.py:234-243, what the reference's ``train.py --no_rnn`` trains), and ``backbone='resnet18'``
+(torchvision BasicBlocks, a 256-wide feature sequence) with either head; inference
 (eval) forward -- plus the train-mode FORWARD (batch-statistics BatchNorm with running-stat updates,
 LSTM / head dropout; train.py:52) and its backward (train.py:278 ``loss.backward()``): with autograd on,
 ``forward`` in train mode returns outputs whose grad_fn runs the library's backward pass and fills
@@ -25,7 +26,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._spec import HEAD_BIAS, RNN_HIDDEN, STEP_COLS, PANO_H, PANO_W, state_dict_spec
+from ._spec import BACKBONES, HEAD_BIAS, RNN_HIDDEN, STEP_COLS, PANO_H, PANO_W, c_last, encoder_channels, state_dict_spec
 
 
 class CircularPadW(nn.Module):
@@ -61,19 +62,38 @@ class _Bottleneck(nn.Module):
                                             nn.BatchNorm2d(planes * 4))
 
 
-class _ResNet50(nn.Module):
-    def __init__(self):
+class _BasicBlock(nn.Module):
+    """torchvision resnet.py BasicBlock: two 3x3 convs (wrapped by LR_PAD, hence ``conv1.1`` / ``conv2.1``), the stride on
+    conv1, the downsample on block 0 of layers 2-4 only."""
+
+    def __init__(self, inplanes, planes, stride, downsample):
         super().__init__()
+        self.conv1 = _wrapped_conv(inplanes, planes, 3, stride, False)
+        self.bn1 = nn.BatchNorm2d(planes)
+        self.relu = nn.ReLU(inplace=True)
+        self.conv2 = _wrapped_conv(planes, planes, 3, 1, False)
+        self.bn2 = nn.BatchNorm2d(planes)
+        if downsample:
+            self.downsample = nn.Sequential(nn.Conv2d(inplanes, planes, 1, stride=stride, bias=False),
+                                            nn.BatchNorm2d(planes))
+
+
+class _ResNet(nn.Module):
+    def __init__(self, backbone):
+        super().__init__()
+        kind, nblocks, planes_l, expansion = BACKBONES[backbone]
+        block = _Bottleneck if kind == 'bottleneck' else _BasicBlock
         self.conv1 = _wrapped_conv(3, 64, 7, 2, False)
         self.bn1 = nn.BatchNorm2d(64)
         self.relu = nn.ReLU(inplace=True)
         self.maxpool = nn.MaxPool2d(3, 2, 1)
         inplanes = 64
-        for li, (nblk, planes) in enumerate(zip((3, 4, 6, 3), (64, 128, 256, 512)), start=1):
+        for li, (nblk, planes) in enumerate(zip(nblocks, planes_l), start=1):
             blocks = []
             for b in range(nblk):
-                blocks.append(_Bottleneck(inplanes, planes, 2 if (b == 0 and li > 1) else 1, b == 0))
-                inplanes = planes * 4
+                stride = 2 if (b == 0 and li > 1) else 1
+                blocks.append(block(inplanes, planes, stride, b == 0 and (stride != 1 or inplanes != planes * expansion)))
+                inplanes = planes * expansion
             setattr(self, f'layer{li}', nn.Sequential(*blocks))
         for m in self.modules():            # torchvision resnet.py:208-213 initialisation
             if isinstance(m, nn.Conv2d):
@@ -81,9 +101,9 @@ class _ResNet50(nn.Module):
 
 
 class _Encoder(nn.Module):
-    def __init__(self):
+    def __init__(self, backbone):
         super().__init__()
-        self.encoder = _ResNet50()
+        self.encoder = _ResNet(backbone)
 
     def list_blocks(self):
         """Same grouping as reference model.py:84-91 (used by train.py --freeze_earlier_blocks)."""
@@ -139,25 +159,26 @@ class HorizonNet(nn.Module):
 
     def __init__(self, backbone, use_rnn):
         super().__init__()
-        if backbone != 'resnet50':
+        if backbone not in BACKBONES:
             raise NotImplementedError(
-                "horizonnet_b200 implements HorizonNet('resnet50', use_rnn=True) and HorizonNet('resnet50', use_rnn=False) "
-                f"only, not the {backbone!r} backbone")
+                f"horizonnet_b200 implements the {' and '.join(sorted(BACKBONES))} backbones (use_rnn=True or False), "
+                f"not {backbone!r}")
         self.backbone = backbone
         self.use_rnn = use_rnn
         self.out_scale = 8
         self.step_cols = STEP_COLS
         self.rnn_hidden_size = RNN_HIDDEN
-        self.feature_extractor = _Encoder()
-        self.reduce_height_module = _HeightStage((256, 512, 1024, 2048), self.out_scale)
+        self.feature_extractor = _Encoder(backbone)
+        self.reduce_height_module = _HeightStage(encoder_channels(backbone), self.out_scale)
+        width = c_last(backbone)                                      # feature sequence: 1024 (resnet50), 256 (resnet18)
         if use_rnn:
-            self.bi_rnn = nn.LSTM(input_size=1024, hidden_size=RNN_HIDDEN, num_layers=2, dropout=0.5,
+            self.bi_rnn = nn.LSTM(input_size=width, hidden_size=RNN_HIDDEN, num_layers=2, dropout=0.5,
                                   batch_first=False, bidirectional=True)
             self.drop_out = nn.Dropout(0.5)
             self.linear = nn.Linear(2 * RNN_HIDDEN, 3 * STEP_COLS)
             head = self.linear
         else:                                                         # model.py:234-243
-            self.linear = nn.Sequential(nn.Linear(1024, RNN_HIDDEN), nn.ReLU(inplace=True), nn.Dropout(0.5),
+            self.linear = nn.Sequential(nn.Linear(width, RNN_HIDDEN), nn.ReLU(inplace=True), nn.Dropout(0.5),
                                         nn.Linear(RNN_HIDDEN, 3 * STEP_COLS))
             head = self.linear[-1]
         with torch.no_grad():
@@ -175,7 +196,7 @@ class HorizonNet(nn.Module):
     def _state_tensors(self):
         if self._slots is None:
             slots = []
-            spec = state_dict_spec(self.use_rnn)
+            spec = state_dict_spec(self.use_rnn, self.backbone)
             for key in spec:
                 *path, leaf = key.split('.')
                 mod = self
@@ -230,8 +251,8 @@ class HorizonNet(nn.Module):
             if h is None:
                 ptr = ctypes.c_void_p()
                 max_batch = max(batch, 1)
-                _lib.check(lib.hn_model_create_head(key, max_batch, 1 if self.use_rnn else 0, ctypes.byref(ptr)),
-                           'hn_model_create_head')
+                _lib.check(lib.hn_model_create_arch(key, max_batch, self.backbone.encode(), 1 if self.use_rnn else 0,
+                                                    ctypes.byref(ptr)), 'hn_model_create_arch')
                 h = {'ptr': ptr, 'max_batch': max_batch, 'sig': None}
                 self._handles[key] = h
             sig = self._weight_signature()

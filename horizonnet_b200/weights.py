@@ -18,13 +18,14 @@ import torch
 from ._spec import state_dict_spec, HEAD_BIAS
 
 
-def synthetic_state_dict(seed=0, bn='identity', use_rnn=True):
+def synthetic_state_dict(seed=0, bn='identity', use_rnn=True, backbone='resnet50'):
     """use_rnn=False: the MLP-head layout.  Its encoder and height-reduction tensors come first in the key order and are
-    drawn identically, so they equal the bi-LSTM model's for the same seed; then linear.0 ~ U(+-1/sqrt(1024)) (weight and
-    bias, PyTorch's nn.Linear default), linear.3.weight ~ U(+-1/sqrt(512)), linear.3.bias = the reference's init."""
+    drawn identically, so they equal the bi-LSTM model's for the same seed; then linear.0 ~ U(+-1/sqrt(c_last)) (weight and
+    bias, PyTorch's nn.Linear default), linear.3.weight ~ U(+-1/sqrt(512)), linear.3.bias = the reference's init.
+    backbone: the key layout of that encoder (horizonnet_b200._spec.BACKBONES), drawn by the same rules."""
     rs = np.random.RandomState(seed)
     sd = OrderedDict()
-    for key, (shape, kind) in state_dict_spec(use_rnn).items():
+    for key, (shape, kind) in state_dict_spec(use_rnn, backbone).items():
         if kind == 'enc_conv':
             co, ci, kh, kw = shape
             a = rs.standard_normal(shape) * math.sqrt(2.0 / (co * kh * kw))

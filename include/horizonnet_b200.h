@@ -33,7 +33,7 @@ const char* hn_build_digest(void);
 /* Number of kernels this library has launched in this process (bench.py "gpu_launches"). */
 long long hn_kernel_launches(void);
 
-/* ---- model.HorizonNet (reference model.py:185-281), resnet50 with the bi-LSTM or the MLP head ---- */
+/* ---- model.HorizonNet (reference model.py:185-281), resnet50 or resnet18 with the bi-LSTM or the MLP head ---- */
 
 /* Creates HorizonNet('resnet50', use_rnn=True) on CUDA device `device`, with activation workspace for up to
  * `max_batch` panoramas per forward.  Replaces HorizonNet.__init__ (model.py:189-246) minus the ImageNet
@@ -44,6 +44,10 @@ int hn_model_create(int device, int max_batch, hn_model** out);
  * 434 state_dict keys: linear.0.* and linear.3.* instead of bi_rnn.* and linear.*.  Every entry point below takes
  * either model. */
 int hn_model_create_head(int device, int max_batch, int use_rnn, hn_model** out);
+/* Any supported backbone: "resnet50" (torchvision Bottlenecks; what hn_model_create / _head build) or "resnet18"
+ * (BasicBlocks, 250 state_dict keys with the bi-LSTM, 236 with the MLP head; the feature sequence is 256 wide instead of
+ * 1024, so bi_rnn.weight_ih_l0* is [2048][256] and linear.0.weight [512][256]).  Other names fail. */
+int hn_model_create_arch(int device, int max_batch, const char* backbone, int use_rnn, hn_model** out);
 
 /* Number of tensors of the reference checkpoint layout (448, or 434 with the MLP head; misc/utils.py:49-58) and the i-th key
  * with its element count; lets a binding iterate the state_dict without knowing the topology. */
@@ -161,7 +165,7 @@ int hn_model_infer_tta(hn_model* m, const float* x_dev, int in_channels, int fli
 /* Test hook: copies an intermediate result of the LAST forward, converted to the reference's
  * layout, into `out_dev` (fp32).  Stages: "stem" (conv1+bn1+relu, NCHW [B,64,256,512], model.py:73-75),
  * "layer1".."layer4" (NCHW [B,C,H,W], model.py:78-81),
- * "feature" ([B,1024,256], model.py:175-178), "rnn_out" ([256,B,1024], model.py:264; bi-LSTM model only),
+ * "feature" ([B,c_last,256], c_last 1024 for resnet50 and 256 for resnet18; model.py:175-178), "rnn_out" ([256,B,1024], model.py:264; bi-LSTM model only),
  * "mlp_hidden" ([B,256,512], the post-ReLU, pre-dropout hidden layer = output of linear[1], model.py:272; MLP model
  * only).  dims receives the 4 (or 3, last = 0) extents. */
 int hn_model_stage(hn_model* m, const char* stage, float* out_dev, long long capacity, int dims[4],
@@ -236,7 +240,9 @@ int hn_rotate_panorama(const void* img_dev, int in_is_f64, double* out_dev, int 
  * ph = zero padding along H, pw = circular padding along W (<= in_halo).
  * impl: 0 = exact fp32 CUDA-core kernel, 1 = split-fp16 wgmma tensor-core kernel (split-plane output, merged to fp32),
  * 2 = the same kernel writing fp32 directly (the epilogue of the LSTM input projections, of the raw pass of a train-mode
- * convolution and of the data gradient; no residual). */
+ * convolution and of the data gradient; no residual), 3 = the narrow height-reduction kernel of resnet18 (conv_narrow.cu:
+ * 3x3, stride (2, 1), pad (1, 1), halo 1, Cin -> Cout 32 -> 32, 32 -> 16 or 16 -> 8; split-plane operands made and merged
+ * inside; no residual). */
 int hn_conv2d(const float* in_dev, int B, int H, int W, int Cin, int in_halo,
               const float* w_packed_dev, const float* scale_dev, const float* shift_dev,
               const float* residual_dev, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
