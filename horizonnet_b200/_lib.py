@@ -8,7 +8,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libhorizonnet_b200.so')
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 _lib = None
 _lock = threading.Lock()
@@ -37,8 +37,6 @@ SIGNATURES = {
     'hn_model_flush': (ctypes.c_int, [vp, vp]),
     'hn_model_num_bn': (ctypes.c_int, [vp]),
     'hn_model_bn_name': (ctypes.c_char_p, [vp, ctypes.c_int]),
-    'hn_model_forward_train': (ctypes.c_int, [vp, vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, ctypes.c_int,
-                                              ctypes.c_ulonglong, ctypes.c_double, ctypes.c_double, vp, vp, vp]),
     'hn_train_forward': (ctypes.c_int, [vp, vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, ctypes.c_int,
                                         ctypes.c_ulonglong, ctypes.c_double, ctypes.c_double, vp, vp, vp]),
     'hn_train_backward': (ctypes.c_int, [vp, vp, vp, vp]),

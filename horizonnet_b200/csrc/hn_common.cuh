@@ -79,12 +79,8 @@ int stem_f32(const float* x_nchw, int B, int in_channels, const float* w_packed,
              const float* shift, const Act& out, cudaStream_t st, bool relu = true);
 int maxpool3x3s2(const Act& in, const Act& out, cudaStream_t st, bool out_split = false);
 
-// train-mode forward pieces (train_fwd.cu): batch-statistics BN and Philox dropout
-int bn_batch_stats(const Act& z, bool planes, double* sums /* [2*C] */, cudaStream_t st);
-int bn_train_finalize(const double* sums, long long count, const float* gamma, const float* beta, const float* bias,
-                      float* running_mean, float* running_var, double factor /* < 0: leave running stats alone */,
-                      float* scale, float* shift, int C, cudaStream_t st);
-int bn_identity_constants(const float* bias, float* scale, float* shift, int C, cudaStream_t st);
+// train-mode forward pieces (train_fwd.cu): batch statistics of a fp32 tensor for BN, and Philox dropout
+int bn_batch_stats(const Act& z, double* sums /* [2*C] */, cudaStream_t st);
 int dropout_inplace(float* x, size_t n, double p, unsigned long long seed, int which, bool mask_only, cudaStream_t st);
 int multiply_inplace(float* x, const float* mask, size_t n, cudaStream_t st);
 

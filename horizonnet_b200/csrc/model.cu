@@ -311,39 +311,13 @@ int refold_bn(hn_model* m, cudaStream_t st) {
     return 0;
 }
 
-// conv + BatchNorm2d (+ identity, ReLU).  Eval (tr == nullptr, or a BN module the caller keeps in eval mode --
-// train.py:251-256 --freeze_earlier_blocks): one launch with the running statistics folded into the epilogue.
-// Train: the same convolution kernel twice -- raw output (+ conv bias) -> batch mean / biased variance and the
-// running-statistics update (train_fwd.cu) -> the real pass with the batch statistics folded into the epilogue.
-int conv_bn(hn_model* m, const ConvLayer& c, const Act& in, const Act& out, const float* res, cudaStream_t st, int cls,
-            const TrainCtx* tr) {
-    if (!tr || !tr->bn_train[c.bn_index]) return run_conv(m, c, in, out, res, st, cls);
-    const int C = c.d.Cout;
-    const float* bias = c.biaskey.empty() ? nullptr : m->T(c.biaskey);
-    ConvLayer t = c;
-    t.d.relu = 0; t.d.scale = m->trn_scale; t.d.shift = m->trn_shift; t.tc_scale = m->trn_aux;
-    if (bn_identity_constants(bias, m->trn_scale, m->trn_shift, C, st)) return -1;
-    // (the narrow convs have no weight planes: their kernel reads trn_scale / trn_shift directly)
-    if (m->use_tc && c.tc_scale && tc_aux_update(m->trn_scale, m->trn_shift, c.tc_scale + 3 * C, m->trn_aux, C, st)) return -1;
-    if (run_conv(m, t, in, out, nullptr, st, cls)) return -1;
-    if (bn_batch_stats(out, m->use_tc != 0, m->trn_sums, st)) return -1;
-    if (bn_train_finalize(m->trn_sums, (long long)out.B * out.H * out.W, m->T(c.bnprefix + ".weight"),
-                          m->T(c.bnprefix + ".bias"), bias, const_cast<float*>(m->T(c.bnprefix + ".running_mean")),
-                          const_cast<float*>(m->T(c.bnprefix + ".running_var")), tr->bn_factor[c.bn_index],
-                          m->trn_scale, m->trn_shift, C, st))
-        return -1;
-    if (m->use_tc && c.tc_scale && tc_aux_update(m->trn_scale, m->trn_shift, c.tc_scale + 3 * C, m->trn_aux, C, st)) return -1;
-    t.d.relu = c.d.relu;
-    return run_conv(m, t, in, out, res, st, cls);
-}
-
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
 extern "C" {
 
 const char* hn_last_error(void) { return g_err.c_str(); }
-int hn_abi_version(void) { return 6; }
+int hn_abi_version(void) { return 7; }
 const char* hn_build_digest(void) { return HN_BUILD_DIGEST; }
 long long hn_kernel_launches(void) { return g_launches.load(); }
 
@@ -415,7 +389,7 @@ int hn_model_create_arch(int device, int max_batch, const char* backbone, int us
         // plane merge of the "feature" test stage.
         struct { float** p; size_t n; } head_bufs[] = {
             {&m->XP, std::max((size_t)256 * B * CL, (size_t)4096 * 1024)},
-            {&m->HID, 256 * B * 512}, {&m->HIDD, 256 * B * 512},
+            {&m->HID, 256 * B * 512},
         };
         for (auto& b : head_bufs)
             if (m->alloc_t(b.p, b.n)) return -1;
@@ -443,9 +417,6 @@ int hn_model_create_arch(int device, int max_batch, const char* backbone, int us
     }
     if (m->alloc_t(&m->error_flag, 1)) return -1;
     if (m->alloc_t(&m->tta_ints, 128)) return -1;
-    if (m->alloc_t(&m->trn_sums, 2 * 4096) || m->alloc_t(&m->trn_scale, 4096) || m->alloc_t(&m->trn_shift, 4096) ||
-        m->alloc_t(&m->trn_aux, 3 * 4096 + 1))
-        return -1;
     HN_CUDA_OK(cudaMemset(m->error_flag, 0, sizeof(int)));
     m->x_slot[0] = m->x_in;
     m->bon_slot[0] = m->bon_out; m->cor_slot[0] = m->cor_out;
@@ -588,13 +559,9 @@ int hn_model_finalize(hn_model* m) {
 // ---- the three parts of HorizonNet.forward (model.py:254-281); static helpers (no extern "C" linkage needed)
 // (1) normalise + stem + max-pool + layer1..4 + the 16 height-reduction convs: leaves gout[] in GO[0..3]
 static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, Act gout[4], cudaStream_t st,
-                           cudaEvent_t x_consumed, const TrainCtx* tr = nullptr) {
-    if (m->bn_stale) {
-        bool need = !tr;                     // eval forward, or a train forward with frozen (eval-mode) BN modules
-        for (size_t i = 0; tr && i < m->bn_names.size(); ++i) need = need || !tr->bn_train[i];
-        if (need && refold_bn(m, st)) return -1;
-    }
-    if (!tr && m->use_tc && m->fold_on && m->fold_stale) {
+                           cudaEvent_t x_consumed) {
+    if (m->bn_stale && refold_bn(m, st)) return -1;
+    if (m->use_tc && m->fold_on && m->fold_stale) {
         for (int l = 0; l < 4; ++l)
             for (auto& b : m->blocks[l])
                 if (b.has_ds && b.kind == hn_model::BOTTLENECK && pack_fold(m, b, st)) return -1;
@@ -604,30 +571,12 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
     Act s0 = mk(m->S0, B, 256, 512, 64);
     {
         Scope sc(m, CLS_STEM, 2.0 * B * 256 * 512 * 64 * 147, st);
-        const bool tc = m->use_tc && m->stem_tc_on;
-        const bool batch_stats = tr && tr->bn_train[m->stem.bn_index];
-        const float *scale = m->stem.scale, *shift = m->stem.shift, *aux = m->stem_aux;
-        for (int pass = batch_stats ? 0 : 1; pass < 2; ++pass) {
-            if (batch_stats) {          // pass 0: raw stem output -> batch statistics; pass 1: the real thing
-                if (pass == 0 && bn_identity_constants(nullptr, m->trn_scale, m->trn_shift, 64, st)) return -1;
-                if (pass == 1) {
-                    if (bn_batch_stats(s0, false, m->trn_sums, st)) return -1;
-                    if (bn_train_finalize(m->trn_sums, (long long)B * 256 * 512, m->T(m->stem.bnprefix + ".weight"),
-                                          m->T(m->stem.bnprefix + ".bias"), nullptr,
-                                          const_cast<float*>(m->T(m->stem.bnprefix + ".running_mean")),
-                                          const_cast<float*>(m->T(m->stem.bnprefix + ".running_var")),
-                                          tr->bn_factor[m->stem.bn_index], m->trn_scale, m->trn_shift, 64, st))
-                        return -1;
-                }
-                if (tc && tc_aux_update(m->trn_scale, m->trn_shift, m->stem_aux + 3 * 64, m->trn_aux, 64, st)) return -1;
-                scale = m->trn_scale; shift = m->trn_shift; aux = m->trn_aux;
-            }
-            if (tc) {
-                // packed input planes live in X[0] (free until layer1): B * 8.6 MB of its B * 33.8 MB
-                if (stem_tc(x, B, in_channels, m->stem_wq, aux, shift, reinterpret_cast<unsigned short*>(m->X[0]), s0, st,
-                            pass == 1)) return -1;
-            } else if (stem_f32(x, B, in_channels, m->stem.w, scale, shift, s0, st, pass == 1)) return -1;
-        }
+        if (m->use_tc && m->stem_tc_on) {
+            // packed input planes live in X[0] (free until layer1): B * 8.6 MB of its B * 33.8 MB
+            if (stem_tc(x, B, in_channels, m->stem_wq, m->stem_aux, m->stem.shift, reinterpret_cast<unsigned short*>(m->X[0]),
+                        s0, st))
+                return -1;
+        } else if (stem_f32(x, B, in_channels, m->stem.w, m->stem.scale, m->stem.shift, s0, st)) return -1;
     }
     if (x_consumed) HN_CUDA_OK(cudaEventRecord(x_consumed, st));       // the input batch is not read after the stem
     Act cur = mk(m->S1, B, 128, 256, 64);
@@ -648,14 +597,14 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
                 const int s = blk.c1.d.sh;
                 Act t1 = mk(m->T1, B, cur.H / s, cur.W / s, blk.c1.d.Cout);
                 Act y = mk(b == nb - 1 ? m->F[l] : m->X[b & 1], B, t1.H, t1.W, blk.c2.d.Cout);
-                if (conv_bn(m, blk.c1, cur, t1, nullptr, st, CLS_ENC_CONV, tr)) return -1;
+                if (run_conv(m, blk.c1, cur, t1, nullptr, st, CLS_ENC_CONV)) return -1;
                 const float* idn = cur.p;
                 if (blk.has_ds) {
                     Act d = mk(m->IDN, B, t1.H, t1.W, blk.ds.d.Cout);
-                    if (conv_bn(m, blk.ds, cur, d, nullptr, st, CLS_ENC_CONV, tr)) return -1;
+                    if (run_conv(m, blk.ds, cur, d, nullptr, st, CLS_ENC_CONV)) return -1;
                     idn = d.p;
                 }
-                if (conv_bn(m, blk.c2, t1, y, idn, st, CLS_ENC_CONV, tr)) return -1;
+                if (run_conv(m, blk.c2, t1, y, idn, st, CLS_ENC_CONV)) return -1;
                 cur = y;
                 continue;
             }
@@ -664,17 +613,17 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
             Act t1 = mk(m->T1, B, cur.H, cur.W, blk.c1.d.Cout);
             Act t2 = mk(m->T2, B, Ho, Wo, blk.c2.d.Cout);
             Act y = mk(b == nb - 1 ? m->F[l] : m->X[b & 1], B, Ho, Wo, blk.c3.d.Cout);
-            if (conv_bn(m, blk.c1, cur, t1, nullptr, st, CLS_ENC_CONV, tr)) return -1;
-            // eval forward on the tensor cores: the downsample runs inside conv3, one GEMM over [t2 | x] (no identity tensor)
-            const bool fold = blk.has_ds && !tr && m->use_tc && m->fold_on;
+            if (run_conv(m, blk.c1, cur, t1, nullptr, st, CLS_ENC_CONV)) return -1;
+            // on the tensor cores: the downsample runs inside conv3, one GEMM over [t2 | x] (no identity tensor)
+            const bool fold = blk.has_ds && m->use_tc && m->fold_on;
             const float* idn = cur.p;
             if (blk.has_ds && !fold) {
                 Act d = mk(m->IDN, B, Ho, Wo, blk.ds.d.Cout);
-                if (conv_bn(m, blk.ds, cur, d, nullptr, st, CLS_ENC_CONV, tr)) return -1;
+                if (run_conv(m, blk.ds, cur, d, nullptr, st, CLS_ENC_CONV)) return -1;
                 idn = d.p;
             }
             const double conv3_k = blk.c3.d.Cin + (fold ? (double)blk.ds.d.Cin : 0.0);
-            if (!tr && m->use_tc && m->fuse_on && blk.c2.wq && blk.c3.wq && bott_tc_supported(blk.c2.d, blk.c3.d, t1, y) &&
+            if (m->use_tc && m->fuse_on && blk.c2.wq && blk.c3.wq && bott_tc_supported(blk.c2.d, blk.c3.d, t1, y) &&
                 (!fold || (cur.C == 64 && cur.H == t1.H && cur.W == t1.W))) {
                 // layer1: conv2 + conv3 in one kernel, the 64-channel intermediate stays in shared memory (conv_tc.cu)
                 const double flops = 2.0 * (double)B * Ho * Wo * (64.0 * 9 * 64 + (double)blk.c3.d.Cout * conv3_k);
@@ -686,14 +635,14 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
                                    fold ? nullptr : idn_planes, fold ? idn_planes : nullptr, st))
                     return -1;
             } else {
-                if (conv_bn(m, blk.c2, t1, t2, nullptr, st, CLS_ENC_CONV, tr)) return -1;
+                if (run_conv(m, blk.c2, t1, t2, nullptr, st, CLS_ENC_CONV)) return -1;
                 if (fold) {
                     Scope sc(m, CLS_ENC_CONV, 2.0 * (double)B * Ho * Wo * blk.c3.d.Cout * conv3_k, st);
                     if (conv_tc_fold_planes(blk.fold.wq, blk.fold.tc_scale, t2, reinterpret_cast<const unsigned short*>(t2.p),
                                             cur, reinterpret_cast<const unsigned short*>(cur.p), s, y,
                                             reinterpret_cast<unsigned short*>(y.p), st))
                         return -1;
-                } else if (conv_bn(m, blk.c3, t2, y, idn, st, CLS_ENC_CONV, tr)) return -1;   // + identity, ReLU
+                } else if (run_conv(m, blk.c3, t2, y, idn, st, CLS_ENC_CONV)) return -1;   // + identity, ReLU
             }
             cur = y;
         }
@@ -706,7 +655,7 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
         for (int j = 0; j < 4; ++j) {
             const ConvLayer& c = m->ghc[s][j];
             Act o = mk(j == 3 ? m->GO[s] : m->G[j & 1], B, g.H / 2, g.W, c.d.Cout);
-            if (conv_bn(m, c, g, o, nullptr, st, CLS_GHC_CONV, tr)) return -1;
+            if (run_conv(m, c, g, o, nullptr, st, CLS_GHC_CONV)) return -1;
             g = o;
         }
         gout[s] = g;
@@ -721,40 +670,23 @@ static int forward_sequence(hn_model* m, const Act gout[4], cudaStream_t st) {
 }
 
 // (3') model.py:270-279 (use_rnn=False): per-column MLP over the rows of SEQ.  Layer 1 (c_last -> 512, bias, ReLU) is the
-// same GEMM-row convolution as the LSTM projections; dropout (train mode) on the hidden layer; layer 2 + the scatter.
-static int forward_mlp(hn_model* m, int B, float* bon, float* cor, cudaStream_t st, const TrainCtx* tr) {
-    const size_t nh = (size_t)256 * B * 512;
+// same GEMM-row convolution as the LSTM projections; layer 2 + the scatter (eval: the dropout between them = identity).
+static int forward_mlp(hn_model* m, int B, float* bon, float* cor, cudaStream_t st) {
     const Act a = mk(m->SEQ, 1, 1, 256 * B, m->c_last, 0);
     const Act h = mk(m->HID, 1, 1, 256 * B, 512, 0);
     if (run_conv(m, m->mlp1, a, h, nullptr, st, CLS_HEAD, true)) return -1;
-    const float* head_in = m->HID;
-    if (tr && tr->head_p > 0.0) {         // train mode: linear[2] = nn.Dropout(0.5) on the post-ReLU hidden layer
-        Scope sc(m, CLS_HEAD, 0.0, st);
-        HN_CUDA_OK(cudaMemcpyAsync(m->HIDD, m->HID, nh * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        if (tr->mask[1] ? multiply_inplace(m->HIDD, tr->mask[1], nh, st)
-                        : dropout_inplace(m->HIDD, nh, tr->head_p, tr->seed, 1, false, st))
-            return -1;
-        head_in = m->HIDD;
-    }
     Scope sc(m, CLS_HEAD, 2.0 * 256 * B * 12 * 512, st);
-    return linear_head(head_in, m->head_w, m->head_b, bon, cor, 256, B, 512, st);
+    return linear_head(m->HID, m->head_w, m->head_b, bon, cor, 256, B, 512, st);
 }
 
 // (3) model.py:264-281: 2-layer bidirectional LSTM (eval: dropout = identity), linear head, reshape, split
-static int forward_rnn(hn_model* m, int B, float* bon, float* cor, cudaStream_t st, const TrainCtx* tr = nullptr) {
-    if (!m->use_rnn) return forward_mlp(m, B, bon, cor, st, tr);
+static int forward_rnn(hn_model* m, int B, float* bon, float* cor, cudaStream_t st) {
+    if (!m->use_rnn) return forward_mlp(m, B, bon, cor, st);
     const float* lin = m->SEQ;
     float* louts[2] = {m->R1, m->R2};
     for (int layer = 0; layer < 2; ++layer) {
         Act a = mk(const_cast<float*>(lin), 1, 1, 256 * B, m->xproj[layer].d.Cin, 0);
         Act xp = mk(m->XP, 1, 1, 256 * B, 4096, 0);
-        if (tr && layer == 1 && tr->rnn_p > 0.0) {
-            // train mode: nn.LSTM(dropout=p) zeroes layer-1 outputs on their way into layer 2 (model.py:226)
-            Scope sc(m, CLS_TAIL, 0.0, st);
-            if (tr->mask[0] ? multiply_inplace(m->R1, tr->mask[0], (size_t)256 * B * 1024, st)
-                            : dropout_inplace(m->R1, (size_t)256 * B * 1024, tr->rnn_p, tr->seed, 0, false, st))
-                return -1;
-        }
         if (m->use_tc && layer == 1) {
             // layer-2 projection operand: the fp32 recurrence output as fp16 hi/lo planes
             Scope sc(m, CLS_TAIL, 0.0, st);
@@ -767,12 +699,6 @@ static int forward_rnn(hn_model* m, int B, float* bon, float* cor, cudaStream_t 
             if (lstm_layer(m->XP, m->whh[layer][0], m->whh[layer][1], louts[layer], 256, B, st)) return -1;
         }
         lin = louts[layer];
-    }
-    if (tr && tr->head_p > 0.0) {         // train mode: self.drop_out before the linear head (model.py:265)
-        Scope sc(m, CLS_TAIL, 0.0, st);
-        if (tr->mask[1] ? multiply_inplace(m->R2, tr->mask[1], (size_t)256 * B * 1024, st)
-                        : dropout_inplace(m->R2, (size_t)256 * B * 1024, tr->head_p, tr->seed, 1, false, st))
-            return -1;
     }
     {
         Scope sc(m, CLS_HEAD, 2.0 * 256 * B * 12 * 1024, st);
@@ -834,35 +760,6 @@ int hn_model_num_bn(const hn_model* m) { return m ? (int)m->bn_names.size() : 0;
 
 const char* hn_model_bn_name(const hn_model* m, int i) {
     return (m && i >= 0 && i < (int)m->bn_names.size()) ? m->bn_names[i].c_str() : nullptr;
-}
-
-int hn_model_forward_train(hn_model* m, const float* x, int B, int in_channels, float* bon, float* cor,
-                           const unsigned char* bn_train, const double* bn_factor, int n_bn, unsigned long long seed,
-                           double rnn_dropout, double head_dropout, const float* rnn_mask, const float* head_mask,
-                           void* stream) {
-    if (forward_args_ok(m, x, B, bon, cor, "hn_model_forward_train")) return -1;
-    HN_CHECK(bn_train && bn_factor && n_bn == (int)m->bn_names.size(),
-             "hn_model_forward_train: bn_train / bn_factor need hn_model_num_bn() entries");
-    HN_CHECK(rnn_dropout >= 0.0 && rnn_dropout < 1.0 && head_dropout >= 0.0 && head_dropout < 1.0,
-             "hn_model_forward_train: dropout probabilities must be in [0, 1)");
-    HN_CHECK(m->use_rnn || (rnn_dropout == 0.0 && !rnn_mask),
-             "hn_model_forward_train: the MLP head (use_rnn = 0) has no LSTM: rnn_dropout must be 0 and rnn_mask NULL");
-    HN_ON_DEVICE(m->device);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (m->rnn_inflight) {
-        HN_CUDA_OK(cudaStreamWaitEvent(st, m->ev_rnn_last, 0));
-        m->rnn_inflight = false;
-    }
-    m->last_batch = B;
-    const TrainCtx tr{bn_train, bn_factor, seed, rnn_dropout, head_dropout, {rnn_mask, head_mask}};
-    Act gout[4];
-    if (forward_encoder(m, x, B, in_channels, gout, st, nullptr, &tr)) return -1;
-    if (forward_sequence(m, gout, st)) return -1;
-    if (forward_rnn(m, B, bon, cor, st, &tr)) return -1;
-    for (int i = 0; i < n_bn; ++i) m->bn_stale = m->bn_stale || (bn_train[i] && bn_factor[i] >= 0.0);
-    HN_CUDA_OK(cudaEventRecord(m->ev_plain_done, st));
-    m->plain_recorded = true;
-    return 0;
 }
 
 int hn_model_get_tensor(hn_model* m, const char* key, float* out, long long numel, int on_device, void* stream) {

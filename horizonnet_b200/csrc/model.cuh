@@ -76,15 +76,6 @@ struct ConvLayer {
     int bn_index = -1;                // position in hn_model::bn_names (train mode: which BatchNorm2d module this is)
 };
 
-// Train-mode forward (hn_model_forward_train): per-BatchNorm2d switches handed in by the caller
-struct TrainCtx {
-    const unsigned char* bn_train;    // [n_bn] 1: batch statistics + running update, 0: module is in eval mode
-    const double* bn_factor;          // [n_bn] exponential_average_factor (momentum, or 1/num_batches_tracked); < 0: none
-    unsigned long long seed;
-    double rnn_p, head_p;             // dropout probabilities (0: off)
-    const float* mask[2];             // caller-supplied multiplicative masks instead of the Philox ones (parity tests)
-};
-
 
 }  // namespace hn
 
@@ -123,12 +114,9 @@ struct hn_model {
     int stem_tc_on = 1;                              // option "stem_tc" / HN_TC_STEM=0: fp32 CUDA-core stem inside the TC path
     int fuse_on = 1;                                 // option "fuse_bottleneck": fused conv2+conv3 kernel for layer1 (bit-identical)
     int fold_on = 1;                                 // option "fold_downsample": block-0 downsample inside conv3 (eval, TC)
-    // train-mode scratch (one layer at a time, stream ordered): batch sums, scale/shift, tensor-core epilogue constants
     std::shared_ptr<void> train_state;               // tape + gradient buffers of the training step (train_step.cu)
     bool bn_stale = false;     // running statistics moved (train forward) since the eval-mode constants were folded
     bool fold_stale = true;    // weights or eval-mode BN constants changed since the folded block-0 packs were built
-    double* trn_sums = nullptr;
-    float *trn_scale = nullptr, *trn_shift = nullptr, *trn_aux = nullptr;
 
     // workspace (sized for max_batch)
     float *S0 = nullptr, *S1 = nullptr, *X[2] = {nullptr, nullptr}, *IDN = nullptr, *T1 = nullptr, *T2 = nullptr;
@@ -136,7 +124,7 @@ struct hn_model {
     float* G[2] = {nullptr, nullptr};
     float* GO[4] = {nullptr, nullptr, nullptr, nullptr};
     float *SEQ = nullptr, *XP = nullptr, *R1 = nullptr, *R2 = nullptr, *R1S = nullptr;
-    float *HID = nullptr, *HIDD = nullptr;           // MLP head: hidden layer [T][B][512] after ReLU, and after dropout
+    float* HID = nullptr;                            // MLP head: hidden layer [T][B][512] after ReLU
     int* error_flag = nullptr;                       // set by a grid-barrier time-out of the cooperative BPTT kernel
     float *x_in = nullptr, *bon_out = nullptr, *cor_out = nullptr;    // for forward_host
     // pipelined host API: 2 input slots, a copy stream and a compute stream (H2D of batch i+1 overlaps forward i)

@@ -1,56 +1,38 @@
-// Train-mode pieces of HorizonNet.forward (reference train.py:52 calls net(x) under net.train()):
-//   * batch-statistics BatchNorm2d (torch.nn.BatchNorm2d training branch; reference model.py:130 and torchvision
-//     Bottleneck bn1..bn3 / downsample.1): per-channel mean and biased variance over (B, H, W) of the raw convolution
-//     output, running_mean / running_var update with the unbiased variance and the module's momentum;
+// Train-mode pieces of HorizonNet.forward (reference train.py:52 calls net(x) under net.train()) that the training step
+// (train_step.cu) runs around its convolutions:
+//   * batch statistics for BatchNorm2d (torch.nn.BatchNorm2d training branch; reference model.py:130 and torchvision
+//     Bottleneck bn1..bn3 / downsample.1): per-channel sums of the raw convolution output and of its square, from which
+//     bn_finalize_full (bwd_kernels.cu) takes the batch mean, the biased variance and the running-statistics update;
 //   * dropout (nn.LSTM(dropout=0.5) between the two recurrent layers, model.py:226, and nn.Dropout(0.5) before the
 //     linear head, model.py:228 / :265): counter-based Philox4x32-10 masks, so a mask is a pure function of
 //     (seed, which, element index) and the oracle can be handed exactly the mask the device applied.
-// The convolutions themselves are the inference kernels: model.cu runs each one twice in train mode -- once with an
-// identity epilogue to obtain the raw output the statistics are taken from, once with the batch-statistics scale/shift
-// (+ identity + ReLU) folded into the same epilogue as in eval mode.  That is a first correct path, not a fast one:
-// the backward pass (SURVEY 8 row f1) is not built.
 #include "hn_common.cuh"
-#include "conv_tc.cuh"
 
 namespace hn {
 namespace {
 
 constexpr int ST_THREADS = 256;
 
-__device__ __forceinline__ float plane_value(const unsigned short* __restrict__ hi, const unsigned short* __restrict__ lo,
-                                             size_t i) {
-    return (__half2float(__ushort_as_half(hi[i])) + __half2float(__ushort_as_half(lo[i]))) * ACT_UNSCALE;
-}
-
-// sums[c] += sum z, sums[C + c] += sum z^2 over the interior pixels of a halo-NHWC tensor (fp32, or fp16 hi/lo planes).
+// sums[c] += sum z, sums[C + c] += sum z^2 over the interior pixels of a fp32 halo-NHWC tensor.
 // Block = CL4 channel-quad lanes x (256 / CL4) pixel lanes: a thread owns 4 consecutive channels (one 16-byte load per
 // pixel) and walks its rows with 32-bit index arithmetic (round 2: the first version spent its time in 64-bit
 // divisions of a flat pixel index and scalar loads: 5.3 ms per batch-8 training step for 3.4 GB of input); the sums
 // stay fp64 per element, so the statistics are unchanged.
-template <bool PLANES>
 __global__ void __launch_bounds__(ST_THREADS)
-bn_stats_kernel(const void* __restrict__ z, int rows, int W, int C, int halo, int CL4, double* __restrict__ sums) {
+bn_stats_kernel(const float* __restrict__ z, int rows, int W, int C, int halo, int CL4, double* __restrict__ sums) {
     __shared__ double sh[ST_THREADS][8];
     const int cl = threadIdx.x % CL4, pl = threadIdx.x / CL4, PL = ST_THREADS / CL4;
     const int c4 = blockIdx.x * CL4 + cl;
     const bool active = c4 * 4 < C;
     const int Wp = W + 2 * halo;
-    const size_t plane = (size_t)rows * Wp * C;
     double a[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     if (active) {
         for (int row = blockIdx.y; row < rows; row += gridDim.y) {
             const size_t base = ((size_t)row * Wp + halo) * C + (size_t)c4 * 4;
             for (int w = pl; w < W; w += PL) {
                 const size_t i = base + (size_t)w * C;
-                float v[4];
-                if (PLANES) {
-                    const unsigned short* q = static_cast<const unsigned short*>(z);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) v[j] = plane_value(q, q + plane, i + j);
-                } else {
-                    const float4 f = *reinterpret_cast<const float4*>(static_cast<const float*>(z) + i);
-                    v[0] = f.x; v[1] = f.y; v[2] = f.z; v[3] = f.w;
-                }
+                const float4 f = *reinterpret_cast<const float4*>(z + i);
+                const float v[4] = {f.x, f.y, f.z, f.w};
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     a[j] += (double)v[j];
@@ -72,38 +54,6 @@ bn_stats_kernel(const void* __restrict__ z, int rows, int W, int C, int halo, in
             atomicAdd(sums + C + c4 * 4 + j, a[4 + j]);
         }
     }
-}
-
-// torch.nn.functional.batch_norm(training=True): normalise with the batch mean and the BIASED variance; running
-// statistics move by `factor` (= momentum, or 1/num_batches_tracked when momentum is None) towards the batch mean and
-// the UNBIASED variance.  Output: the epilogue constants of the second convolution pass,
-//   y = conv * scale + shift,  scale = gamma / sqrt(var + eps),  shift = beta + (bias - mean) * scale
-// (`mean` already contains the conv bias because the first pass added it).
-__global__ void bn_finalize_kernel(const double* __restrict__ sums, double count, const float* __restrict__ gamma,
-                                   const float* __restrict__ beta, const float* __restrict__ bias,
-                                   float* __restrict__ running_mean, float* __restrict__ running_var, double factor,
-                                   float* __restrict__ scale, float* __restrict__ shift, int C) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= C) return;
-    const double mean = sums[i] / count;
-    double var = sums[C + i] / count - mean * mean;
-    if (var < 0.0) var = 0.0;
-    const double s = (double)gamma[i] / sqrt(var + 1e-5);
-    const double b = bias ? (double)bias[i] : 0.0;
-    scale[i] = (float)s;
-    shift[i] = (float)((double)beta[i] + (b - mean) * s);
-    if (running_mean && factor >= 0.0) {
-        const double unbiased = count > 1.0 ? var * count / (count - 1.0) : var;
-        running_mean[i] = (float)((1.0 - factor) * (double)running_mean[i] + factor * mean);
-        running_var[i] = (float)((1.0 - factor) * (double)running_var[i] + factor * unbiased);
-    }
-}
-
-__global__ void ident_kernel(const float* __restrict__ bias, float* __restrict__ scale, float* __restrict__ shift, int C) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= C) return;
-    scale[i] = 1.f;
-    shift[i] = bias ? bias[i] : 0.f;
 }
 
 // ---- Philox4x32-10 (Salmon et al., SC'11): counter = (index / 4, which, 0, 0), key = seed
@@ -154,7 +104,7 @@ int multiply_inplace(float* x, const float* mask, size_t n, cudaStream_t st) {
     return 0;
 }
 
-int bn_batch_stats(const Act& z, bool planes, double* sums, cudaStream_t st) {
+int bn_batch_stats(const Act& z, double* sums, cudaStream_t st) {
     HN_CHECK(z.C >= 4 && z.C <= 4096 && z.C % 4 == 0 && z.B >= 1, "bn_batch_stats: bad tensor (C must be a multiple of 4)");
     HN_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * (size_t)z.C * sizeof(double), st));
     const int C4 = z.C / 4;
@@ -167,23 +117,7 @@ int bn_batch_stats(const Act& z, bool planes, double* sums, cudaStream_t st) {
     if (ysplit > rows) ysplit = rows;
     if (ysplit > 65535) ysplit = 65535;
     dim3 grid((unsigned)cblocks, (unsigned)ysplit);
-    if (planes) bn_stats_kernel<true><<<grid, ST_THREADS, 0, st>>>(z.p, (int)rows, z.W, z.C, z.halo, CL4, sums);
-    else bn_stats_kernel<false><<<grid, ST_THREADS, 0, st>>>(z.p, (int)rows, z.W, z.C, z.halo, CL4, sums);
-    HN_LAUNCH_OK();
-    return 0;
-}
-
-int bn_train_finalize(const double* sums, long long count, const float* gamma, const float* beta, const float* bias,
-                      float* running_mean, float* running_var, double factor, float* scale, float* shift, int C,
-                      cudaStream_t st) {
-    bn_finalize_kernel<<<(C + 255) / 256, 256, 0, st>>>(sums, (double)count, gamma, beta, bias, running_mean, running_var,
-                                                        factor, scale, shift, C);
-    HN_LAUNCH_OK();
-    return 0;
-}
-
-int bn_identity_constants(const float* bias, float* scale, float* shift, int C, cudaStream_t st) {
-    ident_kernel<<<(C + 255) / 256, 256, 0, st>>>(bias, scale, shift, C);
+    bn_stats_kernel<<<grid, ST_THREADS, 0, st>>>(z.p, (int)rows, z.W, z.C, z.halo, CL4, sums);
     HN_LAUNCH_OK();
     return 0;
 }

@@ -24,6 +24,15 @@ namespace {
 
 constexpr int T_STEPS = 256;
 
+// Arguments of hn_train_forward: per-BatchNorm2d switches and the dropouts, kept on the tape for the backward
+struct TrainCtx {
+    const unsigned char* bn_train;    // [n_bn] 1: batch statistics + running update, 0: module is in eval mode
+    const double* bn_factor;          // [n_bn] exponential_average_factor (momentum, or 1/num_batches_tracked); < 0: none
+    unsigned long long seed;
+    double rnn_p, head_p;             // dropout probabilities (0: off)
+    const float* mask[2];             // caller-supplied multiplicative masks instead of the Philox ones (parity tests)
+};
+
 struct Bump {
     float* base = nullptr;
     size_t off = 0;
@@ -135,7 +144,7 @@ int unit_forward(hn_model* m, TrainState* ts, Bump& Y, Bump& Z, Bump& BN, const 
             if (tc_aux_update(ts->ones, raw.shift, c.tc_scale + 3 * c.d.Cout, ts->aux_tmp, c.d.Cout, st)) return -1;
             if (conv_tc_planes(raw, c.wq, ts->aux_tmp, in, planes_of(ts, in), u.z, nullptr, u.z.p, nullptr, st)) return -1;
         } else if (conv_f32(raw, in, u.z, nullptr, st)) return -1;
-        if (u.train && bn_batch_stats(u.z, false, ts->sums, st)) return -1;
+        if (u.train && bn_batch_stats(u.z, ts->sums, st)) return -1;
         if (bn_finalize_full(ts->sums, (long long)in.B * Ho * Wo, m->T(c.bnprefix + ".weight"), m->T(c.bnprefix + ".bias"),
                              bias, const_cast<float*>(m->T(c.bnprefix + ".running_mean")),
                              const_cast<float*>(m->T(c.bnprefix + ".running_var")), tr.bn_factor[c.bn_index], u.train, u.bn,
@@ -174,7 +183,7 @@ int walk_forward(hn_model* m, TrainState* ts, const float* x, int B, int in_chan
                             u.z, st, false))
                     return -1;
             } else if (stem_f32(x, B, in_channels, m->stem.w, ts->ones, ts->zeros, u.z, st, false)) return -1;
-            if (u.train && bn_batch_stats(u.z, false, ts->sums, st)) return -1;
+            if (u.train && bn_batch_stats(u.z, ts->sums, st)) return -1;
             const std::string& p = m->stem.bnprefix;
             if (bn_finalize_full(ts->sums, (long long)B * 256 * 512, m->T(p + ".weight"), m->T(p + ".bias"), nullptr,
                                  const_cast<float*>(m->T(p + ".running_mean")), const_cast<float*>(m->T(p + ".running_var")),
@@ -604,6 +613,9 @@ int hn_train_forward(hn_model* m, const float* x, int B, int in_channels, float*
     ts->have_tape = true;
     for (int i = 0; i < n_bn; ++i) m->bn_stale = m->bn_stale || (bn_train[i] && bn_factor[i] >= 0.0);
     m->last_batch = B;
+    // the stem scratch X[0] and the running statistics are shared with the two-stream forwards: they wait for this
+    HN_CUDA_OK(cudaEventRecord(m->ev_plain_done, st));
+    m->plain_recorded = true;
     return 0;
 }
 
@@ -793,7 +805,7 @@ int hn_bn_forward_backward(const float* z, int B, int H, int W, int C, const flo
                            double* sums, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     Act za = mk(const_cast<float*>(z), B, H, W, C), ya = mk(y, B, H, W, C);
-    if (train && bn_batch_stats(za, false, sums, st)) return -1;
+    if (train && bn_batch_stats(za, sums, st)) return -1;
     if (bn_finalize_full(sums, (long long)B * H * W, gamma, beta, nullptr, running_mean, running_var, factor, train != 0,
                          bn_scratch, C, st))
         return -1;

@@ -13,7 +13,8 @@ per-column MLP head of model.py:234-243, what the reference's ``train.py --no_rn
 (eval) forward -- plus the train-mode FORWARD (batch-statistics BatchNorm with running-stat updates,
 LSTM / head dropout; train.py:52) and its backward (train.py:278 ``loss.backward()``): with autograd on,
 ``forward`` in train mode returns outputs whose grad_fn runs the library's backward pass and fills
-``.grad`` of every parameter -- row f1 as a first correct fp32 path (not tensor-core, no DDP).  The modules below are parameter containers with the reference's names; none of
+``.grad`` of every parameter (row f1; one process per GPU, ``parallel.average_gradients`` in place of DataParallel).
+The modules below are parameter containers with the reference's names; none of
 their torch ``forward`` methods is ever called -- all arithmetic runs in the CUDA library, and there
 is no CPU fallback: a CPU tensor or a missing library raises.
 """
@@ -139,7 +140,7 @@ class _TrainStep(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, net, x, *params):
-        bon, cor = net._train_forward_impl(x, tape=True)
+        bon, cor = net._train_forward_impl(x)
         ctx.net, ctx.device = net, x.device
         ctx.wanted = [p.requires_grad for p in params]
         return bon, cor
@@ -313,16 +314,16 @@ class HorizonNet(nn.Module):
         generator (reproducible under torch.manual_seed) and kept in ``last_dropout_seed``; the masks are this
         library's Philox stream, not torch's.
 
-        With autograd on and a parameter that requires grad this is the TRAINING STEP's forward (hn_train_forward:
-        exact-fp32 kernels + a tape) and the outputs carry a grad_fn whose backward is hn_train_backward: the
-        reference's ``loss.backward()`` (train.py:278) then fills ``.grad`` of every parameter.  Otherwise (no_grad /
-        all frozen) the tensor-core forward without tape runs (hn_model_forward_train)."""
+        Every call runs the training step's forward (hn_train_forward, which keeps a tape; batch <= 64), so the
+        outputs do not depend on whether autograd is on.  With autograd on and a parameter that requires grad they
+        carry a grad_fn whose backward is hn_train_backward: the reference's ``loss.backward()`` (train.py:278) then
+        fills ``.grad`` of every parameter."""
         params = [(k, p) for k, p in self.named_parameters()]
         if torch.is_grad_enabled() and any(p.requires_grad for _, p in params):
             return _TrainStep.apply(self, x, *[p for _, p in params])
-        return self._train_forward_impl(x, tape=False)
+        return self._train_forward_impl(x)
 
-    def _train_forward_impl(self, x, tape):
+    def _train_forward_impl(self, x):
         x, B, C, h, bon, cor, stream = self._forward_prologue(x, train=True)
         lib = _lib.lib()
         bns = self._bn_modules(h)
@@ -344,12 +345,12 @@ class HorizonNet(nn.Module):
                      for t in self.dropout_masks_override]
             shapes = [(256, B, 2 * RNN_HIDDEN)] * 2 if self.use_rnn else [None, (256, B, RNN_HIDDEN)]
             assert all((t is None and s is None) or (t is not None and t.shape == s) for t, s in zip(masks, shapes))
-        fn = lib.hn_train_forward if tape else lib.hn_model_forward_train
-        _lib.check(fn(h['ptr'], x.data_ptr(), B, C, bon.data_ptr(), cor.data_ptr(), flags, factors, len(bns), seed, rnn_p,
-                      head_p, masks[0].data_ptr() if masks[0] is not None else None,
-                      masks[1].data_ptr() if masks[1] is not None else None, stream),
-                   'hn_train_forward' if tape else 'hn_model_forward_train')
-        h['tape_keepalive'] = (x, masks) if tape else None     # the backward reads the masks again
+        _lib.check(lib.hn_train_forward(h['ptr'], x.data_ptr(), B, C, bon.data_ptr(), cor.data_ptr(), flags, factors,
+                                        len(bns), seed, rnn_p, head_p,
+                                        masks[0].data_ptr() if masks[0] is not None else None,
+                                        masks[1].data_ptr() if masks[1] is not None else None, stream),
+                   'hn_train_forward')
+        h['tape_keepalive'] = (x, masks)        # the backward reads the masks again
         with torch.no_grad():
             for i, (name, m) in enumerate(bns):
                 if factors[i] < 0:

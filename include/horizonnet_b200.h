@@ -82,9 +82,20 @@ int hn_model_forward_async(hn_model* m, const float* x_nchw_dev, int batch, int 
 /* Makes `stream` wait for every forward enqueued so far by hn_model_forward_async. */
 int hn_model_flush(hn_model* m, void* stream);
 
-/* TRAIN-mode forward: what `net(x)` computes under `net.train()` (reference train.py:52 inside feed_forward,
- * model.py:254-281 with every nn.BatchNorm2d in training mode and the dropouts active); the backward pass is
- * hn_train_forward / hn_train_backward below.
+/* The BatchNorm2d modules in graph order (hn_train_forward's bn_train / bn_factor index them) and their state_dict
+ * prefixes. */
+int hn_model_num_bn(const hn_model* m);
+const char* hn_model_bn_name(const hn_model* m, int i);
+/* The dropout factors (0 or 1/(1-p)) hn_train_forward multiplies with for this seed and `which` (see below). */
+int hn_dropout_mask(unsigned long long seed, int which, double p, float* out_dev, long long n, void* stream);
+/* Current device copy of a state_dict tensor (e.g. "...bn1.running_mean" after train forwards) -> out
+ * (device pointer if on_device, else host; the host form synchronises). */
+int hn_model_get_tensor(hn_model* m, const char* key, float* out, long long numel, int on_device, void* stream);
+
+/* Training step (row f1; reference train.py:44-58 feed_forward + :272-281 backward).
+ * hn_train_forward is the TRAIN-mode forward: what `net(x)` computes under `net.train()` (reference train.py:52 inside
+ * feed_forward, model.py:254-281 with every nn.BatchNorm2d in training mode and the dropouts active), with or without
+ * autograd.  It keeps a tape (every conv output and activation) for hn_train_backward; batch <= 64.
  *   - BatchNorm2d i (i < hn_model_num_bn(m), state_dict prefix hn_model_bn_name(m, i)): bn_train[i] = 1 normalises
  *     with the batch mean / biased variance of the raw conv output and moves running_mean / running_var (the device
  *     copies inside the model, read them back with hn_model_get_tensor) by bn_factor[i] (= the module's momentum, or
@@ -99,21 +110,7 @@ int hn_model_flush(hn_model* m, void* stream);
  *     the p of linear[2] (model.py:240), which acts on the post-ReLU hidden layer: which = 1 over 256*batch*512
  *     elements, head_mask_dev [256][batch][512] (row t*batch + b, the library's order; the reference's own mask is
  *     [batch][256][512]).
- * Each convolution runs twice (statistics pass + real pass); eval-mode entry points called afterwards fold the moved
- * running statistics again on their own. */
-int hn_model_num_bn(const hn_model* m);
-const char* hn_model_bn_name(const hn_model* m, int i);
-int hn_model_forward_train(hn_model* m, const float* x_nchw_dev, int batch, int in_channels, float* bon_dev,
-                           float* cor_dev, const unsigned char* bn_train, const double* bn_factor, int n_bn,
-                           unsigned long long seed, double rnn_dropout, double head_dropout,
-                           const float* rnn_mask_dev, const float* head_mask_dev, void* stream);
-int hn_dropout_mask(unsigned long long seed, int which, double p, float* out_dev, long long n, void* stream);
-/* Current device copy of a state_dict tensor (e.g. "...bn1.running_mean" after train forwards) -> out
- * (device pointer if on_device, else host; the host form synchronises). */
-int hn_model_get_tensor(hn_model* m, const char* key, float* out, long long numel, int on_device, void* stream);
-
-/* Training step (row f1; reference train.py:44-58 feed_forward + :272-281 backward).  hn_train_forward = the train-mode
- * forward above (same arguments) but with a tape: every conv output and activation is kept.
+ * Eval-mode entry points called afterwards fold the moved running statistics again on their own.
  * hn_train_backward takes d(loss)/d(bon) [batch][2][1024] and d(loss)/d(cor) [batch][1][1024] (device) -- the losses
  * themselves (train.py:53-56: L1 + BCE-with-logits) and the optimizer (train.py:216-223) stay with the caller -- and
  * leaves d(loss)/d(parameter) for every state_dict parameter in the reference's layout (nn.Conv2d OIHW, nn.LSTM

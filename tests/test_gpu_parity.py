@@ -528,7 +528,7 @@ def test_train_forward_matches_the_real_reference_golden(golden_dir, name, tenso
     g, sd, x, masks, running, frozen = train_golden(golden_dir, name)
     net = _train_net(sd, tensor_cores, frozen, float(g['momentum']) if name == 'frozen1' else None)
     net.dropout_masks_override = masks
-    with torch.no_grad():                        # no tape: the tensor-core / fp32 inference kernels, each conv twice
+    with torch.no_grad():                        # the training step's forward, its tape left unused
         bon, cor = net(x.to(DEV))
     net.check()
     assert np.abs(bon.cpu().numpy() - g['bon']).max() < 1e-4
@@ -593,6 +593,26 @@ def test_train_forward_with_device_dropout_masks_matches_oracle_and_is_seeded():
     with torch.no_grad():
         rb, rc = horizonnet_ref.forward(sd, x, train=tm)
     assert (b3.cpu() - rb).abs().max().item() < 1e-4 and (c3.cpu() - rc).abs().max().item() < 1e-4
+
+
+def test_train_forward_is_the_same_with_and_without_autograd():
+    """net.train(); net(x) computes one thing: under torch.no_grad() (e.g. BatchNorm re-estimation) it is the training
+    step's forward too, so outputs and moved running statistics are bit-identical to a call with autograd on."""
+    sd = synthetic_state_dict(5, 'random')
+    x = synthetic_panoramas(2, seed=37).to(DEV)
+    out = []
+    for grad in (False, True):
+        net = _train_net(sd, True)
+        torch.manual_seed(21)
+        with torch.set_grad_enabled(grad):
+            bon, cor = net(x)
+        assert bon.requires_grad == grad
+        out.append((bon.detach(), cor.detach(), net.state_dict()))
+    net.check()
+    (b0, c0, s0), (b1, c1, s1) = out
+    assert torch.equal(b0, b1) and torch.equal(c0, c1)
+    for k in s0:
+        assert torch.equal(s0[k], s1[k]), k
 
 
 # ------------------------------------------------------------------------------- training step: backward (row f1)
