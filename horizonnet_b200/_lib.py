@@ -8,7 +8,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libhorizonnet_b200.so')
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 _lib = None
 _lock = threading.Lock()
@@ -49,7 +49,7 @@ SIGNATURES = {
     'hn_conv_tc_plan': (ctypes.c_int, [ctypes.c_int] * 16 + [c_int_p]),
     'hn_conv_tc_fold_plan': (ctypes.c_int, [ctypes.c_int] * 8 + [c_int_p]),
     'hn_conv_tc_fold': (ctypes.c_int, [vp, vp] + [ctypes.c_int] * 7 + [vp, vp, vp, vp]),
-    'hn_bott_tc_fold': (ctypes.c_int, [vp, vp] + [ctypes.c_int] * 3 + [vp] * 5 + [ctypes.c_int, vp, vp]),
+    'hn_bott_tc': (ctypes.c_int, [vp] * 3 + [ctypes.c_int] * 3 + [vp] * 6 + [ctypes.c_int, vp, vp]),
     'hn_wgrad_tc_enabled': (ctypes.c_int, []),
     'hn_bn_forward_backward': (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp,
                                               ctypes.c_double, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp,

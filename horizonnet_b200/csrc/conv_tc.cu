@@ -993,12 +993,11 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 //             an epilogue buffer ahead of use, updated in place and TMA-stored (the epilogue of gemm_tc_kernel),
 //             halo columns by direct stores.
 // The 64-channel intermediate never visits HBM, and the TMA engine streams the residual and the output of one
-// conv3 tile while the next one computes.  Results are bit-identical to the unfused kernels (same products, same
-// accumulator structure, same epilogue arithmetic); HN_TC_FUSE=0 selects the unfused path.
+// conv3 tile while the next one computes.
 // With the downsample folded in (`fold`, layer1.0) conv3 has no residual: the producer loads the tile's 128 pixels of
 // the block input x once, into the next input-row slot, and every conv3 n-tile accumulates two K chunks, t2 and that x
 // tile, against the folded weights [s3 W3 ; sd Wd] -- the same products in the same order as conv_tc_kernel's two-source
-// conv3, so the result stays bit-identical to the unfused path.
+// conv3.
 //   warp 0      TMA producer (input rows, the x tile, then the conv2 and conv3 weight tiles of the tile through one ring)
 //   warp 2      residual-tile loader          warp 3   TMA store          warps 4-11   two consumer warpgroups
 struct BottArgs {
@@ -1389,10 +1388,9 @@ static long long plan_rows(const ConvDesc& d, const Act& in, const Act& out, boo
     p->box_rows = p->box_imgs = 1;
     if (out.H % p->rows_per_tile == 0) p->box_rows = p->rows_per_tile;
     else { p->box_rows = out.H; p->box_imgs = p->rows_per_tile / out.H; }
-    // dx reuse (HN_TC_DXR=0 disables).  Its epilogue slot is two weight slots, each half an output tile: a plane, or
-    // half of the fp32 boxes -- which needs two of them (BN >= 64)
-    static const int dxr_mode = [] { const char* e = getenv("HN_TC_DXR"); return e ? atoi(e) : 1; }();
-    p->dxr = (dxr_mode != 0 && !p->parity && d.kw == 3 && p->rows_per_tile == 1 && p->tw == BM &&
+    // dx reuse.  Its epilogue slot is two weight slots, each half an output tile: a plane, or half of the fp32 boxes --
+    // which needs two of them (BN >= 64)
+    p->dxr = (!p->parity && d.kw == 3 && p->rows_per_tile == 1 && p->tw == BM &&
               !(out_f32 && p->BN < 64) &&
               (long long)p->wsegs * BM + (in.halo - d.pw) + 2 <= (long long)in.Wp()) ? 1 : 0;
     return (long long)((p->M + p->rows_per_tile - 1) / p->rows_per_tile) * p->wsegs;
@@ -1410,8 +1408,7 @@ int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32,
     p->box_rows = p->box_imgs = 1;
     long long m_tiles;
     // asynchronous-epilogue GEMM kernel: plane output, Cin <= 256, Cout a multiple of 64
-    static const bool gemm_kernel_on = [] { const char* e = getenv("HN_TC_GEMM"); return !(e && atoi(e) == 0); }();
-    if (gemm && gemm_kernel_on && !out_f32 && d.Cin <= 256 && d.Cout % GBN == 0 && d.Cout <= GSmem::MAX_COUT) {
+    if (gemm && !out_f32 && d.Cin <= 256 && d.Cout % GBN == 0 && d.Cout <= GSmem::MAX_COUT) {
         const long long Mtot = (long long)in.B * in.H * in.Wp();
         p->gemm_kernel = 1;
         p->BN = GBN;
@@ -1571,8 +1568,6 @@ int conv_tc_fold_planes(const unsigned short* wq, const float* tc_aux, const Act
 
 // ---------------------------------------------------------------------- fused conv2 + conv3 of a bottleneck (host side)
 bool bott_tc_supported(const ConvDesc& d2, const ConvDesc& d3, const Act& in, const Act& out) {
-    static const bool on = [] { const char* e = getenv("HN_TC_FUSE"); return !(e && atoi(e) == 0); }();
-    if (!on) return false;
     return d2.kh == 3 && d2.kw == 3 && d2.sh == 1 && d2.sw == 1 && d2.ph == 1 && d2.pw == 1 && d2.Cin == 64 && d2.Cout == 64 &&
            d2.relu && d3.kh == 1 && d3.kw == 1 && d3.sh == 1 && d3.sw == 1 && d3.Cin == 64 && d3.Cout % 64 == 0 && d3.relu &&
            in.halo == 1 && out.halo == 1 && in.H == out.H && in.W == out.W && in.B == out.B && out.W % BM == 0 &&
@@ -1842,7 +1837,7 @@ int conv_tc(const ConvDesc& d, const Act& in, const Act& out, const float* resid
     return rc;
 }
 
-// Unit-test conveniences of the folded conv3 and of the fused layer1.0 bottleneck: fp32 halo-NHWC tensors in and out,
+// Unit-test conveniences of the folded conv3 and of the fused layer1 bottleneck: fp32 halo-NHWC tensors in and out,
 // planes and packed weights built on the fly.  `bufs` holds the device allocations, freed on every path.
 namespace {
 struct DevBufs {
@@ -1876,27 +1871,28 @@ int conv_tc_fold(const float* w, const float* shift, const Act& t2, const Act& x
     return merge_planes(po, out.p, out.numel(), st);
 }
 
-int bott_tc_fold(const float* w2, const float* scale2, const float* shift2, const float* w3, const float* shift3,
-                 const Act& in, const Act& x, const Act& out, cudaStream_t st) {
+int bott_tc_f32(const float* w2, const float* scale2, const float* shift2, const float* w3, const float* scale3,
+                const float* shift3, const Act& in, const float* res, const float* x, const Act& out, cudaStream_t st) {
     ConvDesc d2, d3;
     memset(&d2, 0, sizeof(d2));
     d2.Cin = d2.Cout = 64; d2.kh = d2.kw = 3; d2.sh = d2.sw = 1; d2.ph = d2.pw = 1; d2.relu = 1;
     d3 = d2;
     d3.Cout = out.C; d3.kh = d3.kw = 1; d3.ph = d3.pw = 0;
-    HN_CHECK(bott_tc_supported(d2, d3, in, out), "bott_tc_fold: unsupported shape");
-    HN_CHECK(x.B == in.B && x.H == in.H && x.W == in.W && x.C == 64 && x.halo == in.halo,
-             "bott_tc_fold: x must have the conv2 input's geometry");
+    HN_CHECK(bott_tc_supported(d2, d3, in, out), "bott_tc_f32: unsupported shape");
+    HN_CHECK((res != nullptr) != (x != nullptr), "bott_tc_f32: pass the block's identity or, folded, its input");
+    const size_t n2 = x ? in.numel() : out.numel();           // the second source: x in in's geometry, res in out's
+    const int K3 = x ? 128 : 64;
     DevBufs b{st, {}};
-    unsigned short *pi = b.get<unsigned short>(2 * in.numel()), *px = b.get<unsigned short>(2 * x.numel());
+    unsigned short *pi = b.get<unsigned short>(2 * in.numel()), *p2 = b.get<unsigned short>(2 * n2);
     unsigned short *po = b.get<unsigned short>(2 * out.numel());
-    unsigned short *pw2 = b.get<unsigned short>(2 * 64 * 576), *pw3 = b.get<unsigned short>((size_t)2 * out.C * 128);
+    unsigned short *pw2 = b.get<unsigned short>(2 * 64 * 576), *pw3 = b.get<unsigned short>((size_t)2 * out.C * K3);
     float *aux2 = b.get<float>(3 * 64 + 1), *aux3 = b.get<float>(3 * out.C + 1);
-    HN_CHECK(pi && px && po && pw2 && pw3 && aux2 && aux3, "bott_tc_fold: out of device memory");
+    HN_CHECK(pi && p2 && po && pw2 && pw3 && aux2 && aux3, "bott_tc_f32: out of device memory");
     HN_CUDA_OK(cudaMemsetAsync(po, 0xff, out.numel() * 4, st));
-    if (split_planes(in.p, pi, in.numel(), st) || split_planes(x.p, px, x.numel(), st)) return -1;
+    if (split_planes(in.p, pi, in.numel(), st) || split_planes(x ? x : res, p2, n2, st)) return -1;
     if (pack_weight_impl<true>(w2, pw2, scale2, shift2, aux2, aux2 + 3 * 64, 64, 64, 3, 3, st)) return -1;
-    if (pack_weight_impl<true>(w3, pw3, nullptr, shift3, aux3, aux3 + 3 * out.C, out.C, 128, 1, 1, st)) return -1;
-    if (bott_tc_planes(d2, pw2, aux2, d3, pw3, aux3, in, pi, out, po, nullptr, px, st)) return -1;
+    if (pack_weight_impl<true>(w3, pw3, scale3, shift3, aux3, aux3 + 3 * out.C, out.C, K3, 1, 1, st)) return -1;
+    if (bott_tc_planes(d2, pw2, aux2, d3, pw3, aux3, in, pi, out, po, x ? nullptr : p2, x ? p2 : nullptr, st)) return -1;
     return merge_planes(po, out.p, out.numel(), st);
 }
 

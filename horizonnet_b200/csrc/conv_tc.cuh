@@ -69,8 +69,8 @@ struct TcPlan {
     int pf;                                // gemm_tc_kernel: L2 prefetch distance in tile rounds, 0 = off
     int n_tiles, num_tiles, grid;          // tiles along Cout, all tiles, CTAs (persistent, min(num_tiles, sms))
 };
-// Reads HN_TC_DXR and HN_TC_GEMM; -1 (with hn_last_error set) for a shape conv_tc_supported rejects or a residual with fp32
-// output.  conv_tc_planes launches exactly this plan.
+// A function of the shapes and sms alone; -1 (with hn_last_error set) for a shape conv_tc_supported rejects or a residual
+// with fp32 output.  conv_tc_planes launches exactly this plan.
 int conv_tc_plan(const ConvDesc& d, const Act& in, const Act& out, bool out_f32, bool has_residual, int sms, TcPlan* p);
 // fp32 halo-NHWC in/out convenience wrapper (unit tests): splits, runs the plane kernel, merges the output planes, or with
 // out_f32 lets the kernel write fp32 directly (the epilogue of the LSTM projections and of the data gradient; no residual).
@@ -94,18 +94,18 @@ int conv_tc_fold_planes(const unsigned short* wq, const float* tc_aux, const Act
 int conv_tc_fold(const float* w, const float* shift, const Act& t2, const Act& x, int stride, const Act& out,
                  cudaStream_t st);
 // conv2 (3x3 s1, 64 -> 64) + BN + ReLU fused with conv3 (1x1, 64 -> C3) + BN + identity + ReLU of a layer1 bottleneck
-// (conv_tc.cu: bott_tc_kernel); bit-identical to running conv_tc_planes twice; HN_TC_FUSE=0 disables it.  With the
-// downsample folded in (res_planes null, x_planes the block input in `in`'s geometry, wq3 / aux3 the folded pack of
-// conv_tc_fold_planes) it is bit-identical to conv_tc_planes + conv_tc_fold_planes.
+// (conv_tc.cu: bott_tc_kernel).  With the downsample folded in (res_planes null, x_planes the block input in `in`'s
+// geometry, wq3 / aux3 the folded pack of conv_tc_fold_planes) conv3 has no residual.
 bool bott_tc_supported(const ConvDesc& d2, const ConvDesc& d3, const Act& in, const Act& out);
 int bott_tc_planes(const ConvDesc& d2, const unsigned short* wq2, const float* aux2, const ConvDesc& d3,
                    const unsigned short* wq3, const float* aux3, const Act& in, const unsigned short* in_planes, const Act& out,
                    unsigned short* out_planes, const unsigned short* res_planes, const unsigned short* x_planes,
                    cudaStream_t st);
-// fp32 convenience wrapper of the folded bott_tc_planes (unit tests): w2 OIHW [64][64][3][3] with BN scale2 / shift2,
-// w3 the folded fp32 weights [C3][128] with shift3; in / x / out fp32 halo-NHWC
-int bott_tc_fold(const float* w2, const float* scale2, const float* shift2, const float* w3, const float* shift3,
-                 const Act& in, const Act& x, const Act& out, cudaStream_t st);
+// fp32 convenience wrapper of bott_tc_planes (unit tests): w2 OIHW [64][64][3][3] with BN scale2 / shift2; in / out fp32
+// halo-NHWC.  Exactly one of res (the block's identity, out's geometry; w3 the conv3 weights [C3][64] with scale3 /
+// shift3) and x (the block input, in's geometry; w3 the folded weights [C3][128] with shift3, scale3 null).
+int bott_tc_f32(const float* w2, const float* scale2, const float* shift2, const float* w3, const float* scale3,
+                const float* shift3, const Act& in, const float* res, const float* x, const Act& out, cudaStream_t st);
 // 7x7 stride-2 stem on wgmma (conv_tc.cu: stem_tc_kernel): NCHW fp32 input -> fp32 halo-NHWC [B][256][514][64]
 // (interior columns only).  wq [2][64][224] / tc_aux [3*64+1] come from stem_tc_pack_weights (pad_scratch: 64*224 floats);
 // scratch: stem_tc_scratch_bytes(B) bytes of packed input planes.

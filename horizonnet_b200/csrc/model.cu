@@ -317,7 +317,7 @@ int refold_bn(hn_model* m, cudaStream_t st) {
 extern "C" {
 
 const char* hn_last_error(void) { return g_err.c_str(); }
-int hn_abi_version(void) { return 7; }
+int hn_abi_version(void) { return 8; }
 const char* hn_build_digest(void) { return HN_BUILD_DIGEST; }
 long long hn_kernel_launches(void) { return g_launches.load(); }
 
@@ -347,7 +347,6 @@ int hn_model_create_arch(int device, int max_batch, const char* backbone, int us
     m->device = device;
     m->max_batch = max_batch;
     m->use_rnn = use_rnn;
-    if (const char* e = getenv("HN_TC_STEM")) m->stem_tc_on = atoi(e);
     build_graph(m.get(), *arch);
     for (auto& s : m->slots)
         if (!s.ignored && m->alloc_t(&s.dev, (size_t)s.numel)) return -1;
@@ -476,8 +475,6 @@ int hn_model_set_option(hn_model* m, const char* name, int value) {
     HN_CHECK(m && name, "hn_model_set_option: NULL argument");
     if (std::strcmp(name, "tensor_cores") == 0) { m->use_tc = value; return 0; }
     if (std::strcmp(name, "profile") == 0) { m->profile = value; return 0; }
-    if (std::strcmp(name, "stem_tc") == 0) { m->stem_tc_on = value; return 0; }
-    if (std::strcmp(name, "fuse_bottleneck") == 0) { m->fuse_on = value; return 0; }
     if (std::strcmp(name, "fold_downsample") == 0) { m->fold_on = value; return 0; }
     return fail(std::string("hn_model_set_option: unknown option '") + name + "'");
 }
@@ -571,7 +568,7 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
     Act s0 = mk(m->S0, B, 256, 512, 64);
     {
         Scope sc(m, CLS_STEM, 2.0 * B * 256 * 512 * 64 * 147, st);
-        if (m->use_tc && m->stem_tc_on) {
+        if (m->use_tc) {
             // packed input planes live in X[0] (free until layer1): B * 8.6 MB of its B * 33.8 MB
             if (stem_tc(x, B, in_channels, m->stem_wq, m->stem_aux, m->stem.shift, reinterpret_cast<unsigned short*>(m->X[0]),
                         s0, st))
@@ -593,7 +590,7 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
             const hn_model::Block& blk = m->blocks[l][b];
             if (blk.kind == hn_model::BASIC) {
                 // conv1 3x3 (stride) + BN + ReLU; the downsample (block 0 of layers 2-4) as its own launch; conv2 3x3 + BN +
-                // identity + ReLU.  No fold / fused kernel for this block kind: the options change nothing here
+                // identity + ReLU.  No fold / fused kernel for this block kind: option fold_downsample changes nothing here
                 const int s = blk.c1.d.sh;
                 Act t1 = mk(m->T1, B, cur.H / s, cur.W / s, blk.c1.d.Cout);
                 Act y = mk(b == nb - 1 ? m->F[l] : m->X[b & 1], B, t1.H, t1.W, blk.c2.d.Cout);
@@ -623,7 +620,7 @@ static int forward_encoder(hn_model* m, const float* x, int B, int in_channels, 
                 idn = d.p;
             }
             const double conv3_k = blk.c3.d.Cin + (fold ? (double)blk.ds.d.Cin : 0.0);
-            if (m->use_tc && m->fuse_on && blk.c2.wq && blk.c3.wq && bott_tc_supported(blk.c2.d, blk.c3.d, t1, y) &&
+            if (m->use_tc && blk.c2.wq && blk.c3.wq && bott_tc_supported(blk.c2.d, blk.c3.d, t1, y) &&
                 (!fold || (cur.C == 64 && cur.H == t1.H && cur.W == t1.W))) {
                 // layer1: conv2 + conv3 in one kernel, the 64-channel intermediate stays in shared memory (conv_tc.cu)
                 const double flops = 2.0 * (double)B * Ho * Wo * (64.0 * 9 * 64 + (double)blk.c3.d.Cout * conv3_k);
@@ -1175,12 +1172,13 @@ int hn_conv_tc_fold(const float* t2, const float* x, int B, int H, int W, int Ci
     return conv_tc_fold(w, shift, ta, xa, stride, oa, (cudaStream_t)stream);
 }
 
-int hn_bott_tc_fold(const float* in, const float* x, int B, int H, int W, const float* w2, const float* scale2,
-                    const float* shift2, const float* w3, const float* shift3, int C3, float* out, void* stream) {
-    HN_CHECK(in && x && w2 && scale2 && shift2 && w3 && shift3 && out, "hn_bott_tc_fold: NULL argument");
-    HN_CHECK(B >= 1 && H >= 1 && W >= 1 && C3 >= 64, "hn_bott_tc_fold: bad geometry");
-    return bott_tc_fold(w2, scale2, shift2, w3, shift3, mk(const_cast<float*>(in), B, H, W, 64),
-                        mk(const_cast<float*>(x), B, H, W, 64), mk(out, B, H, W, C3), (cudaStream_t)stream);
+int hn_bott_tc(const float* in, const float* res, const float* x, int B, int H, int W, const float* w2, const float* scale2,
+               const float* shift2, const float* w3, const float* scale3, const float* shift3, int C3, float* out,
+               void* stream) {
+    HN_CHECK(in && w2 && scale2 && shift2 && w3 && shift3 && out && (!res || scale3), "hn_bott_tc: NULL argument");
+    HN_CHECK(B >= 1 && H >= 1 && W >= 1 && C3 >= 64, "hn_bott_tc: bad geometry");
+    return bott_tc_f32(w2, scale2, shift2, w3, res ? scale3 : nullptr, shift3, mk(const_cast<float*>(in), B, H, W, 64), res,
+                       x, mk(out, B, H, W, C3), (cudaStream_t)stream);
 }
 
 int hn_lstm_layer(const float* xproj, const float* whf, const float* whb, float* out, int T, int B, void* stream) {

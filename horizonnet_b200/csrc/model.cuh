@@ -111,8 +111,6 @@ struct hn_model {
     std::vector<std::string> bn_names;               // state_dict prefixes of the 69 BatchNorm2d modules, graph order
     unsigned short* stem_wq = nullptr;               // tensor-core stem: [2][64][224] fp16 planes (conv_tc.cu: stem_tc)
     float* stem_aux = nullptr;                       // 3*64 + 1 epilogue constants
-    int stem_tc_on = 1;                              // option "stem_tc" / HN_TC_STEM=0: fp32 CUDA-core stem inside the TC path
-    int fuse_on = 1;                                 // option "fuse_bottleneck": fused conv2+conv3 kernel for layer1 (bit-identical)
     int fold_on = 1;                                 // option "fold_downsample": block-0 downsample inside conv3 (eval, TC)
     std::shared_ptr<void> train_state;               // tape + gradient buffers of the training step (train_step.cu)
     bool bn_stale = false;     // running statistics moved (train forward) since the eval-mode constants were folded

@@ -177,7 +177,7 @@ int walk_forward(hn_model* m, TrainState* ts, const float* x, int B, int in_chan
         ts->w_max = std::max(ts->w_max, (size_t)64 * 3 * 49);
         if (run) {
             if (stem_input_nhwc(x, in_channels, ts->stem_in, B, st)) return -1;
-            if (m->use_tc && m->stem_tc_on) {
+            if (m->use_tc) {
                 if (tc_aux_update(ts->ones, ts->zeros, m->stem_aux + 3 * 64, ts->aux_tmp, 64, st)) return -1;
                 if (stem_tc(x, B, in_channels, m->stem_wq, ts->aux_tmp, ts->zeros, reinterpret_cast<unsigned short*>(m->X[0]),
                             u.z, st, false))

@@ -170,8 +170,6 @@ int hn_model_stage(hn_model* m, const char* stage, float* out_dev, long long cap
 
 /* Options: "tensor_cores" = 1 routes every conv / projection GEMM the wgmma kernel supports
  * through the split-fp16 tensor-core path (default), 0 = exact fp32 CUDA-core kernels everywhere;
- * "stem_tc" = 1 (default; env HN_TC_STEM) runs the 7x7 stem on wgmma when "tensor_cores" is on, 0 = fp32 CUDA-core stem;
- * "fuse_bottleneck" = 1 (default; env HN_TC_FUSE) runs conv2 + conv3 of the layer1 bottlenecks as one kernel (bit-identical results);
  * "fold_downsample" = 1 (default) runs the downsample of each layer's block 0 inside its conv3 in the eval forward on
  * the tensor cores (one GEMM over [t2 | x] with both BN scales folded into the weights, no identity tensor), 0 = a
  * launch of its own and conv3 with a residual;
@@ -270,7 +268,7 @@ int hn_conv2d_dgrad_tc(int B, int H, int W, int Cin, const float* w_oihw, const 
  * 0 conv_tc_kernel), BN, mode (0 GEMM rows, 1 conv rows), M (rows), tile columns, rows per tile, tiles per output row,
  * rowbox (1: conv-row tiles of several output rows, which one box per plane loads), box rows, box images, dx reuse,
  * parity (stride 2 along W), K chunks, chunks per accumulation segment, L2 prefetch distance, tiles along Cout, tiles,
- * CTAs.  Reads HN_TC_DXR and HN_TC_GEMM like the launch.  -1 for a shape the kernel does not take. */
+ * CTAs.  -1 for a shape the kernel does not take. */
 int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
                     int out_halo, int out_f32, int has_residual, int sms, int plan[18]);
 /* The same plan (same 18 fields) for the eval-mode conv3 of a bottleneck's block 0 with its downsample folded in:
@@ -281,11 +279,14 @@ int hn_conv_tc_fold_plan(int B, int H, int W, int Cin, int Cmid, int Cout, int s
  * columns in the geometry above, w the folded weights [Cout][Cmid + Cin], shift [Cout]. */
 int hn_conv_tc_fold(const float* t2, const float* x, int B, int H, int W, int Cin, int Cmid, int Cout, int stride,
                     const float* w, const float* shift, float* out, void* stream);
-/* The fused layer1.0 bottleneck kernel with the downsample folded in (unit tests): in = conv1 output and x = block input,
- * both [B][H][W][64] halo-1 NHWC fp32; w2 OIHW [64][64][3][3] with BN scale2 / shift2; w3 the folded conv3 weights
- * [C3][64 + 64] with shift3; out [B][H][W][C3]. */
-int hn_bott_tc_fold(const float* in, const float* x, int B, int H, int W, const float* w2, const float* scale2,
-                    const float* shift2, const float* w3, const float* shift3, int C3, float* out, void* stream);
+/* The fused layer1 bottleneck kernel, conv2 + conv3 (unit tests): in = conv1 output [B][H][W][64], out [B][H][W][C3],
+ * halo-1 NHWC fp32; w2 OIHW [64][64][3][3] with BN scale2 / shift2.  Exactly one of res and x is non-NULL:
+ * res = the block's identity [B][H][W][C3] (layer1.1, 1.2), w3 the conv3 weights OIHW [C3][64][1][1] with BN scale3 /
+ * shift3; or x = the block input [B][H][W][64] with the downsample folded in (layer1.0), w3 the folded conv3 weights
+ * [C3][64 + 64] with shift3 (scale3 is not read). */
+int hn_bott_tc(const float* in, const float* res, const float* x, int B, int H, int W, const float* w2, const float* scale2,
+               const float* shift2, const float* w3, const float* scale3, const float* shift3, int C3, float* out,
+               void* stream);
 int hn_bn_forward_backward(const float* z, int B, int H, int W, int C, const float* gamma, const float* beta,
                            float* running_mean, float* running_var, double factor, int train, int relu, const float* res,
                            float* y, const float* dy, float* dz, float* dres, float* dgamma, float* dbeta, float* bn_scratch,

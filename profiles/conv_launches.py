@@ -3,9 +3,8 @@
 The tensor-core convolution kernels (conv_tc_kernel, gemm_tc_kernel, bott_tc_kernel) run in a fixed order per forward:
 the units of tests/tc_cases.resnet50_rnn_convs (layer1's conv2 + conv3 fused into one bott_tc_kernel; with the model option
 fold_downsample, the default, each block-0 downsample inside its conv3), then the two LSTM input projections.  Each launch is listed with its plan (hn_conv_tc_plan), its algorithmic FLOPs and a model of the
-operand bytes it pulls from L2 into shared memory.  The HN_TC_* switches in the environment apply, so run one process
-per setting; with programmatic dependent launch on (the default) a kernel's duration includes the time it waits for
-its predecessor, HN_TC_PDL=0 gives the clean attribution.
+operand bytes it pulls from L2 into shared memory.  HN_TC_PDL applies: with programmatic dependent launch on (the
+default) a kernel's duration includes the time it waits for its predecessor, HN_TC_PDL=0 gives the clean attribution.
 
     python profiles/conv_launches.py --out table.json [--reps 5] [--fold-downsample 0]
 """

@@ -3,8 +3,8 @@
 
 No GPU: the plan of the two-source conv_tc_kernel launch (hn_conv_tc_fold_plan) covers the output once at every block-0
 shape of the model, and the committed per-launch table of the folded forward matches profiles/conv_launches.py.
--m gpu: the two-source conv_tc_kernel and bott_tc_kernel with its downsample chunk against fp64, elementwise, and the
-whole batch-32 forward with the option fold_downsample on and off."""
+-m gpu: the two-source conv_tc_kernel and bott_tc_kernel, with its downsample chunk and with an identity, against fp64,
+elementwise, and the whole batch-32 forward with the option fold_downsample on and off."""
 import ctypes
 import json
 import os
@@ -160,36 +160,66 @@ def test_fold_conv_vs_fp64(case):
     assert ratio <= 1.0, ratio
 
 
+# (name, conv3 variant, B, H, W): layer1.0 runs bott_tc_kernel with its downsample folded in, layer1.1 and 1.2 with the
+# block's identity as the residual
+BOTT = [('layer1.0_b1', 'fold', 1, 128, 256), ('layer1.0_b3', 'fold', 3, 128, 256), ('small', 'fold', 2, 4, 128),
+        ('layer1.1_b1', 'identity', 1, 128, 256), ('layer1.1_b3', 'identity', 3, 128, 256),
+        ('small_identity', 'identity', 2, 4, 128)]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize('case', [('layer1.0_b1', 1, 128, 256), ('small', 2, 4, 128)], ids=lambda c: c[0])
-def test_bott_fold_vs_fp64(case):
+@pytest.mark.parametrize('case', BOTT, ids=lambda c: c[0])
+def test_bott_tc_vs_fp64(case):
+    """hn_bott_tc, both variants of the fused layer1 conv2 + conv3 kernel, against fp64 elementwise."""
     import torch
     import gpu_utils as gu
-    name, B, H, W = case
+    name, variant, B, H, W = case
     C3, dev = 256, 'cuda:0'
     g = torch.Generator().manual_seed(17)
     t1 = torch.relu(torch.randn(B, 64, H, W, generator=g)).to(dev)
     w2 = (torch.randn(64, 64, 3, 3, generator=g) / 24.0).to(dev)
     s2, f2 = (torch.rand(64, generator=g) + 0.5).to(dev), (torch.randn(64, generator=g) * 0.1).to(dev)
-    x, _, w3, f3 = _gpu_inputs(g, B, H, W, 64, 64, C3, 1, dev)
+    if variant == 'fold':
+        x, _, w3, f3 = _gpu_inputs(g, B, H, W, 64, 64, C3, 1, dev)
+        s3 = res = None
+    else:
+        w3 = (torch.randn(C3, 64, generator=g) / 8.0).to(dev)
+        s3, f3 = (torch.rand(C3, generator=g) + 0.5).to(dev), (torch.randn(C3, generator=g) * 0.1).to(dev)
+        res = torch.randn(B, C3, H, W, generator=g).to(dev)
+        x = None
     buf, out, n = _run_out((B, H, W, C3), dev)
-    t1h, xh = gu.to_halo_nhwc(t1, 1), gu.to_halo_nhwc(x, 1)
-    rc = _lib.lib().hn_bott_tc_fold(t1h.data_ptr(), xh.data_ptr(), B, H, W, w2.data_ptr(), s2.data_ptr(), f2.data_ptr(),
-                                    w3.data_ptr(), f3.data_ptr(), C3, out.data_ptr(), torch.cuda.current_stream().cuda_stream)
-    _lib.check(rc, 'hn_bott_tc_fold')
+    t1h = gu.to_halo_nhwc(t1, 1)
+    resh, xh = (gu.to_halo_nhwc(t, 1) if t is not None else None for t in (res, x))
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    rc = _lib.lib().hn_bott_tc(t1h.data_ptr(), ptr(resh), ptr(xh), B, H, W, w2.data_ptr(), s2.data_ptr(), f2.data_ptr(),
+                               w3.data_ptr(), ptr(s3), f3.data_ptr(), C3, out.data_ptr(),
+                               torch.cuda.current_stream().cuda_stream)
+    _lib.check(rc, 'hn_bott_tc')
     torch.cuda.synchronize()
     _check_out(buf, out, n)
-    # conv2 in fp64 with its own error bound, which conv3 carries through |W3'|
+    # conv2 in fp64 with its own error bound, which conv3 carries through |W3'| (its weights on t2 in output units)
     t2 = gu.conv2d_reference(t1.double(), w2.double(), s2, f2, (1, 1), 1, 1, True)
     acc2 = gu._conv_abs(t1.double().abs(), w2.double().abs(), (1, 1), 1, 1)
     ones2 = gu._conv_abs(torch.ones_like(t1[:1].double()), w2.double().abs(), (1, 1), 1, 1)
     b2 = s2.double().abs().view(1, -1, 1, 1) * (gu.C_OPERAND * gu.EPS21 * acc2 + gu.EPS20 * ones2) + \
         gu.EPS21 * t2.abs() + gu.EPS21
-    ref, acc, ones = _fold_reference(x, t2, w3, f3, 64, 1)
-    carried = torch.einsum('bchw,nc->bnhw', b2, w3.double()[:, :64].abs())
-    bound = gu.C_OPERAND * gu.EPS21 * acc + gu.EPS20 * ones + gu.EPS21 * ref.abs() + gu.EPS21 + carried
+    if variant == 'fold':
+        ref, acc, ones = _fold_reference(x, t2, w3, f3, 64, 1)
+        w3t = w3.double()[:, :64]
+        bound = gu.C_OPERAND * gu.EPS21 * acc + gu.EPS20 * ones
+    else:
+        w4 = w3.double().view(C3, 64, 1, 1)
+        ref = gu.conv2d_reference(t2, w4, s3, f3, (1, 1), 0, 0, True, res.double())
+        acc = gu._conv_abs(t2.abs(), w4.abs(), (1, 1), 0, 0)
+        ones = gu._conv_abs(torch.ones_like(t2[:1]), w4.abs(), (1, 1), 0, 0)
+        w3t = s3.double().view(-1, 1) * w3.double()
+        # accumulator terms through the BN scale, and the identity's own plane rounding (gpu_utils.run_tc_case)
+        bound = s3.double().abs().view(1, -1, 1, 1) * (gu.C_OPERAND * gu.EPS21 * acc + gu.EPS20 * ones) + \
+            gu.EPS21 * (res.double().abs() + 1.0)
+    carried = torch.einsum('bchw,nc->bnhw', b2, w3t.abs())
+    bound = bound + gu.EPS21 * ref.abs() + gu.EPS21 + carried
     ratio = gu._worst_ratio(gu.from_halo_nhwc(out, 1).double() - ref, bound)
-    gu.record('tc_errors.jsonl', {'test': 'bott_fold', 'case': name, 'ratio': ratio})
+    gu.record('tc_errors.jsonl', {'test': 'bott_' + variant, 'case': name, 'ratio': ratio})
     assert ratio <= 1.0, ratio
 
 

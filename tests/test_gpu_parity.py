@@ -87,8 +87,7 @@ def test_lstm_layer_vs_oracle(T, B):
     """One bidirectional layer against an fp64 recurrence of the same input projection, up to the model's T = 256;
     B = 7 leaves part of an 8-column group empty, and B = 32 and 40 take two column groups per cluster on a card that
     co-schedules fewer than 8 of the 16-CTA clusters."""
-    from tc_runner import lstm_error
-    err = lstm_error(T, B, DEV)
+    err = gu.lstm_error(T, B, DEV)
     gu.record('lstm_errors.jsonl', {'T': T, 'B': B, 'err': err})
     assert err < 2e-6, err
 
@@ -237,33 +236,11 @@ def test_forward_on_does_not_switch_the_current_device():
     assert _lib.lib().hn_build_digest().decode() == __import__('horizonnet_b200.build', fromlist=['x']).source_digest()
 
 
-def test_fused_bottleneck_kernel_is_bitwise_equal_to_the_unfused_convs():
-    """bott_tc_kernel (layer1: conv2 + BN + ReLU -> shared memory -> conv3 + BN + identity + ReLU in one kernel) performs
-    the same products in the same order with the same accumulator structure and epilogue arithmetic as conv_tc_kernel<64> +
-    gemm_tc_kernel, so layer1 and the final outputs must not change by a single bit (B = 3: odd tile counts per CTA)."""
-    sd = synthetic_state_dict(8, 'random')
-    net = _net(sd, True)
-    x = synthetic_panoramas(3, seed=71).to(DEV)
-    got = {}
-    with torch.no_grad():
-        net(x)                                  # creates the handle
-        for mode in (1, 0):
-            net.set_option('fuse_bottleneck', mode)
-            bon, cor = net(x)
-            got[mode] = (bon.clone(), cor.clone(), net.debug_stage('layer1').clone())
-        net.set_option('fuse_bottleneck', 1)
-    net.check()
-    assert torch.isfinite(got[1][2]).all()
-    assert torch.equal(got[1][2], got[0][2]), (got[1][2] - got[0][2]).abs().max().item()
-    assert torch.equal(got[1][0], got[0][0]) and torch.equal(got[1][1], got[0][1])
-
-
-def test_tensor_core_stem_vs_oracle_and_fp32_stem():
-    """stem_tc_kernel (7x7 s2 conv as an implicit GEMM over packed pixel pairs) against the oracle's stem in fp64
-    and against the exact fp32 CUDA-core stem_kernel it replaces on the tensor-core path."""
+def test_tensor_core_stem_and_fp32_stem_vs_oracle():
+    """stem_tc_kernel (7x7 s2 conv as an implicit GEMM over packed pixel pairs), which every tensor-core forward runs,
+    and the exact fp32 CUDA-core stem_kernel of use_tensor_cores(False), each against the oracle's stem in fp64."""
     import torch.nn.functional as F
     sd = synthetic_state_dict(5, 'random')
-    net = _net(sd, True)
     x = synthetic_panoramas(2, seed=33, channels=4)
     e = 'feature_extractor.encoder.'
     sd64 = {k: v.double() for k, v in sd.items() if k.startswith(e + 'conv1') or k.startswith(e + 'bn1.')}
@@ -271,21 +248,16 @@ def test_tensor_core_stem_vs_oracle_and_fp32_stem():
         torch.tensor(horizonnet_ref.X_STD).double().view(1, 3, 1, 1)
     ref = F.relu(horizonnet_ref._bn(horizonnet_ref._circ_conv(xn, sd64[e + 'conv1.1.weight'], None, 2, 3, 3), sd64, e + 'bn1'))
     scale = ref.abs().max().item()
-    got = {}
-    for mode in (1, 0):
+    for tensor_cores in (True, False):
+        net = _net(sd, tensor_cores)
         with torch.no_grad():
-            net(x.to(DEV))                      # creates the handle on first use
-            net.set_option('stem_tc', mode)
-            bon, cor = net(x.to(DEV))
+            net(x.to(DEV))
         net.check()
         stem = net.debug_stage('stem').cpu()
         assert tuple(stem.shape) == (2, 64, 256, 512)
         err = (stem.double() - ref).abs().max().item()
         # split-precision products carry 22 significant bits per operand (measured 5.2e-6 at scale 3.3); fp32 FMA: 1.9e-6
-        assert err <= (4e-6 if mode else 1e-6) * scale + 1e-6, (mode, err, scale)
-        got[mode] = (stem, bon.cpu(), cor.cpu())
-    assert (got[1][1] - got[0][1]).abs().max().item() < 2e-5
-    assert (got[1][2] - got[0][2]).abs().max().item() < 2e-5
+        assert err <= (4e-6 if tensor_cores else 1e-6) * scale + 1e-6, (tensor_cores, err, scale)
 
 
 def test_forward_host_equals_device_forward():

@@ -1,30 +1,20 @@
 """HorizonNet('resnet18', use_rnn): the torchvision BasicBlock encoder with a 256-wide feature sequence, both heads, through
 every layer: spec, synthetic weights, oracle, module surface (CPU) and the library's eval forward, entry points, narrow
 height-reduction kernel, 3x3 residual launches, train-mode forward and training step (GPU).  Fixtures: tests/golden/*_r18*
-(make_golden_r18.py); checker: oracle/horizonnet_r18_ref.py (with horizonnet_ref.TrainMode for train mode).
-
-Run as a script (``python tests/test_resnet18.py dxr``) it prints the 3x3 residual cases as JSON lines: the dx-reuse switch
-HN_TC_DXR is read once per process, so the switched-off path needs a fresh one."""
+(make_golden_r18.py); checker: oracle/horizonnet_r18_ref.py (with horizonnet_ref.TrainMode for train mode)."""
 import json
 import os
-import subprocess
-import sys
 from collections import OrderedDict
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-if __name__ == '__main__':
-    sys.path.insert(0, os.path.dirname(HERE))
-    sys.path.insert(0, HERE)
+import numpy as np
+import pytest
+import torch
+import torch.nn.functional as F
 
-import numpy as np                                                   # noqa: E402
-import pytest                                                        # noqa: E402
-import torch                                                         # noqa: E402
-import torch.nn.functional as F                                      # noqa: E402
-
-from horizonnet_b200._spec import state_dict_spec, HEAD_BIAS, c_last  # noqa: E402
-from horizonnet_b200.model import HorizonNet                         # noqa: E402
-from horizonnet_b200.weights import synthetic_state_dict, synthetic_panoramas   # noqa: E402
-from oracle import horizonnet_ref, horizonnet_r18_ref as r18         # noqa: E402
+from horizonnet_b200._spec import state_dict_spec, HEAD_BIAS, c_last
+from horizonnet_b200.model import HorizonNet
+from horizonnet_b200.weights import synthetic_state_dict, synthetic_panoramas
+from oracle import horizonnet_ref, horizonnet_r18_ref as r18
 
 DEV = 'cuda:0'
 N_PARAMS = {True: 142, False: 128}
@@ -375,27 +365,16 @@ def test_narrow_height_reduction_kernel_vs_fp64(_built, name, Ci, Co, H, W, B):
                                 out.data_ptr(), Co, 3, 3, 2, 1, 1, 1, 1, out.data_ptr(), 1, 3, None) != 0
 
 
-def _run_residual_cases():
+@pytest.mark.gpu
+def test_residual_3x3_launches_vs_fp64_and_their_dx_reuse_plan(_built):
+    """conv2 of every BasicBlock layer against fp64: layers 1 and 2 (W >= 128) run with dx reuse, layers 3 and 4
+    without."""
     import gpu_utils as gu
     from tc_cases import plan
     for c in residual_cases():
-        print(json.dumps({'name': c['name'], 'ratio': gu.run_tc_case(c), 'plan': plan(c, gu.device_sms())}), flush=True)
-
-
-@pytest.mark.gpu
-def test_residual_3x3_launches_vs_fp64_with_dx_reuse_on_and_off(_built):
-    runs = {}
-    for env in ('1', '0'):
-        e = dict(os.environ, HN_TC_DXR=env)
-        p = subprocess.run([sys.executable, os.path.abspath(__file__), 'dxr'], env=e, capture_output=True, text=True,
-                           timeout=900)
-        assert p.returncode == 0, (env, p.stdout[-2000:], p.stderr[-4000:])
-        runs[env] = {r['name']: r for r in (json.loads(l) for l in p.stdout.splitlines() if l.startswith('{'))}
-    assert len(runs['1']) == len(runs['0']) == len(residual_cases())
-    for c in residual_cases():
-        on, off = runs['1'][c['name']], runs['0'][c['name']]
-        assert on['ratio'] <= 1.0 and off['ratio'] <= 1.0, (c['name'], on['ratio'], off['ratio'])
-        assert on['plan']['dxr'] == (1 if c['W'] >= 128 else 0) and off['plan']['dxr'] == 0, c['name']
+        ratio = gu.run_tc_case(c)
+        assert ratio <= 1.0, (c['name'], ratio)
+        assert plan(c, gu.device_sms())['dxr'] == (1 if c['W'] >= 128 else 0), c['name']
 
 
 @pytest.mark.gpu
@@ -474,10 +453,3 @@ def test_resnet18_training_step_gradients_match_the_golden_backward(_built, gold
     assert worst[0][0] < 5e-3, worst[:8]
     head = [e for e in worst if e[1].startswith(('linear', 'bi_rnn.weight_ih_l0'))]
     assert head[0][0] < 5e-3, head
-
-
-if __name__ == '__main__':
-    assert sys.argv[1:] == ['dxr'], sys.argv
-    import __graft_entry__ as entry
-    entry.build()
-    _run_residual_cases()

@@ -16,7 +16,6 @@ from horizonnet_b200 import _lib
 from horizonnet_b200.model import HorizonNet
 from horizonnet_b200.weights import synthetic_state_dict, synthetic_panoramas
 import gpu_utils as gu
-from tc_runner import lstm_reference
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -68,7 +67,7 @@ def test_lstm_two_groups_per_cluster_match_one(B):
     parts = [_lstm(xd[:, c:c + 8].contiguous(), w0, w1) for c in range(0, B, 8)]
     torch.cuda.synchronize()
     assert torch.equal(out, torch.cat(parts, dim=1))
-    err = (out.cpu().double() - lstm_reference(xproj, whh)).abs().max().item()
+    err = (out.cpu().double() - gu.lstm_reference(xproj, whh)).abs().max().item()
     assert err < 2e-6, err
 
 

@@ -4,16 +4,9 @@
   the LSTM projections, of the training step's raw pass and of its data gradients), with the error bound of
   gpu_utils.run_tc_case: NaN-filled output that must be written everywhere, circular halo columns, a canary behind the
   output;
-* the tensor-core data gradient of the training step (hn_conv2d_dgrad_tc) against torch.autograd in fp64;
-* the HN_TC_* switches that select other code paths, each in a fresh process (tests/tc_runner.py), since the library reads
-  them once per process.
+* the tensor-core data gradient of the training step (hn_conv2d_dgrad_tc) against torch.autograd in fp64.
 Worst err / bound per case and variant key go to $HN_TEST_RECORD_DIR/tc_errors.jsonl when that variable is set
 (gpu_utils.record)."""
-import json
-import os
-import subprocess
-import sys
-
 import pytest
 import torch
 
@@ -23,7 +16,6 @@ import gpu_utils as gu
 import tc_cases
 
 pytestmark = pytest.mark.gpu
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope='module', autouse=True)
@@ -87,31 +79,3 @@ def test_dgrad_tc_rejects_shapes_the_kernel_does_not_take():
     assert _lib.lib().hn_conv2d_dgrad_tc(1, 4, 16, 64, z.data_ptr(), z.data_ptr(), 32, 3, 3, 2, 1, 1, 1, z.data_ptr(),
                                          None) != 0
     assert b'not supported' in _lib.lib().hn_last_error()
-
-
-def _run(kind, names, env):
-    e = dict(os.environ)
-    e.update(env)
-    p = subprocess.run([sys.executable, os.path.join(HERE, 'tc_runner.py'), kind] + list(names), env=e,
-                       capture_output=True, text=True, timeout=900)
-    assert p.returncode == 0, (env, p.stdout[-2000:], p.stderr[-4000:])
-    return {r['name']: r for r in (json.loads(l) for l in p.stdout.splitlines() if l.startswith('{'))}
-
-
-# switch -> (cases whose plan it changes, plan field it turns off)
-SWITCHES = {
-    'HN_TC_DXR': (['dxr_bn64_w2', 'dxr_bn128_w1', 'f32_3x3'], 'dxr'),
-    'HN_TC_GEMM': (['gemm_k64_res_pf', 'gemm_k256', 'gemm_cout1024'], 'gemm_kernel'),
-}
-
-
-def test_switched_off_paths_stay_inside_the_bound():
-    names = sorted({n for v in SWITCHES.values() for n in v[0]})
-    base = _run('conv', names, {})
-    for sw, (cases, field) in SWITCHES.items():
-        got = _run('conv', cases, {sw: '0'})
-        for n in cases:
-            r = got[n]
-            gu.record('tc_errors.jsonl', {'test': 'switch', 'switch': sw, 'case': n, 'ratio': r['ratio']})
-            assert r['ratio'] <= 1.0, (sw, n, r['ratio'])
-            assert base[n]['plan'][field] and not r['plan'][field], (sw, n)           # the switch took the other path
