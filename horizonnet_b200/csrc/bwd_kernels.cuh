@@ -17,11 +17,8 @@ int dilate_for_dgrad(const Act& dz, const Act& out, int sh, int sw, cudaStream_t
 // dW[Cout][kh][kw][Cin] (zeroed here, then accumulated); in = the conv's forward input, dz = d(raw conv output)
 int conv_wgrad_f32(const ConvDesc& d, const Act& in, const Act& dz, float* dw_ohwi, cudaStream_t st);
 // The same product on tensor-core (wgrad_tc.cu) from the split planes of the input and of dz (split_planes_pow2; dz_absmax =
-// the float it left behind): Cin, Cout multiples of 64, halo 0 or 1, strides 1 or 2.  HN_WGRAD_TC=0/1 overrides the default.
-#ifndef HN_WGRAD_TC_DEFAULT
-#define HN_WGRAD_TC_DEFAULT 1
-#endif
-bool wgrad_tc_on();
+// the float it left behind): Cin, Cout multiples of 64, halo 0 or 1, strides 1 or 2.  The training step's wgrad runs it
+// wherever option tensor_cores is on and conv_wgrad_tc_supported takes the shape, and conv_wgrad_f32 everywhere else.
 bool conv_wgrad_tc_supported(const ConvDesc& d, const Act& in, const Act& dz);
 int conv_wgrad_tc_plan(const ConvDesc& d, const Act& in, const Act& dz, int sms, int plan[10]);      // host-only (tests)
 int conv_wgrad_tc(const ConvDesc& d, const Act& in, const unsigned short* in_planes, const Act& dz,

@@ -7,10 +7,10 @@
 // Every convolution output z (pre-BN) and every activation y is kept in fp32 on a tape; one gradient buffer mirrors
 // every y.  With the model option tensor_cores (default) the forward convolutions and their data gradients run on the
 // tensor-core conv kernel (conv_tc.cu: fp16 hi/lo operand planes, fp32 result; a data gradient is the same kernel on the
-// zero-dilated dz with flipped weights); the weight gradients of the convolutions with Cin, Cout multiples of 64 can run
-// on the tensor-core weight-gradient kernel (wgrad_tc.cu, HN_WGRAD_TC); the other weight gradients, BatchNorm, LSTM BPTT and
-// the rest are fp32 CUDA-core kernels (bwd_kernels.cu).  tensor_cores = 0: conv_f32.cu everywhere.  Not built: loss
-// scaling, gradient all-reduce overlapped with the backward.
+// zero-dilated dz with flipped weights); every weight gradient goes through wgrad, which runs the tensor-core
+// weight-gradient kernel (wgrad_tc.cu) wherever it takes the shape (Cin, Cout multiples of 64); the other weight
+// gradients, BatchNorm, LSTM BPTT and the rest are fp32 CUDA-core kernels (bwd_kernels.cu).  tensor_cores = 0: conv_f32.cu
+// and conv_wgrad_f32 everywhere.  Not built: loss scaling, gradient all-reduce overlapped with the backward.
 #include <cstdlib>
 #include <cstring>
 #include <memory>
@@ -62,6 +62,8 @@ struct TrainState {
     // tensor-core variant of the step (hn_model option tensor_cores): fp16 hi/lo planes of every activation (same
     // offsets as yarena), of the current dz / dilated dz, an fp32 landing buffer for data gradients, epilogue constants
     float *parena = nullptr, *pl_scratch = nullptr, *pl2_scratch = nullptr, *dtmp = nullptr, *aux_tmp = nullptr;
+    // absmax of the dz planes in pl_scratch (i = 0) / pl2_scratch (1), behind aux_tmp's epilogue constants and weight absmax
+    float* dz_amax(int i) const { return aux_tmp + 3 * 4096 + 1 + i; }
     size_t din_max = 0;
     float *ones = nullptr, *zeros = nullptr;
     double* sums = nullptr;
@@ -380,6 +382,25 @@ int dgrad_tc(const ConvDesc& d, const float* w_oihw, const Act& dz, const Act& d
     return add_inplace(din.p, g.landing.p, din.numel(), st);
 }
 
+// ---- weight gradient: the tensor-core kernel on fp16 hi/lo planes of the input and of dz (dz scaled by a power of two,
+// see split_planes_pow2), or the fp32 CUDA-core kernel
+struct WgradPlanes {
+    unsigned short* in;       // 2 x in.numel()
+    unsigned short* dz;       // 2 x dz.numel()
+    float* dz_amax;           // 1: absmax of dz, the scale of its planes
+    bool in_split, dz_split;  // the buffer already holds those planes; wgrad sets both when it ran on the tensor cores
+};
+
+// dw_ohwi = dW[Cout][kh][kw][Cin], on wgrad_tc_kernel when tc is set and conv_wgrad_tc_supported takes the shape (the stem
+// does not: Cin = 3, halo 3), otherwise on conv_wgrad_f32
+int wgrad(const ConvDesc& d, const Act& in, const Act& dz, bool tc, WgradPlanes& p, float* dw_ohwi, cudaStream_t st) {
+    if (!tc || !conv_wgrad_tc_supported(d, in, dz)) return conv_wgrad_f32(d, in, dz, dw_ohwi, st);
+    if (!p.in_split && split_planes(in.p, p.in, in.numel(), st)) return -1;
+    if (!p.dz_split && split_planes_pow2(dz.p, p.dz, dz.numel(), p.dz_amax, st)) return -1;
+    p.in_split = p.dz_split = true;
+    return conv_wgrad_tc(d, in, p.in, dz, p.dz, p.dz_amax, dw_ohwi, st);
+}
+
 #define GRAD(key) grad_buffer(m, ts, key)
 // MLP head (model.py:238-243, :270-275): from the scatter back to d(sequence), left in *dseq
 int mlp_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dcor, cudaStream_t st, float** dseq) {
@@ -401,13 +422,9 @@ int mlp_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dc
     const Act xa = mk(ts->seq, 1, 1, (int)rows, CL, 0);
     const Act dg = mk(dh, 1, 1, (int)rows, 512, 0);
     ConvDesc wi; wi.Cin = CL; wi.Cout = 512;
-    if (m->use_tc && wgrad_tc_on() && conv_wgrad_tc_supported(wi, xa, dg)) {
-        unsigned short* xpl = reinterpret_cast<unsigned short*>(ts->pl_scratch);
-        unsigned short* gpl = reinterpret_cast<unsigned short*>(ts->pl_scratch + rows * 1024);
-        float* gmax = ts->aux_tmp + 3 * 4096 + 1;
-        if (split_planes(ts->seq, xpl, rows * CL, st) || split_planes_pow2(dh, gpl, nh, gmax, st)) return -1;
-        if (conv_wgrad_tc(wi, xa, xpl, dg, gpl, gmax, GRAD("linear.0.weight"), st)) return -1;
-    } else if (conv_wgrad_f32(wi, xa, dg, GRAD("linear.0.weight"), st)) return -1;
+    unsigned short* pl = reinterpret_cast<unsigned short*>(ts->pl_scratch);      // per row: planes of SEQ (<= 1024), of dH
+    WgradPlanes p = {pl, pl + rows * 2048, ts->dz_amax(0), false, false};
+    if (wgrad(wi, xa, dg, m->use_tc, p, GRAD("linear.0.weight"), st)) return -1;
     // d(sequence) = dH W1      (W1 [512][c_last] is already conv_f32's [K][N] packing)
     ConvDesc di; di.Cin = 512; di.Cout = CL; di.w = m->T("linear.0.weight"); di.scale = ts->ones; di.shift = ts->zeros;
     if (conv_f32(di, dg, mk(ts->db, 1, 1, (int)rows, CL, 0), nullptr, st)) return -1;
@@ -455,27 +472,18 @@ int rnn_backward(hn_model* m, TrainState* ts, const float* dbon, const float* dc
         const Act xa = mk(const_cast<float*>(X), 1, 1, (int)rows, K, 0);
         ConvDesc wi; wi.Cin = K; wi.Cout = 2048;
         ConvDesc wh; wh.Cin = 512; wh.Cout = 2048;
-        const bool lstm_wg_tc = m->use_tc && wgrad_tc_on() &&
-                                conv_wgrad_tc_supported(wi, xa, mk(ts->dgates, 1, 1, (int)rows, 2048, 0)) &&
-                                conv_wgrad_tc_supported(wh, mk(ts->hprev, 1, 1, (int)rows, 512, 0), mk(ts->dgates, 1, 1, (int)rows, 2048, 0));
-        // tensor-core kernel: planes of X, of this direction's H_prev and dG in the plane scratch (3584 floats' worth per row)
-        unsigned short* xpl = reinterpret_cast<unsigned short*>(ts->pl_scratch);
-        unsigned short* hpl = reinterpret_cast<unsigned short*>(ts->pl_scratch + rows * 1024);
-        unsigned short* gpl = reinterpret_cast<unsigned short*>(ts->pl_scratch + rows * 1536);
-        float* gmax = ts->aux_tmp + 3 * 4096 + 1;
-        if (lstm_wg_tc && split_planes(X, xpl, rows * K, st)) return -1;
+        // tensor cores: planes per row of X (<= 1024 wide), this direction's H_prev and dG; X is split once per layer,
+        // H_prev and dG once per direction, and W_ih and W_hh share the planes of dG
+        unsigned short* pl = reinterpret_cast<unsigned short*>(ts->pl_scratch);
+        WgradPlanes px = {pl, pl + rows * 3072, ts->dz_amax(0), false, false};
         for (int dir = 0; dir < 2; ++dir) {
             const std::string sfx = l + (dir ? "_reverse" : "");
             Act dg = mk(ts->dgates + dir * rows * 2048, 1, 1, (int)rows, 2048, 0);
             const Act ha = mk(ts->hprev + dir * rows * 512, 1, 1, (int)rows, 512, 0);
-            if (lstm_wg_tc) {
-                if (split_planes(ha.p, hpl, rows * 512, st) || split_planes_pow2(dg.p, gpl, rows * 2048, gmax, st)) return -1;
-                if (conv_wgrad_tc(wi, xa, xpl, dg, gpl, gmax, GRAD("bi_rnn.weight_ih" + sfx), st)) return -1;
-                if (conv_wgrad_tc(wh, ha, hpl, dg, gpl, gmax, GRAD("bi_rnn.weight_hh" + sfx), st)) return -1;
-            } else {
-                if (conv_wgrad_f32(wi, xa, dg, GRAD("bi_rnn.weight_ih" + sfx), st)) return -1;
-                if (conv_wgrad_f32(wh, ha, dg, GRAD("bi_rnn.weight_hh" + sfx), st)) return -1;
-            }
+            px.dz_split = false;
+            if (wgrad(wi, xa, dg, m->use_tc, px, GRAD("bi_rnn.weight_ih" + sfx), st)) return -1;
+            WgradPlanes ph = {pl + rows * 2048, px.dz, px.dz_amax, false, px.dz_split};
+            if (wgrad(wh, ha, dg, m->use_tc, ph, GRAD("bi_rnn.weight_hh" + sfx), st)) return -1;
             float* bi = GRAD("bi_rnn.bias_ih" + sfx);
             if (col_sum(dg.p, rows, 2048, bi, st)) return -1;
             HN_CUDA_OK(cudaMemcpyAsync(GRAD("bi_rnn.bias_hh" + sfx), bi, 2048 * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -530,19 +538,13 @@ int walk_backward(hn_model* m, TrainState* ts, const float* dbon, const float* d
                    GRAD(c.bnprefix + ".bias"), c.biaskey.empty() ? nullptr : GRAD(c.biaskey), st))
             return -1;
         MARK(1);
-        // planes of dz (gradients are tiny: power-of-two scaling around the split, see split_planes_pow2); a stride-1 unit
-        // shares them between its weight gradient and its data gradient
+        // the input's planes are on the tape; a stride-1 unit's data gradient reuses the planes of dz split here (a strided
+        // unit's splits its dilated dz, so these go to pl2_scratch)
         unsigned short* sp = reinterpret_cast<unsigned short*>(ts->pl_scratch);
-        float* amax = ts->aux_tmp + 3 * 4096 + 1;
         const bool strided = u.d.sh != 1 || u.d.sw != 1;
-        bool sp_is_dz = false;
-        if (m->use_tc && !u.is_stem && wgrad_tc_on() && conv_wgrad_tc_supported(u.d, u.in, dz)) {
-            unsigned short* zp = strided ? reinterpret_cast<unsigned short*>(ts->pl2_scratch) : sp;
-            float* zmax = strided ? amax + 1 : amax;
-            if (split_planes_pow2(dz.p, zp, dz.numel(), zmax, st)) return -1;
-            if (conv_wgrad_tc(u.d, u.in, planes_of(ts, u.in), dz, zp, zmax, ts->dw_scratch, st)) return -1;
-            sp_is_dz = !strided;
-        } else if (conv_wgrad_f32(u.d, u.in, dz, ts->dw_scratch, st)) return -1;
+        WgradPlanes wp = {planes_of(ts, u.in), strided ? reinterpret_cast<unsigned short*>(ts->pl2_scratch) : sp,
+                          ts->dz_amax(strided), true, false};
+        if (wgrad(u.d, u.in, dz, m->use_tc, wp, ts->dw_scratch, st)) return -1;
         if (ohwi_to_oihw(ts->dw_scratch, GRAD(c.wkey), u.d.Cout, u.d.Cin, u.d.kh, u.d.kw, st)) return -1;
         MARK(2);
         if (u.is_stem) { MARK(3); continue; }                      // the image needs no gradient
@@ -550,8 +552,8 @@ int walk_backward(hn_model* m, TrainState* ts, const float* dbon, const float* d
         if (m->use_tc && dgrad_tc_supported(u.d, dz, din)) {
             // tensor cores: planes of the (dilated) dz, flipped weights packed as planes, fp32 result added to the gradient
             const DgradScratch s = {ts->dil_scratch, ts->dtmp, sp, ts->dw_scratch,
-                                    reinterpret_cast<unsigned short*>(ts->wd_scratch), ts->aux_tmp, amax, ts->zeros};
-            if (dgrad_tc(u.d, m->T(c.wkey), dz, din, s, sp_is_dz, st)) return -1;
+                                    reinterpret_cast<unsigned short*>(ts->wd_scratch), ts->aux_tmp, ts->dz_amax(0), ts->zeros};
+            if (dgrad_tc(u.d, m->T(c.wkey), dz, din, s, !strided && wp.dz_split, st)) return -1;
         } else if (u.d.Cout % 16 != 0) {
             // resnet18's ghc0.3 (16 -> 8): conv_dgrad_f32 takes Cout in steps of 16, so dz and the weights get zero channels
             // up to 16 (OIHW: the extra output channels are zero rows after the real ones).  dw_scratch and pl2_scratch are
@@ -708,7 +710,8 @@ int hn_conv2d_backward(const float* in, int B, int H, int W, int Cin, int in_hal
     const size_t nw = (size_t)Cout * Cin * kh * kw;
     float *tmp = nullptr, *ones = nullptr, *dil = nullptr;
     HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&tmp), nw * sizeof(float), st));
-    int rc = conv_wgrad_f32(d, a, z, tmp, st);
+    WgradPlanes none = {};
+    int rc = wgrad(d, a, z, false, none, tmp, st);
     if (!rc) rc = ohwi_to_oihw(tmp, dw_oihw, Cout, Cin, kh, kw, st);
     if (!rc && din) {
         Act di = mk(din, B, H, W, Cin, 1);
@@ -736,11 +739,11 @@ int hn_wgrad_tc_plan(int B, int H, int W, int Cin, int Cout, int kh, int kw, int
     return conv_wgrad_tc_plan(d, a, z, sms, plan);
 }
 
-// 1 when the training step routes the weight gradients the tensor-core kernel supports through it (HN_WGRAD_TC or the built-in default)
-int hn_wgrad_tc_enabled(void) { return wgrad_tc_on() ? 1 : 0; }
+// 1: the training step runs its weight gradients on the tensor-core kernel wherever option tensor_cores is on and the shape fits
+int hn_wgrad_tc_enabled(void) { return 1; }
 
-// Weight gradient on the tensor-core kernel (wgrad_tc.cu) from fp32 halo-1 NHWC tensors: splits both operands into planes
-// (the training step has them already), runs conv_wgrad_tc, returns dW in OIHW.  Fails for shapes the kernel does not take.
+// Weight gradient on the tensor-core kernel (wgrad_tc.cu) from fp32 halo-1 NHWC tensors through the training step's own
+// wgrad, which splits both operands into planes here; returns dW in OIHW.  Fails for shapes the kernel does not take.
 int hn_conv2d_wgrad_tc(const float* in, int B, int H, int W, int Cin, const float* dz, int Cout, int kh, int kw, int sh,
                        int sw, int ph, int pw, float* dw_oihw, void* stream) {
     HN_CHECK(in && dz && dw_oihw, "hn_conv2d_wgrad_tc: NULL argument");
@@ -758,8 +761,8 @@ int hn_conv2d_wgrad_tc(const float* in, int B, int H, int W, int Cin, const floa
     HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&amax), sizeof(float), st));
     HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&ap), a.numel() * 2 * sizeof(unsigned short), st));
     HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&zp), z.numel() * 2 * sizeof(unsigned short), st));
-    int rc = split_planes(a.p, ap, a.numel(), st) || split_planes_pow2(z.p, zp, z.numel(), amax, st) ||
-             conv_wgrad_tc(d, a, ap, z, zp, amax, tmp, st) || ohwi_to_oihw(tmp, dw_oihw, Cout, Cin, kh, kw, st);
+    WgradPlanes p = {ap, zp, amax, false, false};
+    int rc = wgrad(d, a, z, true, p, tmp, st) || ohwi_to_oihw(tmp, dw_oihw, Cout, Cin, kh, kw, st);
     cudaFreeAsync(tmp, st); cudaFreeAsync(amax, st); cudaFreeAsync(ap, st); cudaFreeAsync(zp, st);
     return rc;
 }

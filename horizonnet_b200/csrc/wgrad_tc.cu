@@ -19,7 +19,6 @@
 //              registers), then main + cross, power-of-two rescale and fp32 reductions (red.global.add.v2) into
 //              dW[Cout][taps][Cin] (several pixel slices and the CTAs of different images add into the same tile)
 #include <cuda.h>
-#include <cstdlib>
 #include <cstring>
 
 #include "hn_common.cuh"
@@ -227,12 +226,6 @@ int choose_slices(long long num_kt, long long items, int sms, long long* slices_
 }
 
 }  // namespace
-
-bool wgrad_tc_on() {
-    // HN_WGRAD_TC=0/1 selects the fp32 CUDA-core / the tensor-core weight-gradient kernel for the convolutions it supports
-    const char* e = getenv("HN_WGRAD_TC");
-    return e ? atoi(e) != 0 : HN_WGRAD_TC_DEFAULT != 0;
-}
 
 bool conv_wgrad_tc_supported(const ConvDesc& d, const Act& in, const Act& dz) {
     if (d.Cin % 64 != 0 || d.Cout % 64 != 0) return false;

@@ -115,9 +115,10 @@ int hn_model_get_tensor(hn_model* m, const char* key, float* out, long long nume
  * themselves (train.py:53-56: L1 + BCE-with-logits) and the optimizer (train.py:216-223) stay with the caller -- and
  * leaves d(loss)/d(parameter) for every state_dict parameter in the reference's layout (nn.Conv2d OIHW, nn.LSTM
  * [4H][in], ...), read back with hn_model_get_grad (device pointer).  One backward per forward.  With option
- * "tensor_cores" on, the encoder and height-reduction convolutions, their data gradients (hn_conv2d_dgrad_tc) and their
- * weight gradients (hn_conv2d_wgrad_tc, see hn_wgrad_tc_enabled) run on the split-fp16 wgmma kernels where those take the
- * shape, everything else on exact fp32 CUDA-core kernels; no loss scaling or gradient all-reduce. */
+ * "tensor_cores" on, the encoder and height-reduction convolutions, their data gradients (hn_conv2d_dgrad_tc) and the
+ * weight gradients of those convolutions, the LSTM and the MLP head (hn_conv2d_wgrad_tc) run on the split-fp16 wgmma
+ * kernels where those take the shape, everything else on exact fp32 CUDA-core kernels; no loss scaling or gradient
+ * all-reduce. */
 int hn_train_forward(hn_model* m, const float* x_nchw_dev, int batch, int in_channels, float* bon_dev, float* cor_dev,
                      const unsigned char* bn_train, const double* bn_factor, int n_bn, unsigned long long seed,
                      double rnn_dropout, double head_dropout, const float* rnn_mask_dev, const float* head_mask_dev,
@@ -256,7 +257,8 @@ int hn_conv2d_wgrad_tc(const float* in, int B, int H, int W, int Cin, const floa
  * tile, tiles per row, box rows, images per tile, pixel tiles (64 pixels each), tiles per slice, slices, work items per slice,
  * CTAs.  -1 for a shape the kernel does not take. */
 int hn_wgrad_tc_plan(int B, int H, int W, int Cin, int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int sms, int plan[10]);
-int hn_wgrad_tc_enabled(void);   /* 1: the training step uses that kernel where it applies (env HN_WGRAD_TC=0/1 overrides the default) */
+/* Returns 1: the training step runs the weight gradients on that kernel wherever option "tensor_cores" is on and the shape fits. */
+int hn_wgrad_tc_enabled(void);
 /* The data gradient on the tensor cores exactly as the training step computes it (zero-dilated dz for a strided conv,
  * power-of-two scaled planes of dz, flipped weights as planes, the transposed conv with fp32 output) and ADDED to din:
  * dz [B][Ho][Wo+2][Cout] and din [B][H][W+2][Cin], halo-1 NHWC fp32 with circular halo columns; w_oihw: the forward

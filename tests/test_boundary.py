@@ -224,6 +224,6 @@ def test_every_environment_switch_of_the_library_is_known_and_documented():
         src = open(f).read()
         names |= set(re.findall(r'getenv\("(HN_[A-Z0-9_]+)"\)', src)) | set(re.findall(r"environ\.get\('(HN_[A-Z0-9_]+)'", src))
     doc = open(os.path.join(root, 'INTEGRATION.md')).read()
-    assert names == {'HN_LSTM_VERBOSE', 'HN_TC_PDL', 'HN_TRAIN_PROF', 'HN_WGRAD_TC'}, names
+    assert names == {'HN_LSTM_VERBOSE', 'HN_TC_PDL', 'HN_TRAIN_PROF'}, names
     missing = sorted(n for n in names if n not in doc)
     assert not missing, missing

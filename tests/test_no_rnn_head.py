@@ -451,13 +451,12 @@ def _worst(net, ref):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('tensor_cores,wgrad_tc', [(True, '1'), (True, '0'), (False, '0')])
-def test_no_rnn_training_step_gradients_match_autograd_of_the_oracle(_built, tensor_cores, wgrad_tc, monkeypatch):
+@pytest.mark.parametrize('tensor_cores', [True, False])
+def test_no_rnn_training_step_gradients_match_autograd_of_the_oracle(_built, tensor_cores):
     sd = synthetic_state_dict(1, 'random', use_rnn=False)
     x = synthetic_panoramas(2, seed=41)
     gen = torch.Generator().manual_seed(9)
     y_bon, y_cor = torch.rand(2, 2, 1024, generator=gen) - 0.5, torch.rand(2, 1, 1024, generator=gen)
-    monkeypatch.setenv('HN_WGRAD_TC', wgrad_tc)
     net = _train_net(sd, tensor_cores)
     torch.manual_seed(11)
     bon, cor = net(x.to(DEV))

@@ -149,11 +149,11 @@ def test_graph_follows_the_backbone_specs():
 # kernel tests' ceilings (2e-5 fp32, 1e-4 split-fp16 tensor cores and the head).  Measured worst of three runs (fp32,
 # tensor cores):  forward 6.1e-6, 2.8e-6   head 1.2e-6, 2.4e-6   unit 4.9e-6, 1.7e-6   wgrad 3.3e-6, 7.0e-5
 #                 stem 1.9e-6, 2.4e-6   maxpool 1.0e-6, 1.2e-6   pool_sum 2.2e-8, 1.4e-7
-# wgrad (the conv weight gradients after the stem) counts as "tensor cores" only where HN_WGRAD_TC puts them on
-# wgrad_tc.cu.  Its worst ratios (3.4e-5 to 7.0e-5) are all at layer-1 / layer2.0 weight gradients, whose sums run over
-# 2-3 x 32768 non-negative input pixels, 16-24 x the 4096 of its kernel test; 4x of 7.0e-5 would exceed the ceiling, so the
-# bound is the ceiling.  unit = the data gradient a unit sends to its producers and its BatchNorm (and frozen conv-bias)
-# gradients.
+# wgrad (the conv weight gradients after the stem) takes the tensor-core bound with tensor cores on: the training step
+# then runs them on wgrad_tc.cu wherever that kernel takes the shape.  Its worst ratios (3.4e-5 to 7.0e-5) are all at
+# layer-1 / layer2.0 weight gradients, whose sums run over 2-3 x 32768 non-negative input pixels, 16-24 x the 4096 of
+# its kernel test; 4x of 7.0e-5 would exceed the ceiling, so the bound is the ceiling.  unit = the data gradient a unit
+# sends to its producers and its BatchNorm (and frozen conv-bias) gradients.
 BOUND = {
     'forward':  (2e-5, 1.2e-5),
     'head':     (5e-6, 1e-5),
@@ -165,14 +165,14 @@ BOUND = {
 }
 
 CONFIGS = [
-    # backbone, use_rnn, tensor_cores, HN_WGRAD_TC (None: the built-in default), batch, frozen blocks
-    pytest.param('resnet50', True, True, '1', 3, False, id='r50-lstm-tc-wgradtc-b3'),
-    pytest.param('resnet50', True, True, '0', 2, False, id='r50-lstm-tc-wgradf32-b2'),
-    pytest.param('resnet50', True, False, None, 1, False, id='r50-lstm-fp32-b1'),
-    pytest.param('resnet50', True, True, None, 2, True, id='r50-lstm-tc-frozen-b2'),
-    pytest.param('resnet50', False, True, None, 3, False, id='r50-mlp-tc-b3'),
-    pytest.param('resnet18', True, True, None, 2, False, id='r18-lstm-tc-b2'),
-    pytest.param('resnet18', False, False, None, 3, False, id='r18-mlp-fp32-b3'),
+    # backbone, use_rnn, tensor_cores, batch, frozen blocks
+    pytest.param('resnet50', True, True, 3, False, id='r50-lstm-tc-wgradtc-b3'),
+    pytest.param('resnet50', True, False, 2, False, id='r50-lstm-fp32-b2'),
+    pytest.param('resnet50', True, False, 1, False, id='r50-lstm-fp32-b1'),
+    pytest.param('resnet50', True, True, 2, True, id='r50-lstm-tc-frozen-b2'),
+    pytest.param('resnet50', False, True, 3, False, id='r50-mlp-tc-b3'),
+    pytest.param('resnet18', True, True, 2, False, id='r18-lstm-tc-b2'),
+    pytest.param('resnet18', False, False, 3, False, id='r18-mlp-fp32-b3'),
 ]
 
 
@@ -210,12 +210,12 @@ def slice_ratios(got, ref, keep=None, activation=True):
 class Judge:
     """Collects every comparison of one configuration: records it, keeps the worst ratio per section, lists violations."""
 
-    def __init__(self, config, tensor_cores, wgrad_tc):
-        self.config, self.tc, self.wgrad_tc = config, int(tensor_cores), int(tensor_cores and wgrad_tc)
+    def __init__(self, config, tensor_cores):
+        self.config, self.tc = config, int(tensor_cores)
         self.worst, self.failures = {}, []
 
     def bound(self, section):
-        return BOUND[section][self.wgrad_tc if section == 'wgrad' else self.tc]
+        return BOUND[section][self.tc]
 
     def __call__(self, section, unit, tensor, got, ref, keep=None, activation=True):
         assert got.shape == ref.shape, (section, unit, tensor, tuple(got.shape), tuple(ref.shape))
@@ -302,17 +302,12 @@ def judge_step(net, backbone, use_rnn, sd, x, bon, cor, r_bon, r_cor, frozen_bn,
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('backbone,use_rnn,tensor_cores,wgrad_tc,batch,frozen', CONFIGS)
-def test_training_step_matches_the_fp64_replay_of_its_tape(_built, monkeypatch, request, backbone, use_rnn, tensor_cores,
-                                                            wgrad_tc, batch, frozen):
+@pytest.mark.parametrize('backbone,use_rnn,tensor_cores,batch,frozen', CONFIGS)
+def test_training_step_matches_the_fp64_replay_of_its_tape(_built, request, backbone, use_rnn, tensor_cores, batch, frozen):
     """One net.train() step with dropout on and a linear loss (so d(bon), d(cor) are known exactly), then every step of
     its backward against the fp64 replay built from the device's own inputs to that step: each unit's forward (z, y),
     the sequence adjoint and the head, each conv unit's parameter gradients and the data gradient it sends to its
     producers, the max-pool routing and the stem."""
-    if wgrad_tc is None:
-        monkeypatch.delenv('HN_WGRAD_TC', raising=False)
-    else:
-        monkeypatch.setenv('HN_WGRAD_TC', wgrad_tc)
     config = request.node.callspec.id
     B = batch
     sd = synthetic_state_dict(11, 'random', use_rnn=use_rnn, backbone=backbone)
@@ -339,7 +334,7 @@ def test_training_step_matches_the_fp64_replay_of_its_tape(_built, monkeypatch, 
     loss.backward()
     net.check()
 
-    judge = Judge(config, tensor_cores, _lib.lib().hn_wgrad_tc_enabled() == 1)
+    judge = Judge(config, tensor_cores)
     judge_step(net, backbone, use_rnn, sd, x, bon.detach(), cor.detach(), r_bon, r_cor, frozen_bn, judge, DEV)
     summary = {s: {'ratio': w[0], 'unit': w[1], 'tensor': w[2], 'slice': w[3], 'bound': judge.bound(s)}
                for s, w in judge.worst.items()}

@@ -68,6 +68,7 @@ def _check_plan_covers_every_conv_unit(B, sms):
 
 def test_plan_rejects_what_the_kernel_does_not_take():
     assert plan(2, 16, 32, 48, 64, 3, (1, 1)) is None                # Cin % 64
+    assert plan(2, 512, 1024, 3, 64, 7, (2, 2)) is None              # the stem (Cin = 3): its weight gradient stays fp32
     assert plan(2, 16, 24, 64, 64, 3, (1, 1)) is None                # W = 24: not a power-of-two tile width
     assert plan(2, 6, 16, 64, 64, 3, (1, 1)) is None                 # 4 rows per tile, 6 rows per image
     assert plan(2, 16, 32, 64, 64, 3, (3, 1)) is None                # stride 3
