@@ -129,6 +129,89 @@ __device__ __forceinline__ void chunk_mma(float (&acc)[R], uint32_t a_hi, uint32
     reg_fence(acc);
 }
 
+// Consumer side of an operand ring.  Per K chunk: the weight tile (hi plane, lo plane b_plane bytes on) of ring stage
+// `stage`, and the A operand (hi, lo a_plane bytes on) -- from the same stage, or in dxr mode from one of two input-row
+// slots that three consecutive chunks (taps dx = 0, 1, 2) read at a start address shifted by dx rows of 128 B.  Chunks
+// are acquired and released in ring order; the release cursor trails the acquire cursor by the chunks whose wgmma
+// group may still be in flight.
+struct RingPos {
+    int stage = 0, ast = 0, dx = 0;        // weight stage; dxr: input-row slot and tap
+    uint32_t phase = 0, aph = 0;
+    // one chunk on; selects, no branches
+    template <bool DXR>
+    __device__ __forceinline__ void step(int nst) {
+        const bool wrap = stage + 1 == nst;
+        stage = wrap ? 0 : stage + 1;
+        phase ^= (uint32_t)wrap;
+        if (DXR) {
+            const bool row_end = dx == 2;
+            dx = row_end ? 0 : dx + 1;
+            aph ^= (uint32_t)(row_end && ast == 1);
+            ast ^= (int)row_end;
+        }
+    }
+};
+struct ConsRing {
+    uint32_t a0, a_step, a_plane, b0, b_step, b_plane;     // shared addresses: slot i at a0 + i * a_step (likewise b)
+    uint64_t* full;
+    uint64_t* empty;
+    uint64_t* afull;           // dxr: input-row slot filled / read by its three taps
+    uint64_t* aempty;
+    int nst;
+    RingPos get, rel;
+};
+// hand the oldest unreleased chunk's weight stage (and, after its third tap, its input-row slot) back to the producer;
+// only once the chunk's wgmma group has completed
+template <bool DXR>
+__device__ __forceinline__ void ring_release(ConsRing& q, int lane) {
+    __syncwarp();
+    mbar_arrive_if(q.empty + q.rel.stage, lane == 0);
+    if (DXR) mbar_arrive_if(q.aempty + q.rel.ast, lane == 0 && q.rel.dx == 2);
+    q.rel.step<DXR>(q.nst);
+}
+// One segment of N chunks: the accumulator restarts at its first chunk and is added into `sum` (round-to-nearest fp32)
+// after its last.  Straight-line code with compile-time wgmma wait counts: chunk i + 1 is issued while chunk i's group
+// is in flight, and nothing between an issue and its wait branches (see mbar_arrive_if).
+template <int N, bool DXR, int R>
+__device__ __forceinline__ void mma_segment(float (&acc)[R], float (&sum)[R], ConsRing& q, uint32_t a_row_off, int lane) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+        const RingPos& g = q.get;
+        if (DXR) mbar_wait(q.afull + g.ast, g.aph);   // returns at once for dx = 1, 2: the slot is held until dx = 2 retires
+        mbar_wait(q.full + g.stage, g.phase);
+        const uint32_t a = DXR ? q.a0 + g.ast * q.a_step + g.dx * 128 : q.a0 + g.stage * q.a_step;
+        const uint32_t b = q.b0 + g.stage * q.b_step;
+        chunk_issue(acc, a + a_row_off, a + q.a_plane + a_row_off, b, b + q.b_plane, i == 0);
+        q.get.step<DXR>(q.nst);
+        if (i > 0) {
+            wgmma_wait1();
+            ring_release<DXR>(q, lane);
+        }
+    }
+    wgmma_wait0();
+    reg_fence(acc);
+    ring_release<DXR>(q, lane);
+#pragma unroll
+    for (int j = 0; j < R; ++j) sum[j] += acc[j];
+}
+// sum = the num_kc chunks of one tile in segments of SEG; the last segment takes the K tail.  Nothing is in flight
+// between segments, so the choice of the tail's length branches freely.
+template <bool DXR, int R>
+__device__ __forceinline__ void mma_chunks(float (&acc)[R], float (&sum)[R], ConsRing& q, int num_kc, uint32_t a_row_off,
+                                           int lane) {
+    static_assert(SEG == 4, "mma_chunks: tail segments of 1 to 3 chunks");
+#pragma unroll
+    for (int j = 0; j < R; ++j) sum[j] = 0.f;
+    int kc = 0;
+    for (; kc + SEG <= num_kc; kc += SEG) mma_segment<SEG, DXR>(acc, sum, q, a_row_off, lane);
+    switch (num_kc - kc) {
+        case 3: mma_segment<3, DXR>(acc, sum, q, a_row_off, lane); break;
+        case 2: mma_segment<2, DXR>(acc, sum, q, a_row_off, lane); break;
+        case 1: mma_segment<1, DXR>(acc, sum, q, a_row_off, lane); break;
+        default: break;
+    }
+}
+
 // tile row of accumulator element pair h (0: d[4j], d[4j+1]; 1: d[4j+2], d[4j+3]) of this thread's wgmma fragment
 __device__ __forceinline__ int frag_row(int wg, int warp, int lane, int h) {
     return wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
@@ -435,65 +518,20 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int wg = (warp - CONS_WARP0) >> 2;         // tile rows [64 wg, 64 wg + 64)
         const uint32_t a_row_off = (uint32_t)(wg * 64 * 128);
         float acc[BN / 2], sum[BN / 2];
-        int stage = 0, ast = 0;
-        uint32_t phase = 0, aph = 0;
+        // dxr: the two input-row slots, then the weight slots; otherwise A and B planes of each ring stage
+        const uint32_t s0 = smem_u32(smem);
+        ConsRing ring = a.dxr ? ConsRing{s0, AX_SLOT, AX_PLANE, s0 + BX_OFF, BX_SLOT, S::B_PLANE,
+                                         full_bar, empty_bar, afull_bar, aempty_bar, NST}
+                              : ConsRing{s0, S::STAGE, S::A_PLANE, s0 + 2 * S::A_PLANE, S::STAGE, S::B_PLANE,
+                                         full_bar, empty_bar, afull_bar, aempty_bar, NST};
         for (int it = 0;; ++it) {
             const int tile = tq->next(it);
             __syncwarp();
             if (lane == 0) tq->release(it);
             if (tile >= a.num_tiles) break;
             const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-#pragma unroll
-            for (int j = 0; j < BN / 2; ++j) sum[j] = 0.f;
-            int seg_pos = 0, held = -1;      // held: ring stage whose wgmma group may still be in flight
-            auto release = [&](int st) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + st); };
-            // one K chunk from the operand slot `sA` (hi plane, lo plane `a_plane` bytes on) and the weight slot `sB` of ring
-            // stage `st`.  One wgmma group stays in flight across chunks; `drain` (and the end of a segment) waits for all
-            auto step = [&](uint32_t sA, uint32_t a_plane, uint32_t sB, int st, bool last, bool drain) {
-                chunk_issue(acc, sA + a_row_off, sA + a_plane + a_row_off, sB, sB + S::B_PLANE, seg_pos == 0);
-                const bool seg_end = (++seg_pos == SEG || last);
-                if (seg_end || drain) {
-                    wgmma_wait0();
-                    reg_fence(acc);
-                    if (held >= 0) release(held);
-                    release(st);
-                    held = -1;
-                } else {
-                    wgmma_wait1();
-                    if (held >= 0) release(held);
-                    held = st;
-                }
-                if (seg_end) {
-#pragma unroll
-                    for (int j = 0; j < BN / 2; ++j) sum[j] += acc[j];
-                    seg_pos = 0;
-                }
-            };
-            if (a.dxr) {
-                const int ndyc = a.num_kc / a.kw;
-                int kc = 0;
-                for (int dyc = 0; dyc < ndyc; ++dyc) {
-                    mbar_wait(afull_bar + ast, aph);
-                    const uint32_t sAx = smem_u32(smem + ast * AX_SLOT);
-                    for (int dx = 0; dx < 3; ++dx, ++kc) {
-                        mbar_wait(full_bar + stage, phase);
-                        // tap dx = the same 130-pixel row read from pixel dx on: start address + dx rows of 128 B
-                        step(sAx + dx * 128, AX_PLANE, smem_u32(smem + BX_OFF + stage * BX_SLOT), stage,
-                             kc == a.num_kc - 1, dx == 2);
-                        if (++stage == NST) { stage = 0; phase ^= 1; }
-                    }
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(aempty_bar + ast);    // the input-row slot is free once the three taps retire
-                    if (++ast == 2) { ast = 0; aph ^= 1; }
-                }
-            } else {
-                for (int kc = 0; kc < a.num_kc; ++kc) {
-                    mbar_wait(full_bar + stage, phase);
-                    const uint32_t sA = smem_u32(smem + stage * S::STAGE);
-                    step(sA, S::A_PLANE, sA + 2 * S::A_PLANE, stage, kc == a.num_kc - 1, false);
-                    if (++stage == NST) { stage = 0; phase ^= 1; }
-                }
-            }
+            if (a.dxr) mma_chunks<true>(acc, sum, ring, a.num_kc, a_row_off, lane);
+            else mma_chunks<false>(acc, sum, ring, a.num_kc, a_row_off, lane);
 
             // ---- epilogue in the slot
             HaloStore halo = {a.out_f32 ? static_cast<void*>(a.out_f32) : a.out, a.out_plane, a.Cout, 0, {-1, -1}};
@@ -504,11 +542,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 for (int h = 0; h < 2; ++h)
                     halo.pix[h] = halo_pixel(frag_row(wg, warp, lane, h), (long long)R0 * a.Wop, a.Wop, a.tw, rows, wo0, a.Wo);
             }
-            const int st0 = stage;
+            // the slot's stages go back to the producer through the store warp
+            const int st0 = ring.get.stage;
             const uint32_t x = smem_u32(slot_x(st0)), y = smem_u32(slot_y(st0));
             for (int e = 0; e < epi_stages; ++e) {
-                mbar_wait(full_bar + stage, phase);
-                if (++stage == NST) { stage = 0; phase ^= 1; }
+                mbar_wait(full_bar + ring.get.stage, ring.get.phase);
+                ring.get.step<false>(NST);
+                ring.rel.step<false>(NST);
             }
             const float* sc = cst + nt * BN;
             const float* sf = cst + a.Cout + nt * BN;

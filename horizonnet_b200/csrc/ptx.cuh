@@ -19,6 +19,14 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// the arrive of the threads where `pred` holds, as a predicated instruction rather than a branch: code that runs while
+// a wgmma group is in flight must not diverge, or ptxas serialises every wgmma of the kernel (warning C7518)
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
+        ::"r"(smem_u32(bar)), "r"((uint32_t)pred)
+        : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
