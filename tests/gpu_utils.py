@@ -212,6 +212,95 @@ def run_dgrad_case(B, Ci, H, W, Co, k, stride, dz_scale=1.0, prefill=False, zero
     return _worst_ratio(got - (pre.double() + ref), bound)
 
 
+# ---- elementwise error bound of the tensor-core weight gradient (wgrad_tc.cu): dW = dz^T x over the pixel axis, both operands
+# as split planes (x: fp16 hi / lo of x/16; dz: of dz * f/16 with f = pow2_factor(max|dz|)), products hi*hi + hi*lo + lo*hi
+# accumulated in fp32:
+#  * operands with normal lo planes leave 2^-22 |v| each, the dropped lo*lo is 2^-22 |dz||x| at most: 1.5 * 2^-21 per
+#    product.  The fp32 sums -- wgmma accumulation over a slice of up to 4096 pixels in 16-pixel steps, the reduction of
+#    the pixel slices with red.global.add and the final rounding -- add 2^-24 of a partial sum per step; with BN-backward
+#    dz (zero mean over the pixels of each channel) the partial sums stay far below sum |dz||x|, and 6.5 * 2^-21 of it
+#    leaves them 200 steps of worst-case growth.  C_WGRAD = 8 in all: C_WGRAD * 2^-21 * (|dz|^T |x|);
+#  * activations below 2 in magnitude (every LSTM state) have a subnormal lo plane: 2^-25 * 16 = 2^-21 absolute per
+#    element (2^-20 with margin):  2^-20 * (|dz|^T 1);
+#  * small dz (a channel 2^-20 below the largest) has a subnormal lo plane too: 2^-21 / f absolute per element (2^-20 / f
+#    with margin):  2^-20 / f * (1^T |x|).
+# A lost cross product (hi*lo or lo*hi) leaves an error of about 2^-12 |dz||x| per pixel, i.e. 2^-12 sqrt(N) against the
+# bound's 2^-18 N over N pixels of similar terms: the bound notices it below about 4000 pixels per weight, which every
+# unit case has.
+C_WGRAD = 8.0
+
+
+def wgrad_case_inputs(c, dev, seed=None):
+    """Inputs that look like the training step's: x post-ReLU (about half zeros) or an LSTM state inside (-1, 1); dz of
+    zero mean with per-output-channel scales spread over 2^-20 .. 1, like BatchNorm-backward output."""
+    g = torch.Generator().manual_seed(seed if seed is not None else
+                                      int(hashlib.sha1(c['name'].encode()).hexdigest()[:8], 16))
+    B, Ci, H, W, Co, k = c['B'], c['Cin'], c['H'], c['W'], c['Cout'], c['k']
+    sh, sw = c['stride']
+    Ho, Wo = (H + 2 * (k // 2) - k) // sh + 1, (W + 2 * (k // 2) - k) // sw + 1
+    if c['kind'] == 'lstm':
+        x = torch.rand(B, Ci, H, W, generator=g) * 2 - 1
+    else:
+        x = torch.relu(torch.randn(B, Ci, H, W, generator=g))
+    scale = 2.0 ** (-20 * torch.rand(Co, generator=g))
+    scale[torch.randint(Co, (1,), generator=g)] = 1.0
+    dz = torch.randn(B, Co, Ho, Wo, generator=g) * scale.view(1, -1, 1, 1)
+    return x.to(dev), dz.to(dev)
+
+
+def wgrad_reference(x, dz, k, stride):
+    """dW (OIHW) of the circular-W, zero-H-padded convolution, by autograd in the dtype of the inputs."""
+    w = torch.zeros(dz.shape[1], x.shape[1], k, k, dtype=x.dtype, device=x.device, requires_grad=True)
+    _conv_abs(x, w, stride, k // 2, k // 2).backward(dz)
+    return w.grad
+
+
+def run_wgrad_case(c, zero_dz=False, with_fp32=False, dev='cuda:0'):
+    """Runs one case of tests/wgrad_cases.py through hn_conv2d_wgrad_tc (the training step's wgrad: plane splits, then
+    wgrad_tc_kernel) and checks dW against fp64 elementwise with the bound above.  dW starts NaN-filled with a canary behind
+    it.  zero_dz: dz = 0, for which dW must be exactly 0.  with_fp32: also runs hn_conv2d_backward (the fp32 CUDA-core
+    weight gradient) on the same inputs under the same bound.  Returns worst err / bound (and the fp32 kernel's)."""
+    lib = _lib.lib()
+    x, dz = wgrad_case_inputs(c, dev)
+    if zero_dz:
+        dz.zero_()
+    B, Ci, H, W, Co, k = c['B'], c['Cin'], c['H'], c['W'], c['Cout'], c['k']
+    sh, sw = c['stride']
+    p = k // 2
+    xin, dzin = to_halo_nhwc(x, 1), to_halo_nhwc(dz, 1)
+    st = torch.cuda.current_stream(dev).cuda_stream
+
+    def run(fn, *args):
+        n = Co * Ci * k * k
+        buf = torch.full((n + 4096,), float('nan'), device=dev)
+        buf[n:] = CANARY
+        _lib.check(fn(*args[:-1], buf.data_ptr(), st), fn.__name__)
+        torch.cuda.synchronize(dev)
+        dw = buf[:n].view(Co, Ci, k, k)
+        assert not torch.isnan(dw).any(), f"{c['name']}: dW elements left unwritten"
+        assert bool((buf[n:] == CANARY).all()), f"{c['name']}: write past the end of dW"
+        return dw.double()
+
+    got = run(lib.hn_conv2d_wgrad_tc, xin.data_ptr(), B, H, W, Ci, dzin.data_ptr(), Co, k, k, sh, sw, p, p, None)
+    if zero_dz:
+        assert torch.equal(got, torch.zeros_like(got)), f"{c['name']}: an all-zero dz must give dW = 0 exactly"
+        return 0.0
+    xd, dzd = x.double(), dz.double()
+    ref = wgrad_reference(xd, dzd, k, (sh, sw))
+    acc = wgrad_reference(xd.abs(), dzd.abs(), k, (sh, sw))
+    ones_x = wgrad_reference(torch.ones_like(xd[:, :1]), dzd.abs(), k, (sh, sw)).expand_as(ref)
+    ones_z = wgrad_reference(xd.abs(), torch.ones_like(dzd[:, :1]), k, (sh, sw)).expand_as(ref)
+    f = pow2_factor(dz.abs().max().item())
+    bound = C_WGRAD * EPS21 * acc + EPS20 * ones_x + EPS20 / f * ones_z
+    ratio = _worst_ratio(got - ref, bound)
+    if not with_fp32:
+        return ratio
+    wdev = torch.zeros(Co, Ci, k, k, device=dev)
+    got32 = run(lib.hn_conv2d_backward, xin.data_ptr(), B, H, W, Ci, 1, wdev.data_ptr(), dzin.data_ptr(), Co, k, k, sh, sw,
+                p, p, None, None)
+    return ratio, _worst_ratio(got32 - ref, bound)
+
+
 def device_sms(dev=0):
     return torch.cuda.get_device_properties(dev).multi_processor_count
 

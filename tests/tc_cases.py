@@ -1,45 +1,68 @@
-"""Shapes of HorizonNet('resnet50', rnn) and launch plans of the tensor-core convolution (no GPU needed).
+"""Shapes of HorizonNet('resnet50' / 'resnet18', rnn) and launch plans of the tensor-core convolution (no GPU needed).
 
-* resnet50_rnn_convs -- every conv unit behind the stem (shared with test_wgrad_plan.py);
-* model_launches     -- every conv_tc_planes launch the library makes for a batch: eval forward, train-mode forward (batch
-                        statistics pass and real pass), the fp32 raw pass of the training step, the LSTM input projections
-                        and the data gradient of every unit (train_step.cu: the transposed conv as a stride-1 conv);
+* conv_units         -- every conv unit behind the stem of a backbone (resnet50_rnn_convs: resnet50's, shared with
+                        test_wgrad_plan.py and profiles/conv_launches.py);
+* model_launches     -- every conv_tc_planes launch the library makes for a backbone and a batch: eval forward, train-mode
+                        forward (batch statistics pass and real pass), the fp32 raw pass of the training step, the LSTM
+                        input projections and the data gradient of every unit (train_step.cu: the transposed conv as a
+                        stride-1 conv);
 * plan / variant_key -- hn_conv_tc_plan and the code paths of conv_tc.cu a plan selects;
 * CASES              -- the unit cases of test_tc_kernels.py; test_conv_tc_plan.py checks that they reach every variant
                         key the model reaches."""
 import ctypes
 
 from horizonnet_b200 import _lib
+from horizonnet_b200._spec import BACKBONES, c_last
 
 SMS = 132                     # H100 SXM
+SM_COUNTS = (132, 114)        # H100 SXM, H100 PCIe
+BATCHES = (1, 2, 3, 8, 16, 32, 64)
 PLAN_FIELDS = ('gemm_kernel', 'BN', 'mode', 'M', 'tw', 'rows_per_tile', 'wsegs', 'rowbox', 'box_rows', 'box_imgs', 'dxr',
                'parity', 'num_kc', 'seg', 'pf', 'n_tiles', 'num_tiles', 'grid')
 
 
-def resnet50_rnn_convs():
-    """(name, H, W, Cin, Cout, k, stride) of every conv unit behind the stem, input geometry at 512 x 1024."""
+def conv_units(backbone):
+    """(name, H, W, Cin, Cout, k, stride) of every conv unit behind the stem, input geometry at 512 x 1024, in the order
+    of the forward: per block conv1, downsample, conv2 (and conv3 of a Bottleneck), then ghc{s}.{j}."""
+    kind, nblk, planes, expansion = BACKBONES[backbone]
     out = []
-    planes, nblk = (64, 128, 256, 512), (3, 4, 6, 3)
     H, W, inpl = 128, 256, 64
     for l in range(4):
         p = planes[l]
         for b in range(nblk[l]):
             s = 2 if (b == 0 and l > 0) else 1
             n = f'layer{l + 1}.{b}'
-            out.append((n + '.conv1', H, W, inpl, p, 1, (1, 1)))
-            if b == 0:
-                out.append((n + '.downsample', H, W, inpl, 4 * p, 1, (s, s)))
-            out.append((n + '.conv2', H, W, p, p, 3, (s, s)))
-            out.append((n + '.conv3', H // s, W // s, p, 4 * p, 1, (1, 1)))
-            inpl, H, W = 4 * p, H // s, W // s
+            ds = b == 0 and (s != 1 or inpl != p * expansion)
+            if kind == 'bottleneck':                  # v1.5: the stride on conv2
+                out.append((n + '.conv1', H, W, inpl, p, 1, (1, 1)))
+                if ds:
+                    out.append((n + '.downsample', H, W, inpl, p * expansion, 1, (s, s)))
+                out.append((n + '.conv2', H, W, p, p, 3, (s, s)))
+                out.append((n + '.conv3', H // s, W // s, p, p * expansion, 1, (1, 1)))
+            else:                                     # BasicBlock: the stride on conv1
+                out.append((n + '.conv1', H, W, inpl, p, 3, (s, s)))
+                if ds:
+                    out.append((n + '.downsample', H, W, inpl, p, 1, (s, s)))
+                out.append((n + '.conv2', H // s, W // s, p, p, 3, (1, 1)))
+            inpl, H, W = p * expansion, H // s, W // s
     for s in range(4):
-        c = planes[s] * 4
+        c = planes[s] * expansion
         ch = (c, c // 2, c // 2, c // 4, c // 8)
         h, w = 128 >> s, 256 >> s
         for j in range(4):
             out.append((f'ghc{s}.{j}', h, w, ch[j], ch[j + 1], 3, (2, 1)))
             h //= 2
     return out
+
+
+def resnet50_rnn_convs():
+    return conv_units('resnet50')
+
+
+def has_residual(backbone, name):
+    """The unit adds the block's identity before its ReLU: a Bottleneck's conv3, a BasicBlock's conv2."""
+    last = 'conv3' if BACKBONES[backbone][0] == 'bottleneck' else 'conv2'
+    return name.startswith('layer') and name.endswith(last)
 
 
 def launch(name, B, H, W, Cin, Cout, k, stride, in_halo=1, out_halo=1, out_f32=False, residual=False, pad=None):
@@ -55,16 +78,17 @@ def dgrad_launch(name, B, H, W, Cin, Cout, k, stride):
     return launch(name + ':dgrad', B, H, W, Cout, Cin, k, (1, 1), out_f32=True, pad=(k - 1 - p, k - 1 - p))
 
 
-def model_launches(B):
+def model_launches(backbone, B):
     out = []
-    for name, H, W, Ci, Co, k, st in resnet50_rnn_convs():
-        res = name.endswith('conv3')
+    for name, H, W, Ci, Co, k, st in conv_units(backbone):
+        res = has_residual(backbone, name)
         out.append(launch(name, B, H, W, Ci, Co, k, st, residual=res))                       # eval; train real pass
         out.append(launch(name + ':stats', B, H, W, Ci, Co, k, st))                          # train batch-statistics pass
         out.append(launch(name + ':raw', B, H, W, Ci, Co, k, st, out_f32=True))              # training step raw pass
         out.append(dgrad_launch(name, B, H, W, Ci, Co, k, st))
     for layer in range(2):                                                                   # LSTM input projections
-        out.append(launch(f'xproj{layer}', 1, 1, 256 * B, 1024, 4096, 1, (1, 1), 0, 0, out_f32=True))
+        out.append(launch(f'xproj{layer}', 1, 1, 256 * B, c_last(backbone) if layer == 0 else 1024, 4096, 1, (1, 1), 0, 0,
+                          out_f32=True))
     return out
 
 
@@ -152,8 +176,8 @@ F32_CASES = [
     case('f32_s22', 2, 32, 64, 128, 128, 3, (2, 2), out_f32=True),
 ]
 
-# The cheapest launch of the model (batch 1, 2, 3, 8 or 32; input channels cut where the plan stays the same) for each
-# variant key the cases above leave out, named after the layer.  out_f32 = the training step's raw pass, its data gradients
+# The cheapest launch of the model (batch 1 .. 64; input channels cut where the plan stays the same) for each variant key
+# the cases above leave out at 132 or 114 SMs, named after the layer.  out_f32 = the training step's raw pass, its data gradients
 # (":dgrad": the transposed conv of train_step.cu) and the LSTM projections, all run here through hn_conv2d impl = 2.
 MODEL_CASES = [
     case('ghc0.0_b1', 1, 128, 256, 256, 128, 3, (2, 1)),
@@ -217,6 +241,72 @@ MODEL_CASES = [
     case('layer4.0.downsample_raw_b1', 1, 32, 64, 256, 2048, 1, (2, 2), out_f32=True),
     case('layer4.0.downsample_raw_b3', 3, 32, 64, 256, 2048, 1, (2, 2), out_f32=True),
     case('layer4.1.conv2_b8', 8, 16, 32, 256, 512, 3, (1, 1)),
+    # batches 16 and 64, a 114-SM H100 PCIe and resnet18 (prefix r18.): batch and input channels cut where the key stays
+    case('ghc2.2_b32', 29, 8, 64, 64, 256, 3, (2, 1)),
+    case('ghc2.2_raw_b32', 29, 8, 64, 64, 256, 3, (2, 1), out_f32=True),
+    case('ghc2.3_b1', 1, 4, 64, 64, 128, 3, (2, 1)),
+    case('ghc2.3_b64', 58, 4, 64, 64, 128, 3, (2, 1)),
+    case('ghc2.3_dgrad_b32_cut17', 17, 4, 64, 64, 256, 3, (1, 1), out_f32=True),   # batch cut to 17
+    case('ghc2.3_raw_b1', 1, 4, 64, 64, 128, 3, (2, 1), out_f32=True),
+    case('ghc2.3_raw_b64', 58, 4, 64, 64, 128, 3, (2, 1), out_f32=True),
+    case('ghc3.1_b32', 17, 8, 32, 64, 1024, 3, (2, 1)),
+    case('ghc3.1_raw_b32', 17, 8, 32, 64, 1024, 3, (2, 1), out_f32=True),
+    case('ghc3.2_b32', 29, 4, 32, 256, 512, 3, (2, 1)),
+    case('ghc3.2_b64', 57, 4, 32, 256, 512, 3, (2, 1)),
+    case('ghc3.2_dgrad_b32', 17, 4, 32, 64, 1024, 3, (1, 1), out_f32=True),
+    case('ghc3.2_raw_b32', 29, 4, 32, 256, 512, 3, (2, 1), out_f32=True),
+    case('ghc3.2_raw_b64', 57, 4, 32, 256, 512, 3, (2, 1), out_f32=True),
+    case('ghc3.3_dgrad_b32', 29, 2, 32, 256, 512, 3, (1, 1), out_f32=True),
+    case('ghc3.3_dgrad_b64', 57, 2, 32, 256, 512, 3, (1, 1), out_f32=True),
+    case('layer2.1.conv1_b1', 1, 64, 128, 64, 128, 1, (1, 1)),
+    case('r18.ghc2.3_b1', 1, 4, 64, 64, 32, 3, (2, 1)),
+    case('r18.ghc2.3_raw_b1', 1, 4, 64, 64, 32, 3, (2, 1), out_f32=True),
+    case('r18.ghc3.3_b1', 1, 2, 32, 64, 64, 3, (2, 1)),
+    case('r18.ghc3.3_dgrad_b1', 1, 2, 32, 64, 128, 3, (1, 1), out_f32=True),
+    case('r18.ghc3.3_raw_b1', 1, 2, 32, 64, 64, 3, (2, 1), out_f32=True),
+    case('r18.layer1.0.conv2_b1', 1, 128, 256, 64, 64, 3, (1, 1), residual=True),
+    case('r18.layer2.0.conv2_b1', 1, 64, 128, 64, 128, 3, (1, 1), residual=True),
+    case('r18.layer2.0.conv2_b2', 2, 64, 128, 64, 128, 3, (1, 1), residual=True),
+    case('r18.layer2.0.conv2_b3', 3, 64, 128, 64, 128, 3, (1, 1), residual=True),
+    case('r18.layer3.0.conv2_b8', 4, 32, 64, 256, 256, 3, (1, 1), residual=True),
+    case('r18.layer4.0.conv2_b1', 1, 16, 32, 256, 512, 3, (1, 1), residual=True),
+    case('r18.layer4.0.conv2_b16', 9, 16, 32, 256, 512, 3, (1, 1), residual=True),
+    case('r18.layer4.0.conv2_b8', 5, 16, 32, 256, 512, 3, (1, 1), residual=True),
+    case('r18.layer4.0.downsample_b16', 9, 32, 64, 64, 512, 1, (2, 2)),
+    case('r18.layer4.0.downsample_b8', 5, 32, 64, 64, 512, 1, (2, 2)),
+    case('r18.layer4.0.downsample_raw_b1', 1, 32, 64, 256, 512, 1, (2, 2), out_f32=True),
+    case('r18.layer4.0.downsample_raw_b16', 9, 32, 64, 64, 512, 1, (2, 2), out_f32=True),
+    case('r18.layer4.0.downsample_raw_b8', 5, 32, 64, 64, 512, 1, (2, 2), out_f32=True),
 ]
 
 ALL_CASES = CASES + F32_CASES + MODEL_CASES
+
+# Data gradients of the training step through hn_conv2d_dgrad_tc (test_tc_kernels.py): B, Cin, H, W, Cout, k, stride of the
+# unit.  Together they cover every data-gradient unit kind (dgrad_kind) of resnet50 and resnet18; the first four are
+# also run accumulating into a prefilled din.
+DGRAD_CASES = [
+    (2, 64, 32, 128, 64, 3, (1, 1)),          # 3x3 stride 1 (layer1 conv2): dx reuse
+    (2, 128, 32, 64, 128, 3, (2, 2)),         # 3x3 stride 2 (layer2-4 .0.conv2): dilated dz
+    (2, 256, 32, 64, 512, 1, (2, 2)),         # 1x1 stride 2 (downsample)
+    (3, 256, 16, 64, 128, 3, (2, 1)),         # 3x3 stride (2, 1) (height reduction)
+    (2, 512, 16, 32, 128, 1, (1, 1)),         # 1x1 stride 1, Cin > 256 (conv1 of layer3)
+    (2, 256, 8, 64, 1024, 1, (1, 1)),         # layer3.x.conv3
+    (1, 64, 8, 256, 256, 1, (1, 1)),          # layer1.0.conv3, layer1.0.downsample: W = 256
+    (1, 512, 8, 128, 128, 1, (1, 1)),         # layer2.x.conv1: Cin > 256, W = 128
+    (1, 64, 16, 256, 128, 1, (2, 2)),         # resnet18 layer2.0.downsample
+    (2, 1024, 8, 64, 2048, 1, (2, 2)),        # layer4.0.downsample
+    (1, 512, 8, 128, 1024, 1, (2, 2)),        # layer3.0.downsample
+    (2, 256, 8, 64, 256, 3, (1, 1)),          # layer3.x.conv2: W = 64
+    (2, 512, 4, 32, 512, 3, (1, 1)),          # layer4.x.conv2 (both backbones): W = 32
+    (2, 64, 16, 256, 128, 3, (2, 2)),         # resnet18 layer2.0.conv1: 3x3 stride 2, 64 -> 128
+    (2, 512, 8, 64, 512, 3, (2, 2)),          # layer4.0.conv2
+    (2, 128, 8, 256, 64, 3, (2, 1)),          # ghc0.2: W = 256
+    (1, 512, 8, 128, 256, 3, (2, 1)),         # ghc1.0: Cin > 256, W = 128
+    (2, 512, 8, 64, 512, 3, (2, 1)),          # ghc2.1
+]
+
+
+def dgrad_kind(k, stride, Cin, W):
+    """The unit kinds of the data gradient: kernel size, stride, Cin above 256 (the transposed conv's Cout: two or more
+    output-channel tiles of 128) and input rows of 128 or more pixels (one conv row per tile, dx reuse)."""
+    return k, tuple(stride), Cin > 256, W >= 128

@@ -1,9 +1,9 @@
 """Host plan of the tensor-core convolution (hn_conv_tc_plan = what conv_tc_planes launches), no GPU needed:
 * every conv_tc_planes launch of the model (tc_cases.model_launches: eval and train forwards, the training step's raw pass
   and data gradients, the LSTM projections) has a plan whose tiles cover the output exactly once;
-* coverage guard: every variant key (tc_cases.variant_key) the model reaches on a 132-SM H100 SXM is reached by a case of
-  the -m gpu table (tc_cases.ALL_CASES).  A heuristic change that sends the model into a new variant fails here until a
-  unit case for it is added."""
+* coverage guard: every variant key (tc_cases.variant_key) resnet50 or resnet18 reaches at batch 1 .. 64 on a 132-SM H100
+  SXM or a 114-SM H100 PCIe is reached by a case of the -m gpu table (tc_cases.ALL_CASES) planned for the same SM count.
+  A heuristic change that sends the model into a new variant fails here until a unit case for it is added."""
 import pytest
 
 import __graft_entry__ as entry
@@ -49,10 +49,10 @@ def _check(c, p, sms):
         assert not p['gemm_kernel'], name
 
 
-@pytest.mark.parametrize('sms', [132, 114])                 # H100 SXM, H100 PCIe
-@pytest.mark.parametrize('B', [1, 2, 3, 8, 32])
+@pytest.mark.parametrize('sms', T.SM_COUNTS)                 # H100 SXM, H100 PCIe
+@pytest.mark.parametrize('B', T.BATCHES)
 def test_every_model_launch_has_a_plan_covering_its_output_once(B, sms):
-    launches = T.model_launches(B)
+    launches = T.model_launches('resnet50', B)
     assert len(launches) == 4 * 68 + 2
     for c in launches:
         p = T.plan(c, sms)
@@ -63,24 +63,69 @@ def test_every_model_launch_has_a_plan_covering_its_output_once(B, sms):
         _check(c, p, sms)
 
 
-def test_unit_cases_have_consistent_plans():
-    for c in T.ALL_CASES:
-        p = T.plan(c)
+@pytest.mark.parametrize('sms', T.SM_COUNTS)
+@pytest.mark.parametrize('B', T.BATCHES)
+def test_every_resnet18_launch_has_a_plan_covering_its_output_once(B, sms):
+    launches = T.model_launches('resnet18', B)
+    assert len(launches) == 4 * 35 + 2
+    planned = 0
+    for c in launches:
+        p = T.plan(c, sms)
+        if c['Cin'] % 64:
+            # the narrow height-reduction convs (16 / 32 channels in) run on conv_narrow, their data gradients (and
+            # ghc0.0's, 32 channels in) on conv_dgrad_f32
+            assert p is None, c['name']
+            continue
         assert p is not None, (c['name'], _lib.lib().hn_last_error())
-        _check(c, p, T.SMS)
+        _check(c, p, sms)
+        planned += 1
+    # not planned: eval, statistics and raw pass of ghc0.1-3 and ghc1.3 (32 / 16 channels in), the data gradients of
+    # ghc0.0-3, ghc1.2-3 and ghc2.3 (32 / 16 / 8 channels out)
+    assert planned == 4 * 35 + 2 - 3 * 4 - 7
+
+
+def test_unit_cases_have_consistent_plans():
+    names = [c['name'] for c in T.ALL_CASES]
+    assert len(set(names)) == len(names), sorted({n for n in names if names.count(n) > 1})     # the -m gpu test ids
+    for sms in T.SM_COUNTS:
+        for c in T.ALL_CASES:
+            p = T.plan(c, sms)
+            assert p is not None, (c['name'], _lib.lib().hn_last_error())
+            _check(c, p, sms)
 
 
 def test_unit_cases_reach_every_variant_key_of_the_model():
+    """At each SM count the unit cases, planned for that count, reach every key the model reaches there."""
+    report = []
+    for sms in T.SM_COUNTS:
+        model = {}
+        for backbone in ('resnet50', 'resnet18'):
+            for B in T.BATCHES:
+                for c in T.model_launches(backbone, B):
+                    p = T.plan(c, sms)
+                    if p is not None:
+                        model.setdefault(T.variant_key(c, p), f"{backbone} {c['name']} @ B={B}")
+        cases = {T.variant_key(c, T.plan(c, sms)) for c in T.ALL_CASES}
+        missing = {k: v for k, v in model.items() if k not in cases}
+        assert not missing, f'{len(missing)} variant key(s) at {sms} SMs without a unit case:\n' + \
+            '\n'.join(f'{dict(zip(T.KEY_FIELDS, k))}  (e.g. {v})' for k, v in missing.items())
+        report.append(f'{len(model)} at {sms} SMs')
+    print(f"forward: variant keys of the model {', '.join(report)}, all reached by the {len(T.ALL_CASES)} unit cases")
+
+
+def test_dgrad_cases_cover_every_data_gradient_kind_of_the_model():
     model = {}
-    for B in (1, 2, 3, 8, 32):
-        for c in T.model_launches(B):
-            p = T.plan(c)
-            if p is not None:
-                model.setdefault(T.variant_key(c, p), f"{c['name']} @ B={B}")
-    cases = {T.variant_key(c, T.plan(c)) for c in T.ALL_CASES}
-    missing = {k: v for k, v in model.items() if k not in cases}
-    assert not missing, '\n'.join(f'{dict(zip(T.KEY_FIELDS, k))}  (e.g. {v})' for k, v in missing.items())
-    print(f'{len(model)} variant keys of the model, all reached by the {len(T.ALL_CASES)} unit cases')
+    for backbone in ('resnet50', 'resnet18'):
+        for name, H, W, Ci, Co, k, st in T.conv_units(backbone):
+            if T.plan(T.dgrad_launch(name, 1, H, W, Ci, Co, k, st)) is not None:
+                model.setdefault(T.dgrad_kind(k, st, Ci, W), f'{backbone} {name}')
+    cases = set()
+    for B, Ci, H, W, Co, k, st in T.DGRAD_CASES:
+        assert T.plan(T.dgrad_launch('case', B, H, W, Ci, Co, k, st)) is not None, (B, Ci, H, W, Co, k, st)
+        cases.add(T.dgrad_kind(k, st, Ci, W))
+    missing = {kd: v for kd, v in model.items() if kd not in cases}
+    assert not missing, '\n'.join(f'k, stride, Cin > 256, W >= 128 = {kd}  (e.g. {v})' for kd, v in missing.items())
+    print(f'data gradient: {len(model)} unit kinds of the model, all reached by the {len(T.DGRAD_CASES)} cases')
 
 
 def test_unit_cases_include_the_named_variants():

@@ -45,14 +45,7 @@ def test_fp32_output_rejects_a_residual():
     assert rc != 0 and b'residual' in _lib.lib().hn_last_error()
 
 
-# B, Cin, H, W, Cout, k, stride: data gradients of the model's unit kinds
-DGRAD_CASES = [
-    (2, 64, 32, 128, 64, 3, (1, 1)),          # 3x3 stride 1 (layer1 conv2): dx reuse
-    (2, 128, 32, 64, 128, 3, (2, 2)),         # 3x3 stride 2 (layer2-4 .0.conv2): dilated dz
-    (2, 256, 32, 64, 512, 1, (2, 2)),         # 1x1 stride 2 (downsample)
-    (3, 256, 16, 64, 128, 3, (2, 1)),         # 3x3 stride (2, 1) (height reduction)
-    (2, 512, 16, 32, 128, 1, (1, 1)),         # 1x1 stride 1, Cin > 256 (conv1 of layer3)
-]
+DGRAD_CASES = tc_cases.DGRAD_CASES
 
 
 @pytest.mark.parametrize('dz_scale', [1.0, 1e-6, 1e-12])

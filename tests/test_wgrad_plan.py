@@ -14,6 +14,7 @@ import torch
 import __graft_entry__ as entry
 from horizonnet_b200 import _lib
 from tc_cases import resnet50_rnn_convs
+from wgrad_cases import check_plan, launch
 
 KT = 64
 
@@ -54,15 +55,7 @@ def _check_plan_covers_every_conv_unit(B, sms):
             continue
         assert p is not None, (name, _lib.lib().hn_last_error())
         on_tc += 1
-        Ho, Wo = H // st[0], W // st[1]
-        assert p['tw'] * p['rpt'] == KT and p['wsegs'] * p['tw'] == Wo, name
-        assert p['box_rows'] * p['imgs'] == p['rpt'], name           # rows of one image, or whole images
-        assert (p['imgs'] == 1 and Ho % p['rpt'] == 0) or (p['box_rows'] == Ho), name
-        rows = B * Ho
-        assert p['num_kt'] == -(-rows // p['rpt']) * p['wsegs'] and p['num_kt'] * KT >= rows * Wo, name
-        assert 1 <= p['kt_per_slice'] <= 64, name                    # <= 256 accumulation steps per register accumulator
-        assert (p['slices'] - 1) * p['kt_per_slice'] < p['num_kt'] <= p['slices'] * p['kt_per_slice'], name
-        assert p['items'] == -(-Co // 128) * -(-Ci // 128) * k * k and p['ctas'] == p['items'] * p['slices'], name
+        check_plan(launch(name, B, H, W, Ci, Co, k, st), p)
     assert on_tc == 67
 
 
