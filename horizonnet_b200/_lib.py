@@ -8,7 +8,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libhorizonnet_b200.so')
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 _lib = None
 _lock = threading.Lock()
@@ -47,6 +47,8 @@ SIGNATURES = {
     'hn_wgrad_tc_plan': (ctypes.c_int, [ctypes.c_int] * 12 + [c_int_p]),
     'hn_conv2d_dgrad_tc': (ctypes.c_int, [ctypes.c_int] * 4 + [vp, vp] + [ctypes.c_int] * 7 + [vp, vp]),
     'hn_conv_tc_plan': (ctypes.c_int, [ctypes.c_int] * 16 + [c_int_p]),
+    'hn_conv_f32_plan': (ctypes.c_int, [ctypes.c_int] * 14 + [c_int_p]),
+    'hn_wgrad_f32_plan': (ctypes.c_int, [ctypes.c_int] * 14 + [c_int_p]),
     'hn_conv_tc_fold_plan': (ctypes.c_int, [ctypes.c_int] * 8 + [c_int_p]),
     'hn_conv_tc_fold': (ctypes.c_int, [vp, vp] + [ctypes.c_int] * 7 + [vp, vp, vp, vp]),
     'hn_bott_tc': (ctypes.c_int, [vp] * 3 + [ctypes.c_int] * 3 + [vp] * 6 + [ctypes.c_int, vp, vp]),

@@ -958,28 +958,34 @@ int transpose_f32(const float* in, float* out, int rows, int cols, cudaStream_t 
     return 0;
 }
 
-int conv_wgrad_f32(const ConvDesc& d, const Act& in, const Act& dz, float* dw_ohwi, cudaStream_t st) {
+namespace {
+
+// Checks one weight gradient against what the fp32 kernels take and fills its geometry (no pointers, no GPU work).
+int conv_wgrad_f32_args(const ConvDesc& d, const Act& in, const Act& dz, WgradArgs* a) {
     HN_CHECK(in.C == d.Cin && dz.C == d.Cout && in.B == dz.B, "conv_wgrad: channel / batch mismatch");
     HN_CHECK(d.pw <= in.halo && d.Cout % 4 == 0, "conv_wgrad: circular pad wider than the input halo, or Cout % 4");
     const int Ho = (in.H + 2 * d.ph - d.kh) / d.sh + 1;
     const int Wo = (in.W + 2 * d.pw - d.kw) / d.sw + 1;
     HN_CHECK(Ho == dz.H && Wo == dz.W, "conv_wgrad: output geometry mismatch");
-    WgradArgs a;
-    a.in = in.p; a.dz = dz.p; a.dw = dw_ohwi;
-    a.B = in.B; a.H = in.H; a.Wp = in.Wp(); a.Cin = d.Cin;
-    a.Ho = Ho; a.Wo = Wo; a.Wop = dz.Wp(); a.Cout = d.Cout; a.out_halo = dz.halo;
-    a.kh = d.kh; a.kw = d.kw; a.sh = d.sh; a.sw = d.sw; a.ph = d.ph; a.woff = in.halo - d.pw;
+    a->B = in.B; a->H = in.H; a->Wp = in.Wp(); a->Cin = d.Cin;
+    a->Ho = Ho; a->Wo = Wo; a->Wop = dz.Wp(); a->Cout = d.Cout; a->out_halo = dz.halo;
+    a->kh = d.kh; a->kw = d.kw; a->sh = d.sh; a->sw = d.sw; a->ph = d.ph; a->woff = in.halo - d.pw;
     const long long M = (long long)in.B * Ho * Wo;
     HN_CHECK(M < (1ll << 31), "conv_wgrad: M overflows int");
-    a.M = (int)M; a.K = d.kh * d.kw * d.Cin;
-    HN_CUDA_OK(cudaMemsetAsync(dw_ohwi, 0, (size_t)d.Cout * a.K * sizeof(float), st));
-    if (a.M == 0) return 0;
-    const bool big = d.Cin % 4 == 0 && d.Cout >= 128 && a.K >= 128 && d.Cout % 4 == 0;
+    a->M = (int)M; a->K = d.kh * d.kw * d.Cin;
+    return 0;
+}
+
+// Kernel, grid and pixel slices for a->M pixels on `sms` SMs; sets a->m_per_slice.  plan = kernel (2 conv_wgrad128_kernel,
+// 1 conv_wgrad_kernel<VEC>, 0 conv_wgrad_kernel<scalar>), gx, gy, slices, m_per_slice.
+void conv_wgrad_f32_tiles(WgradArgs* a, int sms, int plan[5]) {
+    const long long M = a->M;
+    const bool big = a->Cin % 4 == 0 && a->Cout >= 128 && a->K >= 128 && a->Cout % 4 == 0;
     const int tile = big ? 128 : 64;
-    const int gx = (a.K + tile - 1) / tile, gy = (d.Cout + tile - 1) / tile;
+    const int gx = (a->K + tile - 1) / tile, gy = (a->Cout + tile - 1) / tile;
     // pixel slices: the CTAs of a launch all do the same amount of work, so pick the slice count whose CTA total fills
     // whole waves of the resident slots best (ncu: 320 CTAs on 296 slots left the SMs idle a third of the time)
-    const long long tiles = (long long)gx * gy, slots = (long long)num_sms() * (big ? 2 : 4);
+    const long long tiles = (long long)gx * gy, slots = (long long)sms * (big ? 2 : 4);
     long long max_slices = (M + 255) / 256;                        // at least 256 pixels per slice
     if (max_slices > 64) max_slices = 64;
     long long slices = 1;
@@ -989,11 +995,34 @@ int conv_wgrad_f32(const ConvDesc& d, const Act& in, const Act& dz, float* dw_oh
         const double fill = (double)total / (double)(waves * slots);
         if (fill > best + 0.02) { best = fill; slices = s; }       // more slices only for a real gain (more atomics)
     }
-    a.m_per_slice = (int)(((M + slices - 1) / slices + 15) / 16 * 16);
-    slices = (M + a.m_per_slice - 1) / a.m_per_slice;
-    dim3 grid((unsigned)gx, (unsigned)gy, (unsigned)slices);
-    if (big) conv_wgrad128_kernel<<<grid, 256, 0, st>>>(a);
-    else if (d.Cin % 4 == 0) conv_wgrad_kernel<true><<<grid, 256, 0, st>>>(a);
+    a->m_per_slice = (int)(((M + slices - 1) / slices + 15) / 16 * 16);
+    slices = (M + a->m_per_slice - 1) / a->m_per_slice;
+    plan[0] = big ? 2 : (a->Cin % 4 == 0 ? 1 : 0);
+    plan[1] = gx; plan[2] = gy; plan[3] = (int)slices; plan[4] = a->m_per_slice;
+}
+
+}  // namespace
+
+int conv_wgrad_f32_plan(const ConvDesc& d, const Act& in, const Act& dz, int sms, int plan[5]) {
+    HN_CHECK(sms >= 1, "conv_wgrad_f32_plan: sms must be positive");
+    WgradArgs a;
+    if (conv_wgrad_f32_args(d, in, dz, &a)) return -1;
+    HN_CHECK(a.M > 0, "conv_wgrad_f32_plan: no pixels");
+    conv_wgrad_f32_tiles(&a, sms, plan);
+    return 0;
+}
+
+int conv_wgrad_f32(const ConvDesc& d, const Act& in, const Act& dz, float* dw_ohwi, cudaStream_t st) {
+    WgradArgs a;
+    if (conv_wgrad_f32_args(d, in, dz, &a)) return -1;
+    a.in = in.p; a.dz = dz.p; a.dw = dw_ohwi;
+    HN_CUDA_OK(cudaMemsetAsync(dw_ohwi, 0, (size_t)d.Cout * a.K * sizeof(float), st));
+    if (a.M == 0) return 0;
+    int p[5];
+    conv_wgrad_f32_tiles(&a, num_sms(), p);
+    dim3 grid((unsigned)p[1], (unsigned)p[2], (unsigned)p[3]);
+    if (p[0] == 2) conv_wgrad128_kernel<<<grid, 256, 0, st>>>(a);
+    else if (p[0] == 1) conv_wgrad_kernel<true><<<grid, 256, 0, st>>>(a);
     else conv_wgrad_kernel<false><<<grid, 256, 0, st>>>(a);
     HN_LAUNCH_OK();
     return 0;

@@ -16,6 +16,9 @@ int dilate_for_dgrad(const Act& dz, const Act& out, int sh, int sw, cudaStream_t
 
 // dW[Cout][kh][kw][Cin] (zeroed here, then accumulated); in = the conv's forward input, dz = d(raw conv output)
 int conv_wgrad_f32(const ConvDesc& d, const Act& in, const Act& dz, float* dw_ohwi, cudaStream_t st);
+// Its launch plan on `sms` SMs (host only): plan = kernel (2: 128 x 128 tiles, 1: 64 x 64 with 16-byte input loads, 0: 64 x 64
+// scalar, Cin % 4 != 0), grid x (K tiles), grid y (Cout tiles), pixel slices, pixels per slice; -1 for a shape it rejects
+int conv_wgrad_f32_plan(const ConvDesc& d, const Act& in, const Act& dz, int sms, int plan[5]);
 // The same product on tensor-core (wgrad_tc.cu) from the split planes of the input and of dz (split_planes_pow2; dz_absmax =
 // the float it left behind): Cin, Cout multiples of 64, halo 0 or 1, strides 1 or 2.  The training step's wgrad runs it
 // wherever option tensor_cores is on and conv_wgrad_tc_supported takes the shape, and conv_wgrad_f32 everywhere else.

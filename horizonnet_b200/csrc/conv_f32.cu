@@ -184,9 +184,8 @@ __global__ void __launch_bounds__(256) conv_igemm_f32(const ConvArgs a) {
     }
 }
 
-}  // namespace
-
-int conv_f32(const ConvDesc& d, const Act& in, const Act& out, const float* residual, cudaStream_t st) {
+// Checks one convolution against what conv_igemm_f32 takes and fills its geometry (no pointers, no GPU work).
+int conv_f32_args(const ConvDesc& d, const Act& in, const Act& out, ConvArgs* a) {
     HN_CHECK(in.C == d.Cin && out.C == d.Cout, "conv_f32: channel mismatch");
     HN_CHECK(d.Cin % BK == 0 && d.Cout % 4 == 0, "conv_f32: Cin must be a multiple of 16, Cout of 4");
     HN_CHECK(d.pw <= in.halo, "conv_f32: circular pad wider than the input halo");
@@ -194,28 +193,46 @@ int conv_f32(const ConvDesc& d, const Act& in, const Act& out, const float* resi
     const int Ho = (in.H + 2 * d.ph - d.kh) / d.sh + 1;
     const int Wo = (in.W + 2 * d.pw - d.kw) / d.sw + 1;
     HN_CHECK(Ho == out.H && Wo == out.W && in.B == out.B, "conv_f32: output geometry mismatch");
-    ConvArgs a;
-    a.in = in.p; a.out = out.p; a.res = residual; a.w = d.w; a.scale = d.scale; a.shift = d.shift;
-    a.B = in.B; a.H = in.H; a.Wp = in.Wp(); a.Cin = d.Cin;
-    a.Ho = Ho; a.Wo = Wo; a.Wop = out.Wp(); a.Cout = d.Cout; a.out_halo = out.halo;
-    a.kh = d.kh; a.kw = d.kw; a.sh = d.sh; a.sw = d.sw; a.ph = d.ph; a.woff = in.halo - d.pw;
-    a.relu = d.relu;
+    a->B = in.B; a->H = in.H; a->Wp = in.Wp(); a->Cin = d.Cin;
+    a->Ho = Ho; a->Wo = Wo; a->Wop = out.Wp(); a->Cout = d.Cout; a->out_halo = out.halo;
+    a->kh = d.kh; a->kw = d.kw; a->sh = d.sh; a->sw = d.sw; a->ph = d.ph; a->woff = in.halo - d.pw;
+    a->relu = d.relu;
     const long long M = (long long)in.B * Ho * Wo;
     HN_CHECK(M < (1ll << 31), "conv_f32: M overflows int");
-    a.M = (int)M; a.K = d.kh * d.kw * d.Cin;
+    a->M = (int)M; a->K = d.kh * d.kw * d.Cin;
+    return 0;
+}
+
+// Tile choice: big tiles when they still fill the SMs, else 64x64.  plan = BM, BN, grid_m, grid_n.
+void conv_f32_tiles(long long M, int Cout, int sms, int plan[4]) {
+    const long long big = ((M + 127) / 128) * ((Cout + 127) / 128);
+    int bm = 64, bn = 64;
+    if (Cout >= 128 && big >= sms) bm = bn = 128;
+    else if (Cout <= 64 && (M + 127) / 128 >= sms) bm = 128;
+    plan[0] = bm; plan[1] = bn; plan[2] = (int)((M + bm - 1) / bm); plan[3] = (Cout + bn - 1) / bn;
+}
+
+}  // namespace
+
+int conv_f32_plan(const ConvDesc& d, const Act& in, const Act& out, int sms, int plan[4]) {
+    HN_CHECK(sms >= 1, "conv_f32_plan: sms must be positive");
+    ConvArgs a;
+    if (conv_f32_args(d, in, out, &a)) return -1;
+    conv_f32_tiles(a.M, d.Cout, sms, plan);
+    return 0;
+}
+
+int conv_f32(const ConvDesc& d, const Act& in, const Act& out, const float* residual, cudaStream_t st) {
+    ConvArgs a;
+    if (conv_f32_args(d, in, out, &a)) return -1;
+    a.in = in.p; a.out = out.p; a.res = residual; a.w = d.w; a.scale = d.scale; a.shift = d.shift;
     if (a.M == 0) return 0;
-    // tile choice: big tiles when they still fill the SMs, else 64x64
-    const long long big = ((M + 127) / 128) * ((d.Cout + 127) / 128);
-    if (d.Cout >= 128 && big >= num_sms()) {
-        dim3 g((unsigned)((M + 127) / 128), (unsigned)((d.Cout + 127) / 128));
-        conv_igemm_f32<128, 128><<<g, 256, 0, st>>>(a);
-    } else if (d.Cout <= 64 && (M + 127) / 128 >= num_sms()) {
-        dim3 g((unsigned)((M + 127) / 128), (unsigned)((d.Cout + 63) / 64));
-        conv_igemm_f32<128, 64><<<g, 256, 0, st>>>(a);
-    } else {
-        dim3 g((unsigned)((M + 63) / 64), (unsigned)((d.Cout + 63) / 64));
-        conv_igemm_f32<64, 64><<<g, 256, 0, st>>>(a);
-    }
+    int p[4];
+    conv_f32_tiles(a.M, d.Cout, num_sms(), p);
+    const dim3 g((unsigned)p[2], (unsigned)p[3]);
+    if (p[0] == 128 && p[1] == 128) conv_igemm_f32<128, 128><<<g, 256, 0, st>>>(a);
+    else if (p[0] == 128) conv_igemm_f32<128, 64><<<g, 256, 0, st>>>(a);
+    else conv_igemm_f32<64, 64><<<g, 256, 0, st>>>(a);
     HN_LAUNCH_OK();
     return 0;
 }

@@ -75,6 +75,8 @@ struct ConvDesc {
 };
 
 int conv_f32(const ConvDesc& d, const Act& in, const Act& out, const float* residual, cudaStream_t st);
+// The tile plan conv_f32 launches with on `sms` SMs (host only): plan = BM, BN, grid_m, grid_n; -1 for a shape it rejects
+int conv_f32_plan(const ConvDesc& d, const Act& in, const Act& out, int sms, int plan[4]);
 int stem_f32(const float* x_nchw, int B, int in_channels, const float* w_packed, const float* scale,
              const float* shift, const Act& out, cudaStream_t st, bool relu = true);
 int maxpool3x3s2(const Act& in, const Act& out, cudaStream_t st, bool out_split = false);

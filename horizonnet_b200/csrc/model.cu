@@ -317,7 +317,7 @@ int refold_bn(hn_model* m, cudaStream_t st) {
 extern "C" {
 
 const char* hn_last_error(void) { return g_err.c_str(); }
-int hn_abi_version(void) { return 8; }
+int hn_abi_version(void) { return 9; }
 const char* hn_build_digest(void) { return HN_BUILD_DIGEST; }
 long long hn_kernel_launches(void) { return g_launches.load(); }
 
@@ -1145,6 +1145,19 @@ int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh,
                        p.dxr, p.parity, p.num_kc, p.seg, p.pf, p.n_tiles, p.num_tiles, p.grid};
     memcpy(plan, v, sizeof(v));
     return 0;
+}
+
+// Tile plan of the fp32 CUDA-core convolution for one shape (no GPU work): the one conv_f32 launches with.
+int hn_conv_f32_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
+                     int out_halo, int sms, int plan[4]) {
+    HN_CHECK(plan, "hn_conv_f32_plan: NULL argument");
+    HN_CHECK(B >= 1 && H >= 1 && W >= 1 && kh >= 1 && kw >= 1 && sh >= 1 && sw >= 1 && in_halo >= 0 && out_halo >= 0,
+             "hn_conv_f32_plan: bad geometry");
+    ConvDesc d;
+    d.Cin = Cin; d.Cout = Cout; d.kh = kh; d.kw = kw; d.sh = sh; d.sw = sw; d.ph = ph; d.pw = pw;
+    const Act a = mk(nullptr, B, H, W, Cin, in_halo);
+    const Act o = mk(nullptr, B, (H + 2 * ph - kh) / sh + 1, (W + 2 * pw - kw) / sw + 1, Cout, out_halo);
+    return conv_f32_plan(d, a, o, sms, plan);
 }
 
 int hn_conv_tc_fold_plan(int B, int H, int W, int Cin, int Cmid, int Cout, int stride, int sms, int plan[18]) {

@@ -739,6 +739,20 @@ int hn_wgrad_tc_plan(int B, int H, int W, int Cin, int Cout, int kh, int kw, int
     return conv_wgrad_tc_plan(d, a, z, sms, plan);
 }
 
+// Launch plan of the fp32 CUDA-core weight gradient (conv_wgrad_f32) for one shape (no GPU work): plan[5] = kernel, grid x,
+// grid y, pixel slices, pixels per slice.  -1 for a shape it does not take.
+int hn_wgrad_f32_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
+                      int out_halo, int sms, int plan[5]) {
+    HN_CHECK(plan, "hn_wgrad_f32_plan: NULL argument");
+    HN_CHECK(B >= 1 && H >= 1 && W >= 1 && kh >= 1 && kw >= 1 && sh >= 1 && sw >= 1 && in_halo >= 0 && out_halo >= 0,
+             "hn_wgrad_f32_plan: bad geometry");
+    ConvDesc d;
+    d.Cin = Cin; d.Cout = Cout; d.kh = kh; d.kw = kw; d.sh = sh; d.sw = sw; d.ph = ph; d.pw = pw;
+    const Act a = mk(nullptr, B, H, W, Cin, in_halo);
+    const Act z = mk(nullptr, B, (H + 2 * ph - kh) / sh + 1, (W + 2 * pw - kw) / sw + 1, Cout, out_halo);
+    return conv_wgrad_f32_plan(d, a, z, sms, plan);
+}
+
 // 1: the training step runs its weight gradients on the tensor-core kernel wherever option tensor_cores is on and the shape fits
 int hn_wgrad_tc_enabled(void) { return 1; }
 

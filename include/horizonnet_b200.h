@@ -257,6 +257,12 @@ int hn_conv2d_wgrad_tc(const float* in, int B, int H, int W, int Cin, const floa
  * tile, tiles per row, box rows, images per tile, pixel tiles (64 pixels each), tiles per slice, slices, work items per slice,
  * CTAs.  -1 for a shape the kernel does not take. */
 int hn_wgrad_tc_plan(int B, int H, int W, int Cin, int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int sms, int plan[10]);
+/* Host-side plan of the fp32 CUDA-core weight gradient (hn_conv2d_backward; the training step's weight gradients the
+ * tensor-core kernel does not take) for one shape (no GPU work; sms = SM count to plan for; dz has out_halo): plan[5] =
+ * kernel (2: 128 x 128 tiles, 1: 64 x 64 with 16-byte input loads, 0: 64 x 64 scalar loads for Cin % 4 != 0), K tiles,
+ * Cout tiles, pixel slices, pixels per slice.  -1 for a shape it does not take. */
+int hn_wgrad_f32_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
+                      int out_halo, int sms, int plan[5]);
 /* Returns 1: the training step runs the weight gradients on that kernel wherever option "tensor_cores" is on and the shape fits. */
 int hn_wgrad_tc_enabled(void);
 /* The data gradient on the tensor cores exactly as the training step computes it (zero-dilated dz for a strided conv,
@@ -273,6 +279,11 @@ int hn_conv2d_dgrad_tc(int B, int H, int W, int Cin, const float* w_oihw, const 
  * CTAs.  -1 for a shape the kernel does not take. */
 int hn_conv_tc_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
                     int out_halo, int out_f32, int has_residual, int sms, int plan[18]);
+/* Host-side tile plan of the fp32 CUDA-core convolution (hn_conv2d impl 0; no GPU work; sms = SM count to plan for):
+ * plan[4] = output pixels per tile (BM), output channels per tile (BN), tiles along the pixels, tiles along Cout.
+ * -1 for a shape that kernel does not take. */
+int hn_conv_f32_plan(int B, int H, int W, int Cin, int in_halo, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
+                     int out_halo, int sms, int plan[4]);
 /* The same plan (same 18 fields) for the eval-mode conv3 of a bottleneck's block 0 with its downsample folded in:
  * relu([t2 | x at every stride-th pixel] . W + shift), x [B][H][W][Cin] (halo 1), t2 and the output [B][H/s][W/s][Cmid],
  * [Cout]; K chunks = (Cmid + Cin) / 64, the first Cmid / 64 over t2.  -1 for a shape the kernel does not take. */

@@ -301,6 +301,184 @@ def run_wgrad_case(c, zero_dz=False, with_fp32=False, dev='cuda:0'):
     return ratio, _worst_ratio(got32 - ref, bound)
 
 
+# ---- elementwise error bound of the fp32 CUDA-core kernels (conv_f32.cu, conv_wgrad_f32): every product a*w is exact to
+# 2^-24 and the fp32 sums add 2^-24 of a partial sum per step, so the error of an output is a multiple of 2^-24 of the
+# magnitude sum sum|a*w| of its terms, times |scale|, plus the epilogue's roundings of shift, residual and the result:
+#   C32 * 2^-24 * (sum|a*w| * |scale| + |shift| + |res|) + 2^-24 * |ref|.
+# C32 = 48 is 3x the worst err / (2^-24 * magnitude sum) measured over the unit cases of tests/f32_cases.py on an H100 SXM
+# (132 SMs, 700 W): 16, a data gradient on 128 x 128 tiles, where one dz channel at scale 1 dominates K = 1152 terms and
+# each later step rounds at that magnitude (sqrt(K) growth, far below the K of the worst case); the forward convolutions
+# reach 10, the weight gradients 4.  A term left out, or added twice, is worth about 2^24 / C32 bounds.
+C32 = 48.0
+EPS24 = 2.0 ** -24
+
+
+def f32_case_inputs(shape, kind, g):
+    """An input operand like the model's: 'act' post-ReLU (about half zeros), 'lstm' an LSTM state in (-1, 1), 'grad' a
+    signed gradient with per-channel scales spread over 2^-20 .. 1 (dim 1 = channels)."""
+    if kind == 'act':
+        return torch.relu(torch.randn(*shape, generator=g))
+    if kind == 'lstm':
+        return torch.rand(*shape, generator=g) * 2 - 1
+    s = 2.0 ** (-20 * torch.rand(shape[1], generator=g))
+    s[0] = 1.0
+    return torch.randn(*shape, generator=g) * s.view(1, -1, *([1] * (len(shape) - 2)))
+
+
+def _seed(name):
+    return int(hashlib.sha1(name.encode()).hexdigest()[:8], 16)
+
+
+def _nan_buffer(n, dev):
+    buf = torch.full((n + 4096,), float('nan'), device=dev)
+    buf[n:] = CANARY
+    return buf
+
+
+def _check_output(name, buf, n, out, halo):
+    assert not torch.isnan(out).any(), f'{name}: output elements left unwritten'
+    assert bool((buf[n:] == CANARY).all()), f'{name}: write past the end of the output'
+    if halo:
+        assert torch.equal(out[:, :, 0], out[:, :, -2]) and torch.equal(out[:, :, -1], out[:, :, 1]), \
+            f'{name}: halo columns are not the circular wrap'
+
+
+def run_f32_conv(c, dev='cuda:0'):
+    """One 'conv' case of tests/f32_cases.py through hn_conv2d impl 0 (conv_f32) against fp64, elementwise.  The output
+    starts NaN-filled with a canary behind it; residual 'inplace' passes the output buffer itself as the residual, filled
+    with a random tensor first (halo columns wrapped).  Returns worst err / bound."""
+    g = torch.Generator().manual_seed(_seed(c['name']))
+    B, Ci, H, W, Co, k = c['B'], c['Cin'], c['H'], c['W'], c['Cout'], c['k']
+    (sh, sw), ph, pw, hi, ho = c['stride'], c['ph'], c['pw'], c['in_halo'], c['out_halo']
+    Ho, Wo = (H + 2 * ph - k) // sh + 1, (W + 2 * pw - k) // sw + 1
+    x = f32_case_inputs((B, Ci, H, W), c['kind'], g)
+    w = torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5
+    scale, shift = torch.rand(Co, generator=g) + 0.5, torch.randn(Co, generator=g) * 0.1
+    res = torch.randn(B, Co, Ho, Wo, generator=g) if c['residual'] != 'none' else None
+    x, w, scale, shift = x.to(dev), w.to(dev), scale.to(dev), shift.to(dev)
+    res = res.to(dev) if res is not None else None
+    n = B * Ho * (Wo + 2 * ho) * Co
+    buf = _nan_buffer(n, dev)
+    out = buf[:n].view(B, Ho, Wo + 2 * ho, Co)
+    resin = None
+    if c['residual'] == 'separate':
+        resin = to_halo_nhwc(res, ho)
+    elif c['residual'] == 'inplace':
+        out.copy_(to_halo_nhwc(res, ho))
+        resin = out
+    xin, wp = to_halo_nhwc(x, hi), pack_weight(w)
+    rc = _lib.lib().hn_conv2d(xin.data_ptr(), B, H, W, Ci, hi, wp.data_ptr(), scale.data_ptr(), shift.data_ptr(),
+                              resin.data_ptr() if resin is not None else None, Co, k, k, sh, sw, ph, pw, int(c['relu']),
+                              out.data_ptr(), ho, 0, torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(rc, 'hn_conv2d')
+    torch.cuda.synchronize(dev)
+    _check_output(c['name'], buf, n, out, ho)
+    y = from_halo_nhwc(out, ho).double()
+    xd, wd = x.double(), w.double()
+    rd = res.double() if res is not None else None
+    ref = conv2d_reference(xd, wd, scale, shift, (sh, sw), ph, pw, c['relu'], rd)
+    acc = _conv_abs(xd.abs(), wd.abs(), (sh, sw), ph, pw)
+    bound = C32 * EPS24 * (acc * scale.double().abs().view(1, -1, 1, 1) + shift.double().abs().view(1, -1, 1, 1)) + \
+        EPS24 * ref.abs()
+    if rd is not None:
+        bound = bound + C32 * EPS24 * rd.abs()
+    return _worst_ratio(y - ref, bound)
+
+
+def _grad_inputs(x, w, dz, stride, ph, pw):
+    """(din, dW) of the circular-W, zero-H-padded convolution by autograd in the inputs' dtype."""
+    xv, wv = x.clone().requires_grad_(), w.clone().requires_grad_()
+    if pw:
+        xp = torch.cat([xv[..., -pw:], xv, xv[..., :pw]], dim=3)
+    else:
+        xp = xv
+    F.conv2d(xp, wv, None, stride=stride, padding=(ph, 0)).backward(dz)
+    return xv.grad, wv.grad
+
+
+def run_f32_backward(c, zero_dz=False, dev='cuda:0'):
+    """One 'wgrad' or 'dgrad' case of tests/f32_cases.py against fp64, elementwise, under the bound of run_f32_conv with
+    scale 1 and no shift.
+    * wgrad: hn_conv2d_backward's weight gradient (conv_wgrad_f32) with the input in the case's halo;
+    * dgrad: hn_conv2d_backward's data gradient (pack_dgrad_weight, the zero dilation of dz, conv_f32 over it into a fresh
+      din), and the same transposed conv through hn_conv2d impl 0 accumulated in place into a prefilled din, as the
+      training step runs it (the dilated dz and flipped weights built here).  A unit whose Cout is not a multiple of 16
+      runs as the training step pads it: Cout rounded up to 16 with zero weight rows and zero dz channels, against the
+      unpadded conv's gradient.
+    The outputs start NaN-filled with a canary behind them.  zero_dz: dz = 0 must give exactly 0 (dgrad: exactly the
+    prefill).  Returns worst err / bound."""
+    g = torch.Generator().manual_seed(_seed(c['name']))
+    B, Ci, H, W, Co, k = c['B'], c['Cin'], c['H'], c['W'], c['Cout'], c['k']
+    (sh, sw), ph, pw = c['stride'], c['ph'], c['pw']
+    Ho, Wo = (H + 2 * ph - k) // sh + 1, (W + 2 * pw - k) // sw + 1
+    lib, st = _lib.lib(), torch.cuda.current_stream(dev).cuda_stream
+    x = f32_case_inputs((B, Ci, H, W), c['kind'] if c['op'] == 'wgrad' else 'act', g).to(dev)
+    w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(dev)
+    dz = f32_case_inputs((B, Co, Ho, Wo), 'grad', g).to(dev)
+    if zero_dz:
+        dz.zero_()
+    xd, wd, dzd = x.double(), w.double(), dz.double()
+    if c['op'] == 'wgrad':
+        hi = c['in_halo']
+        n = Co * Ci * k * k
+        buf = _nan_buffer(n, dev)
+        xin, dzin = to_halo_nhwc(x, hi), to_halo_nhwc(dz, 1)          # (kept alive until the kernels have run)
+        rc = lib.hn_conv2d_backward(xin.data_ptr(), B, H, W, Ci, hi, w.data_ptr(), dzin.data_ptr(), Co, k, k, sh, sw, ph,
+                                    pw, None, buf.data_ptr(), st)
+        _lib.check(rc, 'hn_conv2d_backward')
+        torch.cuda.synchronize(dev)
+        dw = buf[:n].view(Co, Ci, k, k)
+        _check_output(c['name'], buf, n, dw, 0)
+        if zero_dz:
+            assert torch.equal(dw, torch.zeros_like(dw)), f"{c['name']}: an all-zero dz must give dW = 0 exactly"
+            return 0.0
+        ref = _grad_inputs(xd, wd, dzd, (sh, sw), ph, pw)[1]
+        acc = _grad_inputs(xd.abs(), wd, dzd.abs(), (sh, sw), ph, pw)[1]
+        return _worst_ratio(dw.double() - ref, C32 * EPS24 * acc + EPS24 * ref.abs())
+    # data gradient: Cout padded to 16 as walk_backward does
+    cp = -(-Co // 16) * 16
+    wpd = torch.cat([w, torch.zeros(cp - Co, Ci, k, k, device=dev)]) if cp != Co else w
+    dzp = torch.cat([dz, torch.zeros(B, cp - Co, Ho, Wo, device=dev)], dim=1) if cp != Co else dz
+    dzin = to_halo_nhwc(dzp, 1)
+    n = B * H * (W + 2) * Ci
+    buf = _nan_buffer(n, dev)
+    dwbuf = torch.empty(cp * Ci * k * k, device=dev)
+    xin = to_halo_nhwc(x, 1)
+    rc = lib.hn_conv2d_backward(xin.data_ptr(), B, H, W, Ci, 1, wpd.data_ptr(), dzin.data_ptr(), cp, k, k,
+                                sh, sw, ph, pw, buf.data_ptr(), dwbuf.data_ptr(), st)
+    _lib.check(rc, 'hn_conv2d_backward')
+    torch.cuda.synchronize(dev)
+    din = buf[:n].view(B, H, W + 2, Ci)
+    _check_output(c['name'], buf, n, din, 1)
+    # in place: din += conv(dilate(dz), flip(W)) on conv_f32 with the output as its residual
+    pre = torch.randn(B, Ci, H, W, generator=g).to(dev)
+    buf2 = _nan_buffer(n, dev)
+    acc_out = buf2[:n].view(B, H, W + 2, Ci)
+    acc_out.copy_(to_halo_nhwc(pre, 1))
+    dil = torch.zeros(B, cp, H, W, device=dev)
+    dil[:, :, ::sh, ::sw] = dzp
+    wt = wpd.transpose(0, 1).flip(2, 3)
+    ones, zeros = torch.ones(Ci, device=dev), torch.zeros(Ci, device=dev)
+    tph, tpw = k - 1 - ph, k - 1 - pw
+    dilin, wtp = to_halo_nhwc(dil, 1), pack_weight(wt)
+    rc = lib.hn_conv2d(dilin.data_ptr(), B, H, W, cp, 1, wtp.data_ptr(), ones.data_ptr(),
+                       zeros.data_ptr(), acc_out.data_ptr(), Ci, k, k, 1, 1, tph, tpw, 0, acc_out.data_ptr(), 1, 0, st)
+    _lib.check(rc, 'hn_conv2d')
+    torch.cuda.synchronize(dev)
+    _check_output(c['name'], buf2, n, acc_out, 1)
+    got, got_acc = from_halo_nhwc(din, 1).double(), from_halo_nhwc(acc_out, 1).double()
+    pred = pre.double()
+    if zero_dz:
+        assert torch.equal(got, torch.zeros_like(got)), f"{c['name']}: an all-zero dz must give din = 0 exactly"
+        assert torch.equal(got_acc, pred), f"{c['name']}: an all-zero dz must leave din exactly as it was"
+        return 0.0
+    ref = _grad_inputs(xd, wd, dzd, (sh, sw), ph, pw)[0]
+    acc = _grad_inputs(xd, wd.abs(), dzd.abs(), (sh, sw), ph, pw)[0]
+    bound = C32 * EPS24 * acc + EPS24 * ref.abs()
+    return max(_worst_ratio(got - ref, bound),
+               _worst_ratio(got_acc - (pred + ref), bound + C32 * EPS24 * pred.abs() + EPS24 * (pred + ref).abs()))
+
+
 def device_sms(dev=0):
     return torch.cuda.get_device_properties(dev).multi_processor_count
 
