@@ -8,7 +8,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libhorizonnet_b200.so')
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 _lib = None
 _lock = threading.Lock()
@@ -87,6 +87,7 @@ SIGNATURES = {
     'hn_conv2d': (ctypes.c_int, [vp] + [ctypes.c_int] * 5 + [vp, vp, vp, vp] + [ctypes.c_int] * 8 +
                   [vp, ctypes.c_int, ctypes.c_int, vp]),
     'hn_lstm_layer': (ctypes.c_int, [vp, vp, vp, vp, ctypes.c_int, ctypes.c_int, vp]),
+    'hn_lstm_plan': (ctypes.c_int, [ctypes.c_int] * 3 + [c_int_p]),
 }
 
 

@@ -22,7 +22,7 @@
 //   groups  = one or two column groups of 8 per cluster, interleaved step by step (each group has its own exchange
 //             buffers and barriers): while one group's h is in flight between the CTAs the other group's MMAs run.
 //             Two groups per cluster when one group each would not fit in one wave of co-resident clusters (see
-//             lstm_layer): the batch-32 recurrence then takes 4 clusters = 64 of the 132 SMs and leaves the
+//             lstm_plan): the batch-32 recurrence then takes 4 clusters = 64 of the 132 SMs and leaves the
 //             rest to the next batch's encoder.  Clusters beyond what the device co-schedules run in a later wave.
 //   grid    = 2 directions x ceil(B/8) clusters, or 2 directions x ceil(B/16) with two groups per cluster.
 #include <cuda_fp16.h>
@@ -286,10 +286,9 @@ __global__ void __launch_bounds__(NT, 1) lstm_cluster_kernel(const ClArgs a) {
 
 }  // namespace
 
-// One LSTM layer, both directions, on 16-CTA clusters; xproj [T][B][4096], out [T][B][1024].  Returns 0 on success,
-// -1 on error, including a device that cannot co-schedule two such clusters.
-int lstm_layer(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, float* out, int T, int B,
-               cudaStream_t st) {
+// How many of the recurrence's 16-CTA clusters the current device co-schedules (cudaOccupancyMaxActiveClusters, cached
+// per device); -1 on error.
+static int lstm_max_clusters() {
     // function attributes are per device: set them on every call (cheap); the occupancy answer is cached per device
     int dev = 0;
     HN_CUDA_OK(cudaGetDevice(&dev));
@@ -321,18 +320,43 @@ int lstm_layer(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd,
         if (const char* e = getenv("HN_LSTM_VERBOSE"))
             if (atoi(e)) fprintf(stderr, "lstm_cluster: device %d: max active 16-CTA clusters = %d\n", dev, max_clusters);
     }
+    return max_clusters;
+}
+
+int lstm_plan(int T, int B, int max_clusters, int plan[7]) {
+    HN_CHECK(T >= 1 && B >= 1, "lstm_plan: T and B must be positive");
+    if (max_clusters <= 0 && (max_clusters = lstm_max_clusters()) < 0) return -1;
     if (max_clusters < 2)
-        return fail("lstm_layer: not supported on device " + std::to_string(dev) + ": it co-schedules " +
-                    std::to_string(max_clusters) + " of the recurrence's 16-CTA clusters, 2 are needed");
-    ClArgs a;
-    a.xproj = xproj; a.w_hh[0] = w_hh_fwd; a.w_hh[1] = w_hh_bwd; a.out = out;
-    a.T = T; a.B = B; a.ngroups = (B + NCOL - 1) / NCOL;
+        return fail("lstm_layer: not supported: the device co-schedules " + std::to_string(max_clusters) +
+                    " of the recurrence's 16-CTA clusters, 2 are needed");
+    const int ngroups = (B + NCOL - 1) / NCOL;
     // One group per cluster when every cluster fits in one wave: a second group makes a cluster about 1.7x slower
     // (T = 256, kernel time on an H100 at 700 W: 0.71 ms with one group per cluster, 1.20 ms with two).  Two groups
     // per cluster when one group each would need a second wave: batch 32 on the 7 co-resident clusters of that H100
     // then runs on 4 clusters in one wave instead of 8 in two, and leaves 68 SMs to the other stream.
-    a.gpc = (2 * a.ngroups <= max_clusters) ? 1 : MAXG;
-    const int nclusters = 2 * ((a.ngroups + a.gpc - 1) / a.gpc);
+    const int gpc = (2 * ngroups <= max_clusters) ? 1 : MAXG;
+    const int per_dir = (ngroups + gpc - 1) / gpc;
+    plan[0] = max_clusters;
+    plan[1] = ngroups;
+    plan[2] = gpc;
+    plan[3] = 2 * per_dir;
+    plan[4] = ngroups - (per_dir - 1) * gpc;
+    plan[5] = B - (ngroups - 1) * NCOL;
+    plan[6] = (plan[3] + max_clusters - 1) / max_clusters;
+    return 0;
+}
+
+// One LSTM layer, both directions, on 16-CTA clusters; xproj [T][B][4096], out [T][B][1024].  Returns 0 on success,
+// -1 on error, including a device that cannot co-schedule two such clusters.
+int lstm_layer(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, float* out, int T, int B,
+               cudaStream_t st) {
+    int plan[7];
+    if (lstm_plan(T, B, 0, plan)) return -1;          // also sets the kernel's function attributes on this device
+    ClArgs a;
+    a.xproj = xproj; a.w_hh[0] = w_hh_fwd; a.w_hh[1] = w_hh_bwd; a.out = out;
+    a.T = T; a.B = B; a.ngroups = plan[1];
+    a.gpc = plan[2];
+    const int nclusters = plan[3];
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(nclusters * CL);
     cfg.blockDim = dim3(NT);

@@ -317,7 +317,7 @@ int refold_bn(hn_model* m, cudaStream_t st) {
 extern "C" {
 
 const char* hn_last_error(void) { return g_err.c_str(); }
-int hn_abi_version(void) { return 9; }
+int hn_abi_version(void) { return 10; }
 const char* hn_build_digest(void) { return HN_BUILD_DIGEST; }
 long long hn_kernel_launches(void) { return g_launches.load(); }
 
@@ -1197,6 +1197,12 @@ int hn_bott_tc(const float* in, const float* res, const float* x, int B, int H, 
 int hn_lstm_layer(const float* xproj, const float* whf, const float* whb, float* out, int T, int B, void* stream) {
     HN_CHECK(xproj && whf && whb && out && T >= 1 && B >= 1, "hn_lstm_layer: bad argument");
     return lstm_layer(xproj, whf, whb, out, T, B, (cudaStream_t)stream);
+}
+
+// Launch layout of hn_lstm_layer (no GPU work unless max_clusters <= 0 asks the current device): the one lstm_layer takes.
+int hn_lstm_plan(int T, int B, int max_clusters, int plan[7]) {
+    HN_CHECK(plan, "hn_lstm_plan: NULL argument");
+    return lstm_plan(T, B, max_clusters, plan);
 }
 
 }  // extern "C"

@@ -25,6 +25,11 @@ int linear_head(const float* rnn, const float* w, const float* bias, float* bon,
                 cudaStream_t st);
 int lstm_layer(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, float* out, int T, int B,
                cudaStream_t st);
+// The launch layout lstm_layer takes for T steps of B columns when the device co-schedules max_clusters of its 16-CTA
+// clusters (<= 0: ask the current device, as lstm_layer does): plan = max_clusters, column groups, groups per cluster,
+// clusters (both directions), groups in the last cluster, columns in the last group, waves.  No GPU work when
+// max_clusters > 0.  -1 for T < 1, B < 1 or max_clusters < 2.
+int lstm_plan(int T, int B, int max_clusters, int plan[7]);
 int tta_views(const float* x, float* views, int V, const int* modes_dev, const int* shifts_dev, cudaStream_t st);
 int tta_merge(const float* bon, const float* cor, int V, const int* modes_dev, const int* shifts_dev, float* y_bon,
               float* y_cor, cudaStream_t st);

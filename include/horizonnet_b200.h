@@ -320,6 +320,12 @@ int hn_lstm_layer_backward(const float* xp, const float* hout, const float* whf,
  * co-schedule two of the recurrence's 16-CTA clusters. */
 int hn_lstm_layer(const float* xproj_dev, const float* w_hh_fwd_dev, const float* w_hh_bwd_dev,
                   float* out_dev, int T, int B, void* stream);
+/* Host-side launch layout of hn_lstm_layer for T steps of B columns on a device that co-schedules max_clusters of the
+ * recurrence's 16-CTA clusters (max_clusters <= 0: the current device's count, the cached answer hn_lstm_layer uses; no GPU
+ * work otherwise).  plan[7] = max_clusters used, 8-column groups, groups per cluster (1 or 2), clusters (both directions),
+ * groups in the last cluster of a direction, columns in the last group, waves (ceil(clusters / max_clusters)).
+ * -1 for T < 1, B < 1 or max_clusters < 2 (the device hn_lstm_layer refuses). */
+int hn_lstm_plan(int T, int B, int max_clusters, int plan[7]);
 
 #ifdef __cplusplus
 }

@@ -514,3 +514,130 @@ def lstm_reference(xproj, whh):
             o[t] = h
         out.append(o)
     return torch.cat(out, dim=2)
+
+
+# ---- elementwise error bound of the bi-LSTM recurrence (lstm_cluster.cu), by a teacher-forced fp64 replay.
+# A bound on the free-running recurrence would have to grow through W_hh exponentially.  Instead every step is replayed in
+# fp64 from the kernel's own h_{t-1}: pre_t = xp_t + W h^kernel_{t-1} (all steps in one matmul), the gates and the cell scan
+# from c = 0 in fp64.  The reference is driven by the kernel's h, so an error never feeds back through W; the gap between
+# kernel and reference c only carries each step's local error forward, multiplied by sigma(f) <= 1.
+#  * pre-activations.  W is carried as fp16 hi / lo of W * s (s = a per-row power of two that puts max|w| of the row into
+#    (2^13, 2^14]), h as fp16 hi / lo of 256 h; the MMAs take hi*hi + hi*lo + lo*hi (lo*lo dropped) and the partial sums
+#    (k = 16 per MMA, 4 MMAs per warp, 3 products, 8 warps) are added in fp32.  A normal lo leaves 2^-22 |v| of each operand
+#    and the dropped lo*lo is 2^-22 |w h|: 1.5 * 2^-21 per product; the ~14 fp32 additions of the sum (tensor-core adds may
+#    truncate) add up to about 2^-21 of the magnitude sum.  C_LSTM = 8 covers both with margin:  C_LSTM * 2^-21 * |W| |h|.
+#    A subnormal lo plane has an absolute resolution of 2^-25: 2^-33 of h (256 h) and 2^-25 / s <= 2^-38 max|w_row| of w
+#    (2x margin each):  2^-32 * sum|w_row| + 2^-37 * max|w_row| * sum|h|  (none at step 0, which has no product).  The
+#    unscale is a power of two; fmaf(sum, unscale, xp) rounds once:  2^-23 (|xp| + |pre|) with margin.
+#  * gates: each passes e_pre through its derivative at the fp64 value, plus 2^-21 relative for expf / tanhf and the
+#    division of sigmoid = 1 / (1 + expf(-x)) in fp32.
+#  * cell: e_c <- sigma(f) e_c + |c| e_sf + |tanh g| e_si + sigma(i) e_tg + 2^-23 (|sigma(f) c| + |sigma(i) tanh g| + |c'|)
+#    (two products and a sum, or an fma, in fp32; 2x margin).
+#  * output: e_h = sigma(o) (1 - tanh^2 c) e_c + |tanh c| e_so + 2^-21 sigma(o) |tanh c| + 2^-23 |h|.
+# A dropped cross product (hi*lo or lo*hi) leaves about 2^-12 of |W| |h| per step, 2^9 bounds; an h_{t-2} fed in where
+# h_{t-1} belongs is off by |W| |h_{t-1} - h_{t-2}|.  test_lstm_variants.py checks both against a CPU emulation of the
+# kernel's arithmetic.  On an H100 SXM (80 GB HBM3, 700 W limit, 7 co-resident clusters) the worst err / bound over every
+# unit case and input kind is 0.20; most worst elements sit at step 0, where pre = xp and only the fp32 gates and cell count.
+C_LSTM = 8.0
+LSTM_KINDS = ('init', 'trained', 'saturated', 'small')
+
+
+def lstm_inputs(kind, T, B, seed):
+    """xproj [T][B][4096] and W_hh [2048][512] of both directions, on the CPU:
+    * init: today's distribution: W uniform in +-0.04 (PyTorch's nn.LSTM init range is 1/sqrt(512) ~ 0.044), xproj ~ N(0, 0.5);
+    * trained: rows scaled by 2^-6 .. 2 (each row its own power-of-two row scale in the kernel), a few all-zero rows, rows
+      with one dominant entry (the rest 2^-16 below it: subnormal lo planes), xproj ~ N(0, 3);
+    * saturated: i and f pre-activations around +20 and g of either sign (fixed per column and unit), so |c| grows toward T
+      and its error is carried through sigma(f) ~ 1 at every step; o around +20 in half of the columns, so h ~ +-1;
+    * small: o around -9, so sigma(o) ~ 1e-4 and h ~ 1e-4, where the lo plane of 256 h is subnormal."""
+    g = torch.Generator().manual_seed(seed)
+    xp = torch.randn(T, B, 4096, generator=g)
+    W = [torch.rand(2048, 512, generator=g) * 0.08 - 0.04 for _ in range(2)]
+    if kind == 'init':
+        return xp * 0.5, W
+    if kind == 'trained':
+        for w in W:
+            w.mul_(2.0 ** (torch.rand(2048, 1, generator=g) * 7 - 6))
+            rows = torch.randperm(2048, generator=g)[:16]
+            w[rows[:6]] = 0.0
+            for r in rows[6:]:
+                w[r].mul_(2.0 ** -16)
+                w[r, torch.randint(512, (1,), generator=g)] = 0.5
+        return xp * 3.0, W
+    xv = xp.view(T, B, 2, 4, 512)
+    xv.mul_(0.5)
+    if kind == 'saturated':
+        xv[:, :, :, 0:2] += 20.0
+        sign = torch.where(torch.rand(B, 2, 512, generator=g) < 0.5, -1.0, 1.0)
+        xv[:, :, :, 2] += 1.5 * sign
+        xv[:, 1::2, :, 3] += 20.0
+    elif kind == 'small':
+        xv[:, :, :, 3] -= 9.0
+    else:
+        raise ValueError(kind)
+    return xp, W
+
+
+def lstm_bound(h, xp, W):
+    """One direction in step order: h [T][B][512] the kernel's outputs, xp [T][B][2048], W [2048][512] (any device).
+    Returns (reference h, bound), fp64, of the teacher-forced replay above."""
+    h, xp, W = h.double(), xp.double(), W.double()
+    hprev = torch.cat([torch.zeros_like(h[:1]), h[:-1]])
+    pre = xp + hprev @ W.t()
+    Wa = W.abs()
+    step = (torch.arange(h.shape[0], device=h.device) > 0).double().view(-1, 1, 1)
+    e_pre = C_LSTM * EPS21 * (hprev.abs() @ Wa.t()) + 2.0 ** -23 * (xp.abs() + pre.abs()) + \
+        step * (2.0 ** -32 * Wa.sum(1) + 2.0 ** -37 * Wa.amax(1) * hprev.abs().sum(2, keepdim=True))
+    i, f, g, o = pre.chunk(4, 2)
+    ei, ef, eg, eo = e_pre.chunk(4, 2)
+    si, sf, tg, so = torch.sigmoid(i), torch.sigmoid(f), torch.tanh(g), torch.sigmoid(o)
+    esi, esf = si * (1 - si) * ei + EPS21 * si, sf * (1 - sf) * ef + EPS21 * sf
+    etg, eso = (1 - tg * tg) * eg + EPS21 * tg.abs(), so * (1 - so) * eo + EPS21 * so
+    c = torch.zeros_like(h[0])
+    ec = torch.zeros_like(c)
+    ref, bound = torch.empty_like(h), torch.empty_like(h)
+    for t in range(h.shape[0]):
+        fc, ig = sf[t] * c, si[t] * tg[t]
+        cn = fc + ig
+        ec = sf[t] * ec + c.abs() * esf[t] + tg[t].abs() * esi[t] + si[t] * etg[t] + \
+            2.0 ** -23 * (fc.abs() + ig.abs() + cn.abs())
+        c = cn
+        tc = torch.tanh(c)
+        ref[t] = so[t] * tc
+        bound[t] = so[t] * (1 - tc * tc) * ec + tc.abs() * eso[t] + EPS21 * so[t] * tc.abs() + 2.0 ** -23 * ref[t].abs()
+    return ref, bound
+
+
+def lstm_ratio(out, xproj, W):
+    """Worst err / bound of hn_lstm_layer's output [T][B][1024] over both directions (the backward one replayed from
+    t = T-1 down), and the element where it occurs."""
+    worst, where = 0.0, None
+    for d in range(2):
+        h, xp = out[..., d * 512:(d + 1) * 512], xproj[..., d * 2048:(d + 1) * 2048]
+        if d:
+            h, xp = h.flip(0), xp.flip(0)
+        ref, bound = lstm_bound(h, xp, W[d])
+        err = (h.double() - ref).abs()
+        r = torch.where(err == 0, torch.zeros_like(err), err / bound)
+        m = r.max().item()
+        if m >= worst:
+            t, b, u = (int(v) for v in torch.nonzero(r == r.max())[0])
+            worst, where = m, dict(dir=d, t=(h.shape[0] - 1 - t) if d else t, col=b, unit=u)
+    return worst, where
+
+
+def lstm_run(xproj, W, dev='cuda:0'):
+    """hn_lstm_layer on device tensors into a NaN-filled output with a canary behind it; checks that every element is
+    written and finite and nothing past the end.  Returns out [T][B][1024]."""
+    T, B = xproj.shape[:2]
+    n = T * B * 1024
+    buf = torch.full((n + 4096,), float('nan'), device=dev)
+    buf[n:] = CANARY
+    _lib.check(_lib.lib().hn_lstm_layer(xproj.data_ptr(), W[0].data_ptr(), W[1].data_ptr(), buf.data_ptr(), T, B,
+                                        torch.cuda.current_stream(dev).cuda_stream), 'hn_lstm_layer')
+    torch.cuda.synchronize(dev)
+    out = buf[:n].view(T, B, 1024)
+    assert not torch.isnan(out).any(), 'output elements left unwritten'
+    assert torch.isfinite(out).all(), 'non-finite output'
+    assert bool((buf[n:] == CANARY).all()), 'write past the end of the output'
+    return out
