@@ -11,9 +11,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'lib', 'libhorizonnet_b200.so')
-SOURCES = ['model.cu', 'conv_f32.cu', 'conv_tc.cu', 'conv_narrow.cu', 'tail.cu', 'lstm_cluster.cu', 'panostretch.cu', 'rotate.cu', 'tta.cu', 'train_fwd.cu', 'bwd_kernels.cu', 'wgrad_tc.cu', 'train_step.cu']
+SOURCES = ['model.cu', 'conv_f32.cu', 'conv_tc.cu', 'conv_narrow.cu', 'tail.cu', 'lstm_cluster.cu', 'panostretch.cu', 'rotate.cu', 'tta.cu', 'layout.cu', 'train_fwd.cu', 'bwd_kernels.cu', 'wgrad_tc.cu', 'train_step.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-cudart', 'static']
+# per-source flags: the layout post-processing rounds every float64 step like numpy, so no FMA contraction there
+FILE_FLAGS = {'layout.cu': ['--fmad=false']}
 
 
 def _nvcc():
@@ -31,6 +33,7 @@ def _digest():
                 h.update(name.encode())
                 h.update(open(os.path.join(root, name), 'rb').read())
     h.update(' '.join(NVCC_FLAGS).encode())
+    h.update(repr(sorted(FILE_FLAGS.items())).encode())
     return h.hexdigest()
 
 
@@ -52,7 +55,7 @@ def build(force=False, verbose=False):
     procs = []
     for src in SOURCES:
         obj = os.path.join(objdir, src.replace('.cu', '.o'))
-        extra = ['-DHN_BUILD_DIGEST="%s"' % digest] if src == 'model.cu' else []
+        extra = (['-DHN_BUILD_DIGEST="%s"' % digest] if src == 'model.cu' else []) + FILE_FLAGS.get(src, [])
         cmd = [nvcc] + NVCC_FLAGS + extra + (['-Xptxas', '-v'] if verbose else []) + ['-c', os.path.join(CSRC, src), '-o', obj]
         procs.append((src, obj, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     objs = []

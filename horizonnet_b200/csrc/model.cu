@@ -896,16 +896,15 @@ int hn_model_collect_host(hn_model* m, float* bon, float* cor) {
     return 0;
 }
 
-int hn_model_infer_tta(hn_model* m, const float* x, int in_channels, int flip, const int* shifts, int n_rotate,
-                       float* y_bon_pix, float* y_cor, void* stream) {
-    HN_CHECK(m && x && y_bon_pix && y_cor, "hn_model_infer_tta: NULL argument");
-    HN_CHECK(in_channels == 3, "hn_model_infer_tta: expects a 3-channel panorama (inference.py:196-200)");
-    HN_CHECK(n_rotate >= 0 && n_rotate <= 32 && (n_rotate == 0 || shifts), "hn_model_infer_tta: bad rotate list");
+// The views of P panoramas (view-major, as reference augment concatenates them), one forward, the per-panorama merge
+static int infer_views(hn_model* m, const float* x, int P, int flip, const int* shifts, int n_rotate, float* y_bon_pix,
+                       float* y_cor, cudaStream_t st, const char* who) {
+    const std::string w(who);
+    HN_CHECK(n_rotate >= 0 && n_rotate <= 32 && (n_rotate == 0 || shifts), w + ": bad rotate list");
     const int V = 1 + (flip ? 1 : 0) + n_rotate;
-    HN_CHECK(V <= m->max_batch && V <= 64, "hn_model_infer_tta: views exceed max_batch");
-    HN_CHECK(m->submit_count == m->collect_count, "hn_model_infer_tta: collect the submitted batches first");
-    HN_ON_DEVICE(m->device);
-    cudaStream_t st = (cudaStream_t)stream;
+    HN_CHECK(P >= 1, w + ": no panoramas");
+    HN_CHECK(V <= 64 && (long long)V * P <= m->max_batch, w + ": panoramas x views exceed max_batch");
+    HN_CHECK(m->submit_count == m->collect_count, w + ": collect the submitted batches first");
     int host[128];
     int v = 0;
     host[v] = 0; host[64 + v] = 0; ++v;                         // aug_type '' (inference.py:34)
@@ -913,9 +912,40 @@ int hn_model_infer_tta(hn_model* m, const float* x, int in_channels, int flip, c
     for (int i = 0; i < n_rotate; ++i, ++v) { host[v] = 2; host[64 + v] = shifts[i]; }   // 'rotate shift' (:39-42)
     HN_CUDA_OK(cudaMemcpyAsync(m->tta_ints, host, sizeof(host), cudaMemcpyHostToDevice, st));
     HN_CUDA_OK(cudaStreamSynchronize(st));                      // host[] is a stack array
-    if (tta_views(x, m->x_slot[1], V, m->tta_ints, m->tta_ints + 64, st)) return -1;
-    if (hn_model_forward(m, m->x_slot[1], V, 3, m->bon_out, m->cor_out, st)) return -1;
-    return tta_merge(m->bon_out, m->cor_out, V, m->tta_ints, m->tta_ints + 64, y_bon_pix, y_cor, st);
+    if (tta_views(x, m->x_slot[1], V, P, m->tta_ints, m->tta_ints + 64, st)) return -1;
+    if (hn_model_forward(m, m->x_slot[1], V * P, 3, m->bon_out, m->cor_out, st)) return -1;
+    return tta_merge(m->bon_out, m->cor_out, V, P, m->tta_ints, m->tta_ints + 64, y_bon_pix, y_cor, st);
+}
+
+int hn_model_infer_tta(hn_model* m, const float* x, int in_channels, int flip, const int* shifts, int n_rotate,
+                       float* y_bon_pix, float* y_cor, void* stream) {
+    HN_CHECK(m && x && y_bon_pix && y_cor, "hn_model_infer_tta: NULL argument");
+    HN_CHECK(in_channels == 3, "hn_model_infer_tta: expects a 3-channel panorama (inference.py:196-200)");
+    HN_ON_DEVICE(m->device);
+    return infer_views(m, x, 1, flip, shifts, n_rotate, y_bon_pix, y_cor, (cudaStream_t)stream, "hn_model_infer_tta");
+}
+
+int hn_model_infer_layout(hn_model* m, const float* x, int B, int in_channels, int flip, const int* shifts, int n_rotate,
+                          int r_px, float min_v, int force_cuboid, int force_raw, int max_rows, float* y_bon_pix,
+                          float* y_cor, float* cor_id, int* n_rows, float* z0, float* z1, int* status, void* stream) {
+    HN_CHECK(m && x && y_bon_pix && y_cor && cor_id && n_rows && z0 && z1 && status, "hn_model_infer_layout: NULL argument");
+    HN_CHECK(in_channels == 3, "hn_model_infer_layout: expects 3-channel panoramas (inference.py:196-200)");
+    HN_CHECK(r_px >= 1 && r_px <= 1024 && max_rows >= 0, "hn_model_infer_layout: bad r_px or max_rows");
+    HN_ON_DEVICE(m->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (infer_views(m, x, B, flip, shifts, n_rotate, y_bon_pix, y_cor, st, "hn_model_infer_layout")) return -1;
+    return layout_postproc(y_bon_pix, y_cor, B, r_px, min_v, force_cuboid, force_raw, max_rows, cor_id, n_rows, z0, z1,
+                           status, nullptr, nullptr, st);
+}
+
+int hn_layout_postproc(const float* y_bon_pix, const float* y_cor, int B, int r_px, float min_v, int force_cuboid,
+                       int force_raw, int max_rows, float* cor_id, int* n_rows, float* z0, float* z1, int* status,
+                       int* peaks, int* n_peaks, void* stream) {
+    HN_CHECK(y_bon_pix && y_cor && cor_id && n_rows && z0 && z1 && status, "hn_layout_postproc: NULL argument");
+    HN_CHECK(B >= 1 && B <= 65535, "hn_layout_postproc: bad panorama count");
+    HN_CHECK(r_px >= 1 && r_px <= 1024 && max_rows >= 0, "hn_layout_postproc: bad r_px or max_rows");
+    return layout_postproc(y_bon_pix, y_cor, B, r_px, min_v, force_cuboid, force_raw, max_rows, cor_id, n_rows, z0, z1,
+                           status, peaks, n_peaks, (cudaStream_t)stream);
 }
 
 int hn_model_stage(hn_model* m, const char* stage, float* out, long long capacity, int dims[4], void* stream) {

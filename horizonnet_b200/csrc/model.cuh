@@ -30,9 +30,14 @@ int lstm_layer(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd,
 // clusters (both directions), groups in the last cluster, columns in the last group, waves.  No GPU work when
 // max_clusters > 0.  -1 for T < 1, B < 1 or max_clusters < 2.
 int lstm_plan(int T, int B, int max_clusters, int plan[7]);
-int tta_views(const float* x, float* views, int V, const int* modes_dev, const int* shifts_dev, cudaStream_t st);
-int tta_merge(const float* bon, const float* cor, int V, const int* modes_dev, const int* shifts_dev, float* y_bon,
+// P panoramas x V views, view-major (views[v*P + p]); y_bon [P][2][1024], y_cor [P][1024]
+int tta_views(const float* x, float* views, int V, int P, const int* modes_dev, const int* shifts_dev, cudaStream_t st);
+int tta_merge(const float* bon, const float* cor, int V, int P, const int* modes_dev, const int* shifts_dev, float* y_bon,
               float* y_cor, cudaStream_t st);
+// Layout post-processing (layout.cu), one CTA per panorama; peaks / n_peaks may be NULL
+int layout_postproc(const float* y_bon_pix, const float* y_cor, int B, int r_px, float min_v, int force_cuboid, int force_raw,
+                    int max_rows, float* cor_id, int* n_rows, float* z0, float* z1, int* status, int* peaks, int* n_peaks,
+                    cudaStream_t st);
 int pano_stretch_device(const float* img, float* out, int n, int H, int W, int C, const double* kx_dev,
                         const double* ky_dev, double* scratch, int order, cudaStream_t st);
 int pano_stretch_device_f64(const double* img, double* out, int n, int H, int W, int C, const double* kx_dev,

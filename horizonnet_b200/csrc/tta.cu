@@ -9,36 +9,43 @@ namespace hn {
 
 namespace {
 
-// views[v][c][h][w] = x[c][h][src(w)];  mode 0: identity, 1: flip (np.flip axis -1), 2: roll by shift (np.roll)
-__global__ void tta_views_kernel(const float* __restrict__ x, float* __restrict__ views, int V,
+// views[v*P + p][c][h][w] = x[p][c][h][src(w)] (view-major, as augment concatenates the views of a batch);
+// mode 0: identity, 1: flip (np.flip axis -1), 2: roll by shift (np.roll)
+__global__ void tta_views_kernel(const float* __restrict__ x, float* __restrict__ views, int V, int P,
                                  const int* __restrict__ modes, const int* __restrict__ shifts, int H, int W) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t per = (size_t)3 * H * W;
-    if (i >= per * V) return;
-    const int v = (int)(i / per);
-    const size_t r = i - (size_t)v * per;
+    if (i >= per * V * P) return;
+    const int vp = (int)(i / per);
+    const int v = vp / P, p = vp - v * P;
+    const size_t r = i - (size_t)vp * per;
     const int w = (int)(r % W);
-    const size_t row = r / W;                       // c*H + h
+    const size_t row = (size_t)p * 3 * H + r / W;   // (p*3 + c)*H + h
     int src = w;
     if (modes[v] == 1) src = W - 1 - w;
     else if (modes[v] == 2) { src = (w - shifts[v]) % W; if (src < 0) src += W; }      // np.roll(x, shift): out[w] = in[w - shift]
     views[i] = __ldg(x + row * W + src);
 }
 
-// y_bon_pix[s][w] = clip(((mean_v undo(bon[v][s]))[w] / pi + 0.5) * H - 0.5),  y_cor[w] = mean_v undo(sigmoid(cor[v]))[w]
-__global__ void tta_merge_kernel(const float* __restrict__ bon, const float* __restrict__ cor, int V,
+// Per panorama p (blockIdx.y) of P:  y_bon_pix[p][s][w] = clip(((mean_v undo(bon[v*P + p][s]))[w] / pi + 0.5) * H - 0.5),
+// y_cor[p][w] = mean_v undo(sigmoid(cor[v*P + p]))[w]
+__global__ void tta_merge_kernel(const float* __restrict__ bon, const float* __restrict__ cor, int V, int P,
                                  const int* __restrict__ modes, const int* __restrict__ shifts, float* __restrict__ y_bon,
                                  float* __restrict__ y_cor, int H, int W) {
     const int w = blockIdx.x * blockDim.x + threadIdx.x;
+    const int p = blockIdx.y;
     if (w >= W) return;
+    y_bon += (size_t)p * 2 * W;
+    y_cor += (size_t)p * W;
     float sb0 = 0.f, sb1 = 0.f, sc = 0.f;
     for (int v = 0; v < V; ++v) {
         int src = w;
         if (modes[v] == 1) src = W - 1 - w;                                   // undo flip
         else if (modes[v] == 2) { src = (w + shifts[v]) % W; if (src < 0) src += W; }   // np.roll(x, -shift)
-        sb0 += bon[((size_t)v * 2 + 0) * W + src];
-        sb1 += bon[((size_t)v * 2 + 1) * W + src];
-        sc += 1.f / (1.f + expf(-cor[(size_t)v * W + src]));                  // torch.sigmoid before the undo (inference.py:80)
+        const size_t vp = (size_t)v * P + p;
+        sb0 += bon[(vp * 2 + 0) * W + src];
+        sb1 += bon[(vp * 2 + 1) * W + src];
+        sc += 1.f / (1.f + expf(-cor[vp * W + src]));                         // torch.sigmoid before the undo (inference.py:80)
     }
     const float inv = (float)V;
     const float pi = 3.14159265358979323846f;
@@ -53,16 +60,16 @@ __global__ void tta_merge_kernel(const float* __restrict__ bon, const float* __r
 
 }  // namespace
 
-int tta_views(const float* x, float* views, int V, const int* modes_dev, const int* shifts_dev, cudaStream_t st) {
-    const size_t total = (size_t)V * 3 * 512 * 1024;
-    tta_views_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x, views, V, modes_dev, shifts_dev, 512, 1024);
+int tta_views(const float* x, float* views, int V, int P, const int* modes_dev, const int* shifts_dev, cudaStream_t st) {
+    const size_t total = (size_t)V * P * 3 * 512 * 1024;
+    tta_views_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x, views, V, P, modes_dev, shifts_dev, 512, 1024);
     HN_LAUNCH_OK();
     return 0;
 }
 
-int tta_merge(const float* bon, const float* cor, int V, const int* modes_dev, const int* shifts_dev, float* y_bon,
+int tta_merge(const float* bon, const float* cor, int V, int P, const int* modes_dev, const int* shifts_dev, float* y_bon,
               float* y_cor, cudaStream_t st) {
-    tta_merge_kernel<<<4, 256, 0, st>>>(bon, cor, V, modes_dev, shifts_dev, y_bon, y_cor, 512, 1024);
+    tta_merge_kernel<<<dim3(4, P), 256, 0, st>>>(bon, cor, V, P, modes_dev, shifts_dev, y_bon, y_cor, 512, 1024);
     HN_LAUNCH_OK();
     return 0;
 }

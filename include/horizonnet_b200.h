@@ -160,6 +160,16 @@ int hn_model_collect_host(hn_model* m, float* bon_host, float* cor_host);
 int hn_model_infer_tta(hn_model* m, const float* x_dev, int in_channels, int flip, const int* shifts_host,
                        int n_rotate, float* y_bon_pix_dev, float* y_cor_dev, void* stream);
 
+/* Room layouts of B panoramas (reference inference.py:65-141, the whole inference() per panorama): x [B][3][512][1024]
+ * fp32 on the device; the views of all panoramas (identity, + flip, + one np.roll per shift as in hn_model_infer_tta) run as
+ * ONE forward of B * views panoramas, view-major like the reference's augment; the merge leaves y_bon_pix [B][2][1024] and
+ * y_cor [B][1024] (device, caller-owned, the values hn_model_infer_tta gives per panorama) and hn_layout_postproc turns them
+ * into corners with the remaining arguments.  Needs B * views <= max_batch and views <= 64. */
+int hn_model_infer_layout(hn_model* m, const float* x_dev, int B, int in_channels, int flip, const int* shifts_host,
+                          int n_rotate, int r_px, float min_v, int force_cuboid, int force_raw, int max_rows,
+                          float* y_bon_pix_dev, float* y_cor_dev, float* cor_id_dev, int* n_rows_dev, float* z0_dev,
+                          float* z1_dev, int* status_dev, void* stream);
+
 /* Test hook: copies an intermediate result of the LAST forward, converted to the reference's
  * layout, into `out_dev` (fp32).  Stages: "stem" (conv1+bn1+relu, NCHW [B,64,256,512], model.py:73-75),
  * "layer1".."layer4" (NCHW [B,C,H,W], model.py:78-81),
@@ -207,6 +217,31 @@ int hn_pano_stretch_f64(const double* img_dev, double* out_dev, int n, int h, in
                         const double* kx_host, const double* ky_host, int order, void* stream);
 int hn_pano_stretch_host_f64(const double* img_host, double* out_host, int n, int h, int w, int c,
                              const double* kx_host, const double* ky_host, int order);
+
+/* ---- layout post-processing (reference inference.py:95-141, misc/post_proc.py), one CTA per panorama ----------------
+ *
+ * y_bon_pix [B][2][1024] (ceiling / floor boundary rows in pixels, clipped) and y_cor [B][1024] (corner probability), fp32
+ * on the device, as hn_model_infer_tta leaves them.  r_px = int(round(1024 * r / 2)) of inference.py:108 (Python rounding,
+ * host side); min_v: the peak threshold (inference.py:106-107 picks 0 for cuboids, 0.05 otherwise).  force_raw exports the
+ * 1024-column raw polygon.  Outputs (device): cor_id [B][max_rows][2] fp32 -- the first n_rows[b] rows are the reference's
+ * cor_id (ceiling / floor pairs, normalised by W and H), the rest are zero; max_rows = 2048 holds every result, force_raw
+ * included -- n_rows [B], z0 [B] (= 50), z1 [B] and status [B]:
+ *   HN_LAYOUT_OK 0, HN_LAYOUT_FALLBACK 1 (the general layout was not a simple polygon; a cuboid replaced it, the
+ *   reference's "Generate cuboid as fallback"), and where the reference raises: HN_LAYOUT_ERR_GROUPS 2 (gen_ww's
+ *   AssertionError on the number of wall groups: a cuboid without 4 peaks, a general layout without any), HN_LAYOUT_ERR_VOTE
+ *   3 (vote's AssertionError: the best run is one value), HN_LAYOUT_ERR_RING 4 (shapely's ValueError: fewer than 3 walls);
+ *   HN_LAYOUT_ERR_OVERFLOW 5: the corners do not fit in max_rows rows (nothing is truncated).  n_rows is 0 unless the
+ *   status is 0 or 1.  peaks [B][1024] / n_peaks [B] (NULL to skip): the peak columns of the fit that produced the result
+ *   (the cuboid's after a fallback), -1 padded.  Top-4 ties in value go to the lower column. */
+#define HN_LAYOUT_OK 0
+#define HN_LAYOUT_FALLBACK 1
+#define HN_LAYOUT_ERR_GROUPS 2
+#define HN_LAYOUT_ERR_VOTE 3
+#define HN_LAYOUT_ERR_RING 4
+#define HN_LAYOUT_ERR_OVERFLOW 5
+int hn_layout_postproc(const float* y_bon_pix_dev, const float* y_cor_dev, int B, int r_px, float min_v, int force_cuboid,
+                       int force_raw, int max_rows, float* cor_id_dev, int* n_rows_dev, float* z0_dev, float* z1_dev,
+                       int* status_dev, int* peaks_dev, int* n_peaks_dev, void* stream);
 
 /* ---- dataset.PanoCorBonDataset.__getitem__, image path (reference dataset.py:53, 69-105, 124) ------
  *
