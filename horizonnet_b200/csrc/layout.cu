@@ -8,11 +8,12 @@
 //   walls    gen_ww in float64: column -> wall group (get_gpid), floor-plane projection (np_coor2xy), vote per group and
 //            axis (block sort + the first longest run within tol covering 40 %, or the median), gen_ww_cuboid or the
 //            gen_ww_general loop (a block argmax picks the wall, thread 0 decides, the block shifts the wall list);
-//   validity the general result's float32 ring xy2d must be a simple polygon, else a cuboid fit on the top-4 peaks with
+//   validity the general result's float32 ring xy2d must be a simple polygon (ring.cuh), else a cuboid fit on the top-4 peaks with
 //            min_v 0 replaces it (status HN_LAYOUT_FALLBACK);
 //   output   np_xy2coor, the roll to the smallest ceiling column, infer_coory, cor_id rows normalised by W and H.
 // This file is compiled without FMA contraction (build.py) so the float64 steps round like numpy's.
 #include "hn_common.cuh"
+#include "ring.cuh"
 
 namespace hn {
 
@@ -437,19 +438,6 @@ __device__ int fit_walls(Smem& s, int r_px, float min_v, bool cuboid, float tol)
     return general_loop(s);
 }
 
-__device__ double orient(const float* a, const float* b, const float* c) {
-    return ((double)b[0] - a[0]) * ((double)c[1] - a[1]) - ((double)b[1] - a[1]) * ((double)c[0] - a[0]);
-}
-__device__ bool on_box(const float* a, const float* b, const float* c) {
-    return fminf(a[0], b[0]) <= c[0] && c[0] <= fmaxf(a[0], b[0]) && fminf(a[1], b[1]) <= c[1] && c[1] <= fmaxf(a[1], b[1]);
-}
-__device__ bool segments_meet(const float* a, const float* b, const float* c, const float* d) {
-    const double o1 = orient(a, b, c), o2 = orient(a, b, d), o3 = orient(c, d, a), o4 = orient(c, d, b);
-    if (((o1 > 0 && o2 < 0) || (o1 < 0 && o2 > 0)) && ((o3 > 0 && o4 < 0) || (o3 < 0 && o4 > 0))) return true;
-    return (o1 == 0 && on_box(a, b, c)) || (o2 == 0 && on_box(a, b, d)) || (o3 == 0 && on_box(c, d, a)) ||
-           (o4 == 0 && on_box(c, d, b));
-}
-
 // The float32 ring xy2d of the walls (inference.py:115-119) is a simple polygon (DESIGN.md section 8).
 __device__ bool ring_is_simple(Smem& s) {
     const int n = s.n_walls;
@@ -461,44 +449,7 @@ __device__ bool ring_is_simple(Smem& s) {
         s.ring[i][1] = s.waxis[p] == 1 ? vp : (s.waxis[i] == 1 ? vi : 0.f);
     }
     __syncthreads();
-    // drop vertices equal to their predecessor, cyclically (a ring of one repeated point keeps one)
-    int keep[WMAX / NT], cnt = 0;
-    float kx[WMAX / NT], ky[WMAX / NT];
-    for (int k = 0; k < WMAX / NT; ++k) {
-        const int i = threadIdx.x * (WMAX / NT) + k;
-        keep[k] = 0;
-        if (i < n) {
-            const int p = (i - 1 + n) % n;
-            keep[k] = !(s.ring[i][0] == s.ring[p][0] && s.ring[i][1] == s.ring[p][1]);
-            kx[k] = s.ring[i][0];
-            ky[k] = s.ring[i][1];
-        }
-        cnt += keep[k];
-    }
-    int o = block_scan(s, cnt);
-    const int m = s.bi;
-    __syncthreads();
-    for (int k = 0; k < WMAX / NT; ++k) if (keep[k]) { s.ring[o][0] = kx[k]; s.ring[o][1] = ky[k]; ++o; }
-    if (threadIdx.x == 0) s.flag = 0;
-    __syncthreads();
-    if (m < 3) return false;
-    for (int i = threadIdx.x; i < m; i += NT) {                  // no fold-back at a vertex
-        const float* a = s.ring[(i - 1 + m) % m];
-        const float* b = s.ring[i];
-        const float* c = s.ring[(i + 1) % m];
-        const double d1x = (double)b[0] - a[0], d1y = (double)b[1] - a[1], d2x = (double)c[0] - b[0], d2y = (double)c[1] - b[1];
-        if (d1x * d2y - d1y * d2x == 0 && d1x * d2x + d1y * d2y < 0) s.flag = 1;
-    }
-    const long long pairs = (long long)m * m;                    // no two non-adjacent edges meet
-    bool met = false;
-    for (long long t = threadIdx.x; t < pairs && !met; t += NT) {
-        const int i = (int)(t / m), j = (int)(t % m);
-        if (j < i + 2 || (i == 0 && j == m - 1)) continue;
-        met = segments_meet(s.ring[i], s.ring[(i + 1) % m], s.ring[j], s.ring[(j + 1) % m]);
-    }
-    if (met) s.flag = 1;
-    __syncthreads();
-    return s.flag == 0;
+    return ring::is_simple<NT, WMAX>(s.ring, n, s.scan, &s.flag);
 }
 
 __global__ void __launch_bounds__(NT, 1)

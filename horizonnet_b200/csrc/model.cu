@@ -948,6 +948,47 @@ int hn_layout_postproc(const float* y_bon_pix, const float* y_cor, int B, int r_
                            status, peaks, n_peaks, (cudaStream_t)stream);
 }
 
+int hn_model_validate(hn_model* m, const float* x, int B, int in_channels, const float* gt, const int* gt_rows,
+                      int max_rows, double* iou2d, double* iou3d, double* rmse, double* delta_1, int* status,
+                      void* stream) {
+    HN_CHECK(m && x && gt && gt_rows && iou2d && iou3d && rmse && delta_1 && status, "hn_model_validate: NULL argument");
+    HN_CHECK(in_channels == 3, "hn_model_validate: expects 3-channel panoramas (inference.py:196-200)");
+    HN_CHECK(B >= 1 && B <= 65535 && max_rows >= 0 && max_rows <= 2048, "hn_model_validate: bad B or max_rows");
+    HN_ON_DEVICE(m->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    // inference(net, x, force_raw=True) without augmentation (train.py:306), its outputs kept on the device
+    constexpr int R = 2048;
+    const size_t nf = (size_t)B * (2 * 1024 + 1024 + R * 2 + 2);
+    float* buf = nullptr;
+    int* ibuf = nullptr;
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&buf), nf * sizeof(float), st));
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&ibuf), (size_t)B * 2 * sizeof(int), st));
+    float* y_bon = buf;
+    float* y_cor = y_bon + (size_t)B * 2 * 1024;
+    float* cor_id = y_cor + (size_t)B * 1024;
+    float* z0 = cor_id + (size_t)B * R * 2;
+    float* z1 = z0 + B;
+    int rc = infer_views(m, x, B, 0, nullptr, 0, y_bon, y_cor, st, "hn_model_validate");
+    if (!rc) rc = layout_postproc(y_bon, y_cor, B, 26, 0.05f, 0, 1, R, cor_id, ibuf, z0, z1, ibuf + B, nullptr, nullptr, st);
+    // a failed inference is scored as train.py:309-313's fallback box (layout statuses 2..5)
+    if (!rc) rc = layout_eval_general(cor_id, ibuf, ibuf + B, R, gt, gt_rows, max_rows, B, iou2d, iou3d, rmse, delta_1,
+                                      status, nullptr, st);
+    cudaFreeAsync(buf, st);
+    cudaFreeAsync(ibuf, st);
+    return rc;
+}
+
+int hn_layout_eval_general(const float* dt, const int* dt_rows, const int* dt_status, const float* gt, const int* gt_rows,
+                           int B, int max_rows, double* iou2d, double* iou3d, double* rmse, double* delta_1, int* status,
+                           float* depth_out, void* stream) {
+    HN_CHECK(dt && dt_rows && gt && gt_rows && iou2d && iou3d && rmse && delta_1 && status,
+             "hn_layout_eval_general: NULL argument");
+    HN_CHECK(B >= 1 && B <= 65535, "hn_layout_eval_general: bad pair count");
+    HN_CHECK(max_rows >= 0 && max_rows <= 2048, "hn_layout_eval_general: max_rows must be in 0..2048");
+    return layout_eval_general(dt, dt_rows, dt_status, max_rows, gt, gt_rows, max_rows, B, iou2d, iou3d, rmse, delta_1,
+                               status, depth_out, (cudaStream_t)stream);
+}
+
 int hn_model_stage(hn_model* m, const char* stage, float* out, long long capacity, int dims[4], void* stream) {
     HN_CHECK(m && stage && out && dims, "hn_model_stage: NULL argument");
     HN_CHECK(m->last_batch > 0, "hn_model_stage: no forward has run yet");

@@ -38,6 +38,10 @@ int tta_merge(const float* bon, const float* cor, int V, int P, const int* modes
 int layout_postproc(const float* y_bon_pix, const float* y_cor, int B, int r_px, float min_v, int force_cuboid, int force_raw,
                     int max_rows, float* cor_id, int* n_rows, float* z0, float* z1, int* status, int* peaks, int* n_peaks,
                     cudaStream_t st);
+// Layout evaluation (layout_eval.cu): eval_general's metrics of B (dt, gt) pairs; dt_status / depth_out may be NULL
+int layout_eval_general(const float* dt, const int* dt_rows, const int* dt_status, int dt_max_rows, const float* gt,
+                        const int* gt_rows, int gt_max_rows, int B, double* iou2d, double* iou3d, double* rmse,
+                        double* delta_1, int* status, float* depth_out, cudaStream_t st);
 int pano_stretch_device(const float* img, float* out, int n, int H, int W, int C, const double* kx_dev,
                         const double* ky_dev, double* scratch, int order, cudaStream_t st);
 int pano_stretch_device_f64(const double* img, double* out, int n, int H, int W, int C, const double* kx_dev,

@@ -243,6 +243,40 @@ int hn_layout_postproc(const float* y_bon_pix_dev, const float* y_cor_dev, int B
                        int force_raw, int max_rows, float* cor_id_dev, int* n_rows_dev, float* z0_dev, float* z1_dev,
                        int* status_dev, int* peaks_dev, int* n_peaks_dev, void* stream);
 
+/* ---- layout evaluation (reference eval_general.py:14-122 test_general / layout_2_depth), on the device --------------
+ *
+ * B (dt, gt) corner-list pairs, each padded to max_rows (<= 2048) rows of [x, y] fp32 on the device: dt [B][max_rows][2]
+ * normalised by W and H, as hn_layout_postproc leaves it (scaled by (1024, 512) in fp32 inside, eval_general.py:157-158),
+ * with dt_rows [B]; gt [B][max_rows][2] in pixels, as the label_cor txt files hold them, with gt_rows [B].  dt_status [B]
+ * (NULL to skip): the hn_layout_postproc status of each dt; a pair whose status is 2..5 is scored with train.py:309-313's
+ * fallback box [k//2 * 1024, 256 - ((k%2)*2 - 1) * 120], k = 0..7, in int64 arithmetic like the reference.  Only 1024 x 512
+ * panoramas: test_general hard-codes that size.  Outputs (device, fp64): iou2d, iou3d, rmse, delta_1 [B] and status [B]:
+ *   HN_EVAL_OK 0; HN_EVAL_DT_INVALID 1 (the dt floor ring is not a simple polygon: iou2d = iou3d = 0, the reference's
+ *   except branches); HN_EVAL_SKIP_GT_INVALID 2 (the gt floor ring is not a simple polygon: the reference skips the pair,
+ *   all outputs NaN); and where the reference raises, all outputs NaN: HN_EVAL_ERR_GT_DEPTH 3 (layout_2_depth's assertions
+ *   on the gt), HN_EVAL_ERR_COLUMNS 4 (an odd row count, or ceiling and floor columns that differ, eval_general.py:61-62),
+ *   HN_EVAL_ERR_RING 5 (fewer than 3 floor corners, or a row count outside 0..max_rows).  layout_2_depth's assertions on the
+ *   dt make its depth all zeros (rmse = RMS of the gt depth, delta_1 = 0), as the reference's except does.  Validity is
+ *   layout.cu's simple-ring definition on the fp32 floor ring (DESIGN.md sections 8, 9).  depth_out [B][2][512][1024] fp32
+ *   (NULL to skip) receives the dt (0) and gt (1) depth maps of every pair whose status is 0, 1 or 2; a dt map on which
+ *   layout_2_depth asserts is all zeros. */
+#define HN_EVAL_OK 0
+#define HN_EVAL_DT_INVALID 1
+#define HN_EVAL_SKIP_GT_INVALID 2
+#define HN_EVAL_ERR_GT_DEPTH 3
+#define HN_EVAL_ERR_COLUMNS 4
+#define HN_EVAL_ERR_RING 5
+int hn_layout_eval_general(const float* dt_dev, const int* dt_rows_dev, const int* dt_status_dev, const float* gt_dev,
+                           const int* gt_rows_dev, int B, int max_rows, double* iou2d_dev, double* iou3d_dev,
+                           double* rmse_dev, double* delta_1_dev, int* status_dev, float* depth_out_dev, void* stream);
+
+/* The validation of train.py:301-318 for B panoramas: hn_model_infer_layout with force_raw = 1 and no augmentation, then
+ * hn_layout_eval_general of its device outputs against gt [B][max_rows][2] (pixels) / gt_rows [B], a failed inference
+ * scored as the fallback box.  Outputs as hn_layout_eval_general's.  Needs B <= max_batch. */
+int hn_model_validate(hn_model* m, const float* x_dev, int B, int in_channels, const float* gt_dev, const int* gt_rows_dev,
+                      int max_rows, double* iou2d_dev, double* iou3d_dev, double* rmse_dev, double* delta_1_dev,
+                      int* status_dev, void* stream);
+
 /* ---- dataset.PanoCorBonDataset.__getitem__, image path (reference dataset.py:53, 69-105, 124) ------
  *
  * One fused gather pass per image:  uint8 HWC / 255 -> pano_stretch(kx, ky) -> flip -> roll(dx) -> ** gamma -> CHW:
