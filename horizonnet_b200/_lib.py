@@ -74,6 +74,9 @@ SIGNATURES = {
                                           ctypes.c_int] + [vp] * 8),
     'hn_layout_eval_general': (ctypes.c_int, [vp] * 5 + [ctypes.c_int, ctypes.c_int] + [vp] * 7),
     'hn_model_validate': (ctypes.c_int, [vp, vp, ctypes.c_int, ctypes.c_int, vp, vp, ctypes.c_int] + [vp] * 6),
+    'hn_layout_eval_cuboid': (ctypes.c_int, [vp] * 7 + [ctypes.c_int, ctypes.c_int] + [vp] * 5),
+    'hn_model_eval_cuboid': (ctypes.c_int, [vp, vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_int_p, ctypes.c_int,
+                                            ctypes.c_int, ctypes.c_float, vp, vp, ctypes.c_int] + [vp] * 5),
     'hn_model_stage': (ctypes.c_int, [vp, ctypes.c_char_p, vp, ctypes.c_longlong, c_int_p, vp]),
     'hn_model_set_option': (ctypes.c_int, [vp, ctypes.c_char_p, ctypes.c_int]),
     'hn_model_check': (ctypes.c_int, [vp]),

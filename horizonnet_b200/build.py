@@ -11,11 +11,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'lib', 'libhorizonnet_b200.so')
-SOURCES = ['model.cu', 'conv_f32.cu', 'conv_tc.cu', 'conv_narrow.cu', 'tail.cu', 'lstm_cluster.cu', 'panostretch.cu', 'rotate.cu', 'tta.cu', 'layout.cu', 'layout_eval.cu', 'train_fwd.cu', 'bwd_kernels.cu', 'wgrad_tc.cu', 'train_step.cu']
+SOURCES = ['model.cu', 'conv_f32.cu', 'conv_tc.cu', 'conv_narrow.cu', 'tail.cu', 'lstm_cluster.cu', 'panostretch.cu', 'rotate.cu', 'tta.cu', 'layout.cu', 'layout_eval.cu', 'layout_cuboid.cu', 'train_fwd.cu', 'bwd_kernels.cu', 'wgrad_tc.cu', 'train_step.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-cudart', 'static']
 # per-source flags: the layout post-processing and evaluation round every float64 step like numpy, so no FMA contraction
-FILE_FLAGS = {'layout.cu': ['--fmad=false'], 'layout_eval.cu': ['--fmad=false']}
+FILE_FLAGS = {'layout.cu': ['--fmad=false'], 'layout_eval.cu': ['--fmad=false'], 'layout_cuboid.cu': ['--fmad=false']}
 
 
 def _nvcc():

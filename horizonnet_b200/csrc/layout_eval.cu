@@ -13,6 +13,7 @@
 // run in float32 and the per-column ones in float64; train.py's fallback box is int64, and for it every step is float64.
 // This file is compiled without FMA contraction (build.py) so the float64 steps round like numpy's.
 #include "hn_common.cuh"
+#include "pano_connect.cuh"
 #include "ring.cuh"
 
 namespace hn {
@@ -27,6 +28,11 @@ constexpr int BT = 512, CPT = W / BT;      // bound_kernel threads; columns (and
 constexpr int IT = 256;                    // iou_kernel threads
 constexpr int DT_ = 256, RB = 16, NBLK = H / RB;   // depth_kernel threads, rows per CTA, CTAs per pair
 constexpr double PI = 3.141592653589793;
+using pano::tan_;
+using pano::sin_;
+using pano::cos_;
+using pano::wall_range;
+using pano::wall_row;
 enum { ST_OK = 0, ST_DT_INVALID = 1, ST_SKIP = 2, ST_ERR_GT_DEPTH = 3, ST_ERR_COLUMNS = 4, ST_ERR_RING = 5 };
 
 struct Part {
@@ -64,14 +70,6 @@ __device__ void corner(const Pairs& p, int b, int gt, int row, double& x, double
     else { x = c[0] * 1024.f; y = c[1] * 512.f; }   // eval_general.py:157-158, train.py:307-308, float32
 }
 
-// transcendental functions of numpy's float32 / float64 scalars (float32: the float64 result rounded, as layout.cu)
-__device__ float tan_(float v) { return (float)tan((double)v); }
-__device__ float sin_(float v) { return (float)sin((double)v); }
-__device__ float cos_(float v) { return (float)cos((double)v); }
-__device__ double tan_(double v) { return tan(v); }
-__device__ double sin_(double v) { return sin(v); }
-__device__ double cos_(double v) { return cos(v); }
-
 // --------------------------------------------------------------------------------------------- cor_2_1d
 struct BSmem {
     float px[MAXC], py[MAXC];                        // this boundary's corners (exact in float32 in both modes)
@@ -86,35 +84,6 @@ struct BSmem {
     double dred[BT / 32];
     double ymax;
 };
-
-// pano_connect_points' column range of the wall p1 -> p2 (in T, the corners' dtype); false for a vertical wall
-template <typename T>
-__device__ bool wall_range(T ax, T bx, long long& s, long long& e) {
-    if (ax == bx) return false;
-    T ps, pe;
-    if (fabs((double)(ax - bx)) < W / 2.0) { ps = ceil(fmin(ax, bx)); pe = floor(fmax(ax, bx)); }
-    else { ps = ceil(fmax(ax, bx)); pe = floor(fmin(ax, bx) + (T)W); }
-    s = (long long)ps;
-    e = (long long)pe;                               // np.arange(ps, pe + 1): integers s .. e
-    return true;
-}
-
-// pano_connect_points' row at sampled column c of the wall (ax, ay) -> (bx, by) on the plane z
-template <typename T>
-__device__ double wall_row(T ax, T ay, T bx, T by, int c, double z) {
-    const T pi = (T)PI;
-    const T u1 = ((ax + (T)0.5) / (T)W - (T)0.5) * (T)2 * pi, v1 = ((ay + (T)0.5) / (T)H - (T)0.5) * pi;
-    const T u2 = ((bx + (T)0.5) / (T)W - (T)0.5) * (T)2 * pi, v2 = ((by + (T)0.5) / (T)H - (T)0.5) * pi;
-    const T c1 = (T)z / tan_(v1), c2 = (T)z / tan_(v2);
-    const T x1 = c1 * cos_(u1), y1 = c1 * sin_(u1), x2 = c2 * cos_(u2), y2 = c2 * sin_(u2);
-    const T vx = x2 - x1, vy = y2 - y1;
-    const double us = (((double)c + 0.5) / W - 0.5) * 2 * PI;
-    const double t = tan(us);
-    const double ps = (t * (double)x1 - (double)y1) / ((double)vy - t * (double)vx);
-    const double qx = (double)x1 + ps * (double)vx, qy = (double)y1 + ps * (double)vy;
-    const double cs = sqrt(qx * qx + qy * qy);
-    return (atan2(z, cs) / PI + 0.5) * H - 0.5;
-}
 
 // slot order for the argsort + np.unique: valid slots first, then by x, key, concatenation index
 __device__ bool slot_less(const BSmem& s, int i, int j, int nslot) {
@@ -296,22 +265,7 @@ __device__ void boundary(BSmem& s, int nw, bool floor_b, double* v_out, int* fla
     bool bad = false;
     for (int c = threadIdx.x; c < W; c += BT) {
         const double x = (double)c;
-        int lo = -1, hi = n - 1;                         // the last j with xp[j] <= x
-        while (lo < hi) {
-            const int m = (lo + hi + 1) >> 1;
-            if (s.ex[m] <= x) lo = m; else hi = m - 1;
-        }
-        double r;
-        if (lo < 0) r = s.ey[0];
-        else if (lo == n - 1 || s.ex[lo] == x) r = s.ey[lo];
-        else {
-            const double slope = (s.ey[lo + 1] - s.ey[lo]) / (s.ex[lo + 1] - s.ex[lo]);
-            r = slope * (x - s.ex[lo]) + s.ey[lo];
-            if (isnan(r)) {
-                r = slope * (x - s.ex[lo + 1]) + s.ey[lo + 1];
-                if (isnan(r) && s.ey[lo] == s.ey[lo + 1]) r = s.ey[lo];
-            }
-        }
+        const double r = pano::interp(s.ex, s.ey, n, x);
         const double v = ((r + 0.5) / H - 0.5) * PI;
         v_out[c] = v;
         bad |= floor_b ? v < 0 : v > 0;                  // layout_2_depth's two assertions

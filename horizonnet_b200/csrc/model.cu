@@ -989,6 +989,48 @@ int hn_layout_eval_general(const float* dt, const int* dt_rows, const int* dt_st
                                status, depth_out, (cudaStream_t)stream);
 }
 
+int hn_layout_eval_cuboid(const float* dt, const int* dt_rows, const int* dt_status, const double* z0, const double* z1,
+                          const float* gt, const int* gt_rows, int B, int max_rows, double* ce, double* pe, double* iou3d,
+                          int* status, void* stream) {
+    HN_CHECK(dt && dt_rows && z0 && z1 && gt && gt_rows && ce && pe && iou3d && status,
+             "hn_layout_eval_cuboid: NULL argument");
+    HN_CHECK(B >= 1 && B <= 65535, "hn_layout_eval_cuboid: bad pair count");
+    HN_CHECK(max_rows >= 8 && max_rows <= 2048, "hn_layout_eval_cuboid: max_rows must be in 8..2048");
+    return layout_eval_cuboid(dt, dt_rows, dt_status, max_rows, z0, z1, nullptr, nullptr, gt, gt_rows, max_rows, B, ce, pe,
+                              iou3d, status, (cudaStream_t)stream);
+}
+
+int hn_model_eval_cuboid(hn_model* m, const float* x, int B, int in_channels, int flip, const int* shifts, int n_rotate,
+                         int r_px, float min_v, const float* gt, const int* gt_rows, int max_rows, double* ce, double* pe,
+                         double* iou3d, int* status, void* stream) {
+    HN_CHECK(m && x && gt && gt_rows && ce && pe && iou3d && status, "hn_model_eval_cuboid: NULL argument");
+    HN_CHECK(in_channels == 3, "hn_model_eval_cuboid: expects 3-channel panoramas (inference.py:196-200)");
+    HN_CHECK(B >= 1 && B <= 65535 && max_rows >= 8 && max_rows <= 2048, "hn_model_eval_cuboid: bad B or max_rows");
+    HN_CHECK(r_px >= 1 && r_px <= 1024, "hn_model_eval_cuboid: bad r_px");
+    HN_ON_DEVICE(m->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    // inference(net, x, flip, rotate, force_cuboid=True) (eval_cuboid's protocol), its outputs kept on the device
+    constexpr int R = 8;
+    const size_t nf = (size_t)B * (2 * 1024 + 1024 + R * 2 + 2);
+    float* buf = nullptr;
+    int* ibuf = nullptr;
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&buf), nf * sizeof(float), st));
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&ibuf), (size_t)B * 2 * sizeof(int), st));
+    float* y_bon = buf;
+    float* y_cor = y_bon + (size_t)B * 2 * 1024;
+    float* cor_id = y_cor + (size_t)B * 1024;
+    float* z0 = cor_id + (size_t)B * R * 2;
+    float* z1 = z0 + B;
+    int rc = infer_views(m, x, B, flip, shifts, n_rotate, y_bon, y_cor, st, "hn_model_eval_cuboid");
+    if (!rc) rc = layout_postproc(y_bon, y_cor, B, r_px, min_v, 1, 0, R, cor_id, ibuf, z0, z1, ibuf + B, nullptr, nullptr, st);
+    // a failed inference has no cuboid to score (status HN_CUBOID_DT_FAILED)
+    if (!rc) rc = layout_eval_cuboid(cor_id, ibuf, ibuf + B, R, nullptr, nullptr, z0, z1, gt, gt_rows, max_rows, B, ce, pe,
+                                     iou3d, status, st);
+    cudaFreeAsync(buf, st);
+    cudaFreeAsync(ibuf, st);
+    return rc;
+}
+
 int hn_model_stage(hn_model* m, const char* stage, float* out, long long capacity, int dims[4], void* stream) {
     HN_CHECK(m && stage && out && dims, "hn_model_stage: NULL argument");
     HN_CHECK(m->last_batch > 0, "hn_model_stage: no forward has run yet");

@@ -42,6 +42,11 @@ int layout_postproc(const float* y_bon_pix, const float* y_cor, int B, int r_px,
 int layout_eval_general(const float* dt, const int* dt_rows, const int* dt_status, int dt_max_rows, const float* gt,
                         const int* gt_rows, int gt_max_rows, int B, double* iou2d, double* iou3d, double* rmse,
                         double* delta_1, int* status, float* depth_out, cudaStream_t st);
+// Cuboid evaluation (layout_cuboid.cu): eval_cuboid's metrics of B (dt, gt) pairs; z0 / z1 float64, or (NULL) z0f / z1f
+// float32 per pair; dt_status may be NULL
+int layout_eval_cuboid(const float* dt, const int* dt_rows, const int* dt_status, int dt_max_rows, const double* z0,
+                       const double* z1, const float* z0f, const float* z1f, const float* gt, const int* gt_rows,
+                       int gt_max_rows, int B, double* ce, double* pe, double* iou3d, int* status, cudaStream_t st);
 int pano_stretch_device(const float* img, float* out, int n, int H, int W, int C, const double* kx_dev,
                         const double* ky_dev, double* scratch, int order, cudaStream_t st);
 int pano_stretch_device_f64(const double* img, double* out, int n, int H, int W, int C, const double* kx_dev,

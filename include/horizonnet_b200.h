@@ -277,6 +277,40 @@ int hn_model_validate(hn_model* m, const float* x_dev, int B, int in_channels, c
                       int max_rows, double* iou2d_dev, double* iou3d_dev, double* rmse_dev, double* delta_1_dev,
                       int* status_dev, void* stream);
 
+/* ---- cuboid evaluation (reference eval_cuboid.py:13-145 test / eval_3diou), on the device ---------------------------
+ *
+ * B (dt, gt) pairs of cuboid corner lists, each padded to max_rows (8..2048) rows of [x, y] fp32 on the device: dt
+ * [B][max_rows][2] normalised by W and H, as hn_layout_postproc leaves it (scaled by (1024, 512) in fp32 inside,
+ * eval_cuboid.py:192-194), with dt_rows [B]; gt [B][max_rows][2] in pixels, as the label_cor txt files hold them, with
+ * gt_rows [B]; z0 [B], z1 [B] fp64 (the json floats of inference.py).  dt_status [B] (NULL to skip): the
+ * hn_layout_postproc status of each dt.  Only 1024 x 512 panoramas: eval_3diou and pano_connect_points hard-code that
+ * size.  Outputs (device, fp64): ce, pe (percent) and iou3d (percent) [B], and status [B]:
+ *   HN_CUBOID_OK 0; where the reference raises, with all outputs NaN, the first exception in its order:
+ *   HN_CUBOID_ERR_ROWS 1 (dt or gt is not 8 rows -- a deliberate restriction: with two equal row counts other than 8 the
+ *   reference raises IndexError or scores the first 8 rows in PE, which is not a cuboid metric; with two different
+ *   counts it raises ValueError), HN_CUBOID_ERR_INDEX 2 (a mark of the label surfaces rounds to a row >= 512 or
+ *   < -512, or is NaN: IndexError; also a non-finite column or a boundary no wall samples), HN_CUBOID_ERR_COLUMNS 3
+ *   (ceiling and floor columns differ: eval_3diou's AssertionError), HN_CUBOID_ERR_HULL 4 (qhull refuses: an unbounded
+ *   or flat region, a NaN corner, a plane through the camera); HN_CUBOID_DT_FAILED 5: dt_status is 2..5, there is no
+ *   cuboid to score.  The 3D IoU clips a box by the reference's oriented planes (DESIGN.md section 10). */
+#define HN_CUBOID_OK 0
+#define HN_CUBOID_ERR_ROWS 1
+#define HN_CUBOID_ERR_INDEX 2
+#define HN_CUBOID_ERR_COLUMNS 3
+#define HN_CUBOID_ERR_HULL 4
+#define HN_CUBOID_DT_FAILED 5
+int hn_layout_eval_cuboid(const float* dt_dev, const int* dt_rows_dev, const int* dt_status_dev, const double* z0_dev,
+                          const double* z1_dev, const float* gt_dev, const int* gt_rows_dev, int B, int max_rows,
+                          double* ce_dev, double* pe_dev, double* iou3d_dev, int* status_dev, void* stream);
+
+/* The README's cuboid protocol for B panoramas: hn_model_infer_layout with force_cuboid = 1 (flip / shifts_host /
+ * n_rotate / r_px / min_v as there), then hn_layout_eval_cuboid of its device outputs against gt [B][max_rows][2]
+ * (pixels) / gt_rows [B], z1 taken from the fp32 inference result.  A failed inference gives HN_CUBOID_DT_FAILED.
+ * Outputs as hn_layout_eval_cuboid's.  Needs B * views <= max_batch. */
+int hn_model_eval_cuboid(hn_model* m, const float* x_dev, int B, int in_channels, int flip, const int* shifts_host,
+                         int n_rotate, int r_px, float min_v, const float* gt_dev, const int* gt_rows_dev, int max_rows,
+                         double* ce_dev, double* pe_dev, double* iou3d_dev, int* status_dev, void* stream);
+
 /* ---- dataset.PanoCorBonDataset.__getitem__, image path (reference dataset.py:53, 69-105, 124) ------
  *
  * One fused gather pass per image:  uint8 HWC / 255 -> pano_stretch(kx, ky) -> flip -> roll(dx) -> ** gamma -> CHW:
