@@ -8,7 +8,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libhorizonnet_b200.so')
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 _lib = None
 _lock = threading.Lock()
@@ -98,6 +98,15 @@ SIGNATURES = {
                   [vp, ctypes.c_int, ctypes.c_int, vp]),
     'hn_lstm_layer': (ctypes.c_int, [vp, vp, vp, vp, ctypes.c_int, ctypes.c_int, vp]),
     'hn_lstm_plan': (ctypes.c_int, [ctypes.c_int] * 3 + [c_int_p]),
+    'hn_stem': (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, ctypes.c_int, ctypes.c_int, vp, vp]),
+    'hn_maxpool': (ctypes.c_int, [vp] + [ctypes.c_int] * 5 + [vp, vp]),
+    'hn_maxpool_backward': (ctypes.c_int, [vp, vp] + [ctypes.c_int] * 4 + [vp, vp]),
+    'hn_feature_sequence': (ctypes.c_int, [ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(vp), ctypes.c_int, vp, vp]),
+    'hn_feature_sequence_backward': (ctypes.c_int, [ctypes.c_char_p, ctypes.c_int, vp, ctypes.POINTER(vp), vp]),
+    'hn_linear_head': (ctypes.c_int, [vp] * 5 + [ctypes.c_int] * 3 + [vp]),
+    'hn_linear_head_backward': (ctypes.c_int, [vp] * 7 + [ctypes.c_int] * 3 + [vp]),
+    'hn_col_sum': (ctypes.c_int, [vp, ctypes.c_longlong, ctypes.c_int, vp, vp]),
+    'hn_stem_input': (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_int, vp, vp]),
 }
 
 

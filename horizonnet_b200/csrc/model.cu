@@ -11,6 +11,7 @@
 #include <atomic>
 
 #include "model.cuh"
+#include "bwd_kernels.cuh"
 #include "../../include/horizonnet_b200.h"
 
 #ifndef HN_BUILD_DIGEST
@@ -317,7 +318,7 @@ int refold_bn(hn_model* m, cudaStream_t st) {
 extern "C" {
 
 const char* hn_last_error(void) { return g_err.c_str(); }
-int hn_abi_version(void) { return 10; }
+int hn_abi_version(void) { return 11; }
 const char* hn_build_digest(void) { return HN_BUILD_DIGEST; }
 long long hn_kernel_launches(void) { return g_launches.load(); }
 
@@ -1316,6 +1317,111 @@ int hn_lstm_layer(const float* xproj, const float* whf, const float* whb, float*
 int hn_lstm_plan(int T, int B, int max_clusters, int plan[7]) {
     HN_CHECK(plan, "hn_lstm_plan: NULL argument");
     return lstm_plan(T, B, max_clusters, plan);
+}
+
+// The stem as the model runs it: impl 0 = stem_f32 on the weights packed as pack_conv packs them; impl 1 = the weight
+// planes and epilogue constants of stem_tc_pack_weights (as finalize makes them) and stem_tc.  relu = 0 with ones / zeros
+// is the training step's raw pass: there tc_aux_update(ones, zeros) replaces the constants of weights packed with the BN
+// scale, and the planes depend on the weights alone (their power of two), so packing with ones / zeros gives the same
+// planes and the same constants.
+int hn_stem(const float* x_nchw, int B, int in_channels, const float* w_oihw, const float* scale, const float* shift,
+            int relu, int impl, float* out, void* stream) {
+    HN_CHECK(x_nchw && w_oihw && scale && shift && out, "hn_stem: NULL argument");
+    HN_CHECK(B >= 1 && B <= 2048 && in_channels >= 3, "hn_stem: bad geometry");
+    HN_CHECK(impl == 0 || impl == 1, "hn_stem: impl must be 0 or 1");
+    cudaStream_t st = (cudaStream_t)stream;
+    const Act o = mk(out, B, 256, 512, 64);
+    if (impl == 0) {
+        float* wp = nullptr;
+        HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&wp), 64 * 147 * sizeof(float), st));
+        pack_oihw_kernel<<<(64 * 147 + 255) / 256, 256, 0, st>>>(w_oihw, wp, 64, 3, 7, 7);
+        count_launch();
+        int rc = cudaGetLastError() != cudaSuccess ? fail("hn_stem: weight packing failed") : 0;
+        if (!rc) rc = stem_f32(x_nchw, B, in_channels, wp, scale, shift, o, st, relu != 0);
+        cudaFreeAsync(wp, st);
+        return rc;
+    }
+    // one scratch block: packed input planes | weight planes [2][64][224] | padded weights [64][224] | tc_aux [3*64+1]
+    const size_t n_planes = stem_tc_scratch_bytes(B), n_wq = 2 * 64 * 224 * sizeof(unsigned short);
+    const size_t n_pad = 64 * 224 * sizeof(float), n_aux = (3 * 64 + 1) * sizeof(float);
+    uint8_t* scratch = nullptr;
+    HN_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&scratch), n_planes + n_wq + n_pad + n_aux, st));
+    unsigned short* planes = reinterpret_cast<unsigned short*>(scratch);
+    unsigned short* wq = reinterpret_cast<unsigned short*>(scratch + n_planes);
+    float* pad = reinterpret_cast<float*>(scratch + n_planes + n_wq);
+    float* aux = reinterpret_cast<float*>(scratch + n_planes + n_wq + n_pad);
+    int rc = stem_tc_pack_weights(w_oihw, pad, wq, scale, shift, aux, st);
+    if (!rc) rc = stem_tc(x_nchw, B, in_channels, wq, aux, shift, planes, o, st, relu != 0);
+    cudaFreeAsync(scratch, st);
+    return rc;
+}
+
+int hn_maxpool(const float* in, int B, int H, int W, int C, int out_planes, float* out, void* stream) {
+    HN_CHECK(in && out && B >= 1 && H >= 1 && W >= 1 && C >= 4, "hn_maxpool: bad argument");
+    return maxpool3x3s2(mk(const_cast<float*>(in), B, H, W, C), mk(out, B, (H - 1) / 2 + 1, (W - 1) / 2 + 1, C),
+                        (cudaStream_t)stream, out_planes != 0);
+}
+
+int hn_maxpool_backward(const float* x, const float* dp, int B, int H, int W, int C, float* dx, void* stream) {
+    HN_CHECK(x && dp && dx && B >= 1 && H >= 1 && W >= 1 && C >= 1, "hn_maxpool_backward: bad argument");
+    return maxpool_bwd(mk(const_cast<float*>(x), B, H, W, C), mk(const_cast<float*>(dp), B, (H - 1) / 2 + 1, (W - 1) / 2 + 1, C),
+                       dx, (cudaStream_t)stream);
+}
+
+namespace {
+// The four height-reduction outputs of an encoder as build_graph makes them: C/8 channels of layer s at H = 8 >> s,
+// W = 256 >> s (halo 1)
+int ghc_outputs(const char* backbone, int B, float* const p[4], Act a[4]) {
+    HN_CHECK(backbone && B >= 1, "feature sequence: bad argument");
+    const Arch* arch = nullptr;
+    for (const Arch& c : ARCHS)
+        if (std::string(backbone) == c.name) arch = &c;
+    HN_CHECK(arch, std::string("feature sequence: unknown backbone ") + backbone);
+    for (int s = 0; s < 4; ++s) {
+        HN_CHECK(p[s], "feature sequence: NULL argument");
+        a[s] = mk(p[s], B, 8 >> s, 256 >> s, (64 << s) * arch->expansion / 8);
+    }
+    return 0;
+}
+}  // namespace
+
+int hn_feature_sequence(const char* backbone, int B, const float* const ghc[4], int planes, float* seq, void* stream) {
+    HN_CHECK(ghc && seq, "hn_feature_sequence: NULL argument");
+    Act a[4];
+    float* const p[4] = {const_cast<float*>(ghc[0]), const_cast<float*>(ghc[1]), const_cast<float*>(ghc[2]),
+                         const_cast<float*>(ghc[3])};
+    if (ghc_outputs(backbone, B, p, a)) return -1;
+    return ghc_to_sequence(a, seq, (cudaStream_t)stream, planes != 0);
+}
+
+int hn_feature_sequence_backward(const char* backbone, int B, const float* dseq, float* const dghc[4], void* stream) {
+    HN_CHECK(dseq && dghc, "hn_feature_sequence_backward: NULL argument");
+    Act a[4];
+    if (ghc_outputs(backbone, B, dghc, a)) return -1;
+    return ghc_to_sequence_bwd(dseq, a, (cudaStream_t)stream);
+}
+
+int hn_linear_head(const float* rnn, const float* w, const float* b, float* bon, float* cor, int T, int B, int K,
+                   void* stream) {
+    HN_CHECK(rnn && w && b && bon && cor && T >= 1 && T <= 256 && B >= 1, "hn_linear_head: bad argument");
+    return linear_head(rnn, w, b, bon, cor, T, B, K, (cudaStream_t)stream);
+}
+
+int hn_linear_head_backward(const float* dbon, const float* dcor, const float* rnn, const float* w, float* drnn, float* dw,
+                            float* db, int T, int B, int K, void* stream) {
+    HN_CHECK(dbon && dcor && rnn && w && drnn && dw && db && T >= 1 && T <= 256 && B >= 1,
+             "hn_linear_head_backward: bad argument");
+    return head_bwd(dbon, dcor, rnn, w, drnn, dw, db, T, B, K, (cudaStream_t)stream);
+}
+
+int hn_col_sum(const float* x, long long rows, int cols, float* out, void* stream) {
+    HN_CHECK(x && out && rows >= 0 && cols >= 1, "hn_col_sum: bad argument");
+    return col_sum(x, (size_t)rows, cols, out, (cudaStream_t)stream);
+}
+
+int hn_stem_input(const float* x_nchw, int in_channels, int B, float* out, void* stream) {
+    HN_CHECK(x_nchw && out && in_channels >= 3 && B >= 1, "hn_stem_input: bad argument");
+    return stem_input_nhwc(x_nchw, in_channels, out, B, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -430,6 +430,38 @@ int hn_lstm_layer(const float* xproj_dev, const float* w_hh_fwd_dev, const float
  * -1 for T < 1, B < 1 or max_clusters < 2 (the device hn_lstm_layer refuses). */
 int hn_lstm_plan(int T, int B, int max_clusters, int plan[7]);
 
+/* Kernels at the two ends of the network, each through the library function the model calls (unit tests; asynchronous on
+ * `stream`, scratch from cudaMallocAsync on it).  Halo-1 NHWC fp32 tensors unless said otherwise.
+ * Stem: x [B][in_channels >= 3][512][1024] in [0, 1] (channels past 3 are not read), w OIHW [64][3][7][7], scale / shift
+ * [64] -> out [B][256][514][64].  impl 0: stem_kernel (fp32; writes the wrap columns too); impl 1: stem_pack_kernel +
+ * stem_tc_kernel (split-fp16 wgmma; interior columns only).  relu = 0 gives the raw conv * scale + shift of the training
+ * step's statistics pass (with ones / zeros: the same weight planes and epilogue constants it runs with). */
+int hn_stem(const float* x_nchw, int B, int in_channels, const float* w_oihw, const float* scale, const float* shift,
+            int relu, int impl, float* out, void* stream);
+/* MaxPool2d(3, 2, 1) with -inf padding: in [B][H][W+2][C] -> out [B][(H+1)/2][(W+1)/2+2][C], C a multiple of 4;
+ * out_planes = 1 writes split planes (fp16 hi / lo of v * 2^-4, hi plane first) in the same bytes instead of fp32. */
+int hn_maxpool(const float* in, int B, int H, int W, int C, int out_planes, float* out, void* stream);
+/* Its backward: each output gradient dp is ADDED (atomically) to the first maximum of its window in scan order; dx has x's
+ * geometry and its halo columns are not written. */
+int hn_maxpool_backward(const float* x, const float* dp, int B, int H, int W, int C, float* dx, void* stream);
+/* The feature sequence (model.py:152-155, 175-178, 263) of backbone "resnet50" (c_last 1024) or "resnet18" (256) from the
+ * four height-reduction outputs ghc[s] [B][8 >> s][(256 >> s) + 2][C_s], C_s = the layer's channels / 8, into
+ * seq [256][B][c_last]; planes = 1: inputs and output are split planes.  The backward ADDS the adjoint of d seq to the
+ * interior columns of dghc (atomically). */
+int hn_feature_sequence(const char* backbone, int B, const float* const ghc[4], int planes, float* seq, void* stream);
+int hn_feature_sequence_backward(const char* backbone, int B, const float* dseq, float* const dghc[4], void* stream);
+/* Linear(K -> 12) head, K = 1024 (bi-LSTM) or 512 (MLP), over rows t*B + b of rnn [T][B][K] with w [12][K], b [12]:
+ * output o = 4s + k of row (t, b) goes to column 4t + k of cor [B][1][1024] (s = 0) or bon [B][2][1024] (s = 1, 2).  The
+ * backward writes drnn [T][B][K], dw [12][K] and db [12]. */
+int hn_linear_head(const float* rnn, const float* w, const float* b, float* bon, float* cor, int T, int B, int K,
+                   void* stream);
+int hn_linear_head_backward(const float* dbon, const float* dcor, const float* rnn, const float* w, float* drnn, float* dw,
+                            float* db, int T, int B, int K, void* stream);
+/* out[c] = sum over the rows of x [rows][cols] (the bias gradients of the LSTM and the MLP head). */
+int hn_col_sum(const float* x, long long rows, int cols, float* out, void* stream);
+/* The stem's weight-gradient operand: x as above -> the normalised input, halo-3 NHWC [B][512][1030][3]. */
+int hn_stem_input(const float* x_nchw, int in_channels, int B, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

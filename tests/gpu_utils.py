@@ -641,3 +641,113 @@ def lstm_run(xproj, W, dev='cuda:0'):
     assert torch.isfinite(out).all(), 'non-finite output'
     assert bool((buf[n:] == CANARY).all()), 'write past the end of the output'
     return out
+
+
+# ---- split planes (conv_tc.cuh split_scaled / merge_scaled) emulated in torch: s = v * 2^-4 clamped to the fp16 range,
+# hi = fp16(s) and lo = fp16(s - hi), both rounded to nearest even.  Returns the two int16 bit patterns.
+def split_planes_torch(v):
+    s = (v.float() * 0.0625).clamp(-65504.0, 65504.0)
+    hi = s.half()
+    lo = (s - hi.float()).half()
+    return hi.view(torch.int16), lo.view(torch.int16)
+
+
+def merge_planes_torch(hi, lo):
+    return (hi.view(torch.float16).float() + lo.view(torch.float16).float()) * 16.0
+
+
+# ---- the stem (conv_f32.cu: stem_kernel; conv_tc.cu: stem_pack_kernel + stem_tc_kernel): normalise, 7x7 stride-2 conv
+# with circular W / zero H padding 3, y = conv * scale + shift (ReLU in eval, none in the training step's raw pass).
+# The kernels normalise in fp32 with fp32 constants; the fp64 reference normalises the same fp32 constants in fp64, and the
+# fp32 rounding of (x - mean) / std is 2^-23 |x^| at most:  2^-23 * (|x^| conv |w|) * |scale|.
+# Tensor-core stem, in the terms of run_tc_case:
+#  * the input plane is 16 x^ (exact), its lo plane normal above |x^| = 2^-7: 2^-22 |x^|; below, the lo plane rounds to
+#    half its subnormal spacing, 2^-25 / 16 = 2^-29 of x^ (2^-27 with a 4x margin):  2^-27 * (1 conv |w|) per output;
+#  * the weights are split at the per-tensor power of two 2^t of pack_weight_tc (max|w| 2^t in (2^13, 2^14]): 2^-22 |w|
+#    for a normal lo, else 2^-25 2^-t < 2^-38 max|w| absolute (2^-36 with a 4x margin):  2^-36 max|w| * (|x^| conv 1);
+#  * the dropped lo*lo (2^-22 |x^ w|) and the fp32 accumulation of 42 MMAs (14 K-steps x 3 products) in the tensor
+#    cores, which is not round-to-nearest: with the operand terms, C_STEM_TC * 2^-21 * (|x^| conv |w|);
+#  * the epilogue is one fmaf with the exact power-of-two rescale, after the accumulator's own last rounding: 2^-24 |y|
+#    each.  Where the products are exact (8-bit inputs, power-of-two-scaled filters) or the scale is small and the shift
+#    large, these roundings are all of the error, so the term carries the 3x margin itself:  2^-22 |y|.
+# The fp32 stem (147 fmaf per output in fp32, then the epilogue fmaf): the terms of run_f32_conv's bound with its own
+# constant, C_STEM_F32 * 2^-24 * (sum|a*w| * |scale| + |shift|), and the same 2^-22 |y| output term.
+# Worst err / bound on an H100 80GB HBM3 at a 700 W power limit, over every stem case of tests/test_stem_pool_tail.py
+# (B = 1, 2, 3 and images 0, 31, 63 of B = 64): 0.30 for the tensor cores and 0.28 for stem_kernel, both on 8-bit panoramas
+# with checkpoint-like weights; 0.24 and 0.19 on the smallest-output channel of a case.  How the constants were set there:
+#  * with C = 8 of the other tensor-core convolutions and the subnormal terms at 2x (2^-28, 2^-37) the tensor-core stem
+#    reached 0.50 of its bound; C = 12 gave 0.35 and C = 14 0.33, both at uniform inputs near the mean, i.e. the
+#    subnormal lo-plane term was the limit.  With that term at 4x the uniform cases fell to 0.21;
+#  * stem_kernel reached 0.37 of the shared C32 = 48 bound, its accumulation term dominant; C_STEM_F32 = 64 gives 0.28.
+X_MEAN32 = torch.tensor([0.485, 0.456, 0.406], dtype=torch.float32)
+X_STD32 = torch.tensor([0.229, 0.224, 0.225], dtype=torch.float32)
+EPS22, EPS23, EPS27, EPS36 = 2.0 ** -22, 2.0 ** -23, 2.0 ** -27, 2.0 ** -36
+C_STEM_TC, C_STEM_F32 = 14.0, 64.0
+
+
+def normalise_f32(x):
+    """The kernels' normalisation (x - mean) / std in fp32 with fp32 constants, on the first 3 channels (NCHW)."""
+    m, s = X_MEAN32.to(x.device).view(1, 3, 1, 1), X_STD32.to(x.device).view(1, 3, 1, 1)
+    return (x[:, :3] - m) / s
+
+
+def normalise_f64(x):
+    m, s = X_MEAN32.to(x.device).double().view(1, 3, 1, 1), X_STD32.to(x.device).double().view(1, 3, 1, 1)
+    return (x[:, :3].double() - m) / s
+
+
+def stem_reference(x, w, scale, shift, relu):
+    """fp64 stem of x (NCHW fp32, >= 3 channels, any H, W) with folded BN scale / shift: (ref, acc = |x^| conv |w|,
+    ones = 1 conv |w| with the zero H padding, xsum = |x^| conv 1)."""
+    xn, wd = normalise_f64(x), w.double()
+    y = _conv_abs(xn, wd, (2, 2), 3, 3) * scale.double().view(1, -1, 1, 1) + shift.double().view(1, -1, 1, 1)
+    if relu:
+        y = F.relu(y)
+    acc = _conv_abs(xn.abs(), wd.abs(), (2, 2), 3, 3)
+    ones = _conv_abs(torch.ones_like(xn[:1]), wd.abs(), (2, 2), 3, 3)
+    xsum = _conv_abs(xn.abs(), torch.ones_like(wd[:1]), (2, 2), 3, 3)
+    return y, acc, ones, xsum
+
+
+def stem_bound(impl, w, scale, shift, ref, acc, ones, xsum):
+    sc = scale.double().abs().view(1, -1, 1, 1)
+    if impl == 1:
+        wmax = w.abs().max().item()
+        return sc * (C_STEM_TC * EPS21 * acc + EPS23 * acc + EPS27 * ones + EPS36 * wmax * xsum) + EPS22 * ref.abs()
+    return C_STEM_F32 * EPS24 * (acc * sc + shift.double().abs().view(1, -1, 1, 1)) + sc * EPS23 * acc + EPS22 * ref.abs()
+
+
+def run_stem(x, w, scale, shift, relu, impl):
+    """hn_stem into [B][256][514][64] whose interior starts NaN and whose halo columns hold the canary, with the canary
+    behind it; checks that every interior element is written, nothing past the end, and the halo columns: the circular
+    wrap (impl 0) or untouched (impl 1).  Returns the output (halo-NHWC)."""
+    B, Cx = x.shape[:2]
+    dev = x.device
+    n = B * 256 * 514 * 64
+    buf = torch.full((n + 4096,), CANARY, device=dev)
+    out = buf[:n].view(B, 256, 514, 64)
+    out[:, :, 1:-1] = float('nan')
+    _lib.check(_lib.lib().hn_stem(x.data_ptr(), B, Cx, w.data_ptr(), scale.data_ptr(), shift.data_ptr(), int(relu), impl,
+                                  out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream), 'hn_stem')
+    torch.cuda.synchronize(dev)
+    assert not torch.isnan(out[:, :, 1:-1]).any(), f'stem impl {impl}: output elements left unwritten'
+    assert bool((buf[n:] == CANARY).all()), f'stem impl {impl}: write past the end of the output'
+    if impl == 0:
+        assert torch.equal(out[:, :, 0], out[:, :, -2]) and torch.equal(out[:, :, -1], out[:, :, 1]), \
+            'stem impl 0: halo columns are not the circular wrap'
+    else:
+        assert bool((out[:, :, 0] == CANARY).all()) and bool((out[:, :, -1] == CANARY).all()), \
+            'stem impl 1: a halo column was written'
+    return out
+
+
+def stem_ratio(out, x, w, scale, shift, relu, impl):
+    """Worst err / bound of a stem output against fp64, elementwise (so each channel against its own bound), and the
+    worst ratio of the channel whose outputs are smallest."""
+    ref, acc, ones, xsum = stem_reference(x, w, scale, shift, relu)
+    bound = stem_bound(impl, w, scale, shift, ref, acc, ones, xsum)
+    err = (from_halo_nhwc(out, 1).double() - ref).abs()
+    r = torch.where(err == 0, torch.zeros_like(err), err / bound)
+    per_ch = r.amax(dim=(0, 2, 3))
+    small = int(ref.abs().amax(dim=(0, 2, 3)).argmin())
+    return r.max().item(), per_ch[small].item()
