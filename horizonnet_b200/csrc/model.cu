@@ -1001,6 +1001,16 @@ int hn_layout_eval_cuboid(const float* dt, const int* dt_rows, const int* dt_sta
                               iou3d, status, (cudaStream_t)stream);
 }
 
+int hn_train_targets(const float* cor0, const float* cor, const int* rows, const int* flip, const int* dx, int N, int max_rows,
+                     double p_base, float* y_bon, float* y_cor, float* cor_out, int* occlusion, int* status, void* stream) {
+    HN_CHECK(cor0 && cor && rows && flip && dx && y_bon && y_cor && status, "hn_train_targets: NULL argument");
+    HN_CHECK(N >= 1 && N <= 65535, "hn_train_targets: bad sample count");
+    HN_CHECK(max_rows >= 1 && max_rows <= 2048, "hn_train_targets: max_rows must be in 1..2048");
+    HN_CHECK(p_base > 0 && p_base < 1, "hn_train_targets: p_base must be in (0, 1)");
+    return train_targets(cor0, cor, rows, flip, dx, N, max_rows, p_base, y_bon, y_cor, cor_out, occlusion, status,
+                         (cudaStream_t)stream);
+}
+
 int hn_model_eval_cuboid(hn_model* m, const float* x, int B, int in_channels, int flip, const int* shifts, int n_rotate,
                          int r_px, float min_v, const float* gt, const int* gt_rows, int max_rows, double* ce, double* pe,
                          double* iou3d, int* status, void* stream) {

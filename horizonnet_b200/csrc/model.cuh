@@ -47,6 +47,9 @@ int layout_eval_general(const float* dt, const int* dt_rows, const int* dt_statu
 int layout_eval_cuboid(const float* dt, const int* dt_rows, const int* dt_status, int dt_max_rows, const double* z0,
                        const double* z1, const float* z0f, const float* z1f, const float* gt, const int* gt_rows,
                        int gt_max_rows, int B, double* ce, double* pe, double* iou3d, int* status, cudaStream_t st);
+// Training targets (targets.cu): dataset.py's y_bon / y_cor of N samples; cor_out / occlusion may be NULL
+int train_targets(const float* cor0, const float* cor, const int* rows, const int* flip, const int* dx, int N, int max_rows,
+                  double p_base, float* y_bon, float* y_cor, float* cor_out, int* occlusion, int* status, cudaStream_t st);
 int pano_stretch_device(const float* img, float* out, int n, int H, int W, int C, const double* kx_dev,
                         const double* ky_dev, double* scratch, int order, cudaStream_t st);
 int pano_stretch_device_f64(const double* img, double* out, int n, int H, int W, int C, const double* kx_dev,

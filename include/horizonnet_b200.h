@@ -323,6 +323,30 @@ int hn_augment(const unsigned char* img_u8_dev, float* out_chw_dev, int n, int h
                const double* kx_host, const double* ky_host, const int* flip_host, const int* dx_host,
                const float* gamma_host, void* stream);
 
+/* ---- dataset.PanoCorBonDataset.__getitem__, label path (reference dataset.py:56-67, 84-120) -----------------------
+ *
+ * The training targets of N samples, on the device.  cor0 [N][max_rows][2] fp32: the corner lists as read (pixels,
+ * rolled so the ceiling corner with the smallest x comes first, dataset.py:62); cor [N][max_rows][2] fp32: the same
+ * corners after the stretch (cor0 itself without one); rows [N]; flip [N] (0 / 1); dx [N] (the np.roll shift,
+ * 0 <= dx < 1024, or < 0 for no roll).  max_rows <= 2048, 0 < p_base < 1.  Only 1024 x 512 panoramas.  Outputs (device):
+ * y_bon [N][2][1024] fp32 (cor_2_1d of cor, then flipped and rolled), y_cor [N][1][1024] fp32 (p_base ** the circular
+ * distance to the nearest corner the camera sees), cor_out [N][max_rows][2] fp32 (cor flipped and rolled; NULL to skip)
+ * and occlusion [N][max_rows] (find_occlusion of the ceiling corners of cor0, repeated to both rows of each corner; NULL
+ * to skip) -- both written for every sample whose status is not ERR_ROWS or ERR_CORNERS -- and status [N]:
+ *   HN_TARGETS_OK 0; where the reference raises, with y_bon and y_cor NaN, the first exception in its order:
+ *   HN_TARGETS_ERR_ROWS 1 (an odd row count, or one outside 1..max_rows), HN_TARGETS_ERR_CORNERS 2 (fewer than 3 ceiling
+ *   corners: shapely refuses the one-point polyline of the other corners), HN_TARGETS_ERR_BOUNDARY 3 (a boundary no wall
+ *   samples: ys.max() of nothing), HN_TARGETS_ERR_OCCLUDED 4 (every corner occluded: dist.min(0) of nothing).
+ * The occlusion test is exact on the fp32 floor-plane points (DESIGN.md section 11). */
+#define HN_TARGETS_OK 0
+#define HN_TARGETS_ERR_ROWS 1
+#define HN_TARGETS_ERR_CORNERS 2
+#define HN_TARGETS_ERR_BOUNDARY 3
+#define HN_TARGETS_ERR_OCCLUDED 4
+int hn_train_targets(const float* cor0_dev, const float* cor_dev, const int* rows_dev, const int* flip_dev,
+                     const int* dx_dev, int N, int max_rows, double p_base, float* y_bon_dev, float* y_cor_dev,
+                     float* cor_out_dev, int* occlusion_dev, int* status_dev, void* stream);
+
 /* ---- misc.pano_lsd_align.rotatePanorama (reference misc/pano_lsd_align.py:125-171, warpImageFast :101-122) ----
  *
  * n images [h][w][c] on the device, float32 (in_is_f64 = 0) or float64 (1) -> n float64 images [h][w][c] rotated by
