@@ -290,4 +290,21 @@ CASES = [
     launch('r50.mlp.linear.0_b1_tc', 'conv', 1, 1, 64, 64, 512, 1, (1, 1), in_halo=0, out_halo=0, relu=True),
     launch('r50.mlp.linear.0_b32_tc', 'conv', 1, 1, 4352, 64, 512, 1, (1, 1), in_halo=0, out_halo=0, relu=True),
     launch('r50.stem:wgrad_b1_tc', 'wgrad', 1, 4, 1024, 3, 64, 7, (2, 2), in_halo=3),
+    # batches between those above and past 64 (132 SMs, then 114 SMs)
+    launch('r18.layer2.0.downsample:wgrad_b15_f32', 'wgrad', 1, 24, 256, 64, 128, 1, (2, 2)),
+    launch('r50.bi_rnn.weight_ih_l1_b35_f32', 'wgrad', 1, 1, 272, 128, 2048, 1, (1, 1), in_halo=0, out_halo=0, kind='lstm'),
+    launch('r50.layer1.0.conv1:wgrad_b55_f32', 'wgrad', 1, 11, 256, 64, 64, 1, (1, 1)),
+    launch('r50.ghc3.2_b65_f32', 'conv', 65, 4, 32, 16, 512, 3, (2, 1), relu=True),
+    launch('r50.ghc3.2:raw_b65_f32', 'conv', 65, 4, 32, 16, 512, 3, (2, 1)),
+    launch('r50.ghc3.3:dgrad_b65_f32', 'dgrad', 65, 2, 32, 512, 256, 3, (2, 1), kind='grad'),
+    launch('r18.ghc3.3_b525_f32', 'conv', 525, 2, 32, 16, 64, 3, (2, 1), relu=True),
+    launch('r18.ghc3.3:raw_b525_f32', 'conv', 525, 2, 32, 16, 64, 3, (2, 1)),
+    launch('r18.layer2.0.downsample:wgrad_b15_f32_h20', 'wgrad', 1, 20, 256, 64, 128, 1, (2, 2)),
+    launch('r50.layer1.0.conv1:wgrad_b15_f32', 'wgrad', 1, 10, 256, 64, 64, 1, (1, 1)),
+    launch('r50.layer1.0.conv2:wgrad_b25_f32', 'wgrad', 1, 2, 256, 64, 64, 3, (1, 1)),
+    launch('r50.ghc3.2_b57_f32', 'conv', 57, 4, 32, 16, 512, 3, (2, 1), relu=True),
+    launch('r50.ghc3.2:raw_b57_f32', 'conv', 57, 4, 32, 16, 512, 3, (2, 1)),
+    launch('r50.ghc3.3:dgrad_b57_f32', 'dgrad', 57, 2, 32, 512, 256, 3, (2, 1), kind='grad'),
+    launch('r18.ghc3.3_b453_f32', 'conv', 453, 2, 32, 16, 64, 3, (2, 1), relu=True),
+    launch('r18.ghc3.3:raw_b453_f32', 'conv', 453, 2, 32, 16, 64, 3, (2, 1)),
 ]

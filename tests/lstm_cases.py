@@ -1,9 +1,9 @@
 """Launches of the bi-LSTM recurrence (lstm_cluster.cu: lstm_cluster_kernel) and the layouts lstm_layer gives them (no GPU
 needed).
 
-* model_launches -- every recurrence launch of the model at one batch: the eval forward (model.cu forward_rnn), the
-                    training forward (train_step.cu) and TTA (hn_model_infer_tta: up to 64 views in one forward), each
-                    with both layers at T = 256;
+* model_launches -- every recurrence launch of the model at one batch (any in tc_cases.ACCEPTED_BATCHES, 1 .. 1024): the
+                    eval forward (model.cu forward_rnn), the training forward (train_step.cu) and TTA (hn_model_infer_tta:
+                    up to 64 views in one forward), each with both layers at T = 256;
 * abi_launches   -- hn_lstm_layer takes any T >= 1: T = 1 (no exchange at all), 2 (one exchange, no re-arming) and 3
                     (an odd T);
 * plan / variant_key -- hn_lstm_plan and the paths of the kernel a layout takes: one or two 8-column groups per cluster,
@@ -17,11 +17,11 @@ has not been measured, so the census takes every count from 2 (the least hn_lstm
 import ctypes
 
 from horizonnet_b200 import _lib
+from tc_cases import ACCEPTED_BATCHES
 
 PLAN_FIELDS = ('max_clusters', 'ngroups', 'gpc', 'clusters', 'last_cluster_groups', 'last_group_cols', 'waves')
 KEY_FIELDS = ('gpc', 'multi_cluster', 'last_cluster_one_group', 'partial_group', 'second_wave', 'T')
 MAX_CLUSTERS = tuple(range(2, 9))
-BATCHES = tuple(range(1, 65))          # the training step's and TTA's largest batch is 64
 MODEL_T = 256
 T_CLASSES = ('1', '2', 'odd', 'even')
 # the T each unit case runs at: odd T = 5 is the first odd T whose waits reuse a barrier phase (step 3 waits for h_2 on
@@ -98,20 +98,21 @@ LAYOUTS = [
     (2, True, True, False, False),       # B = 40 (6-8 clusters)
     (2, True, False, True, False),       # B = 25 (4-7 clusters)
     (2, True, False, False, False),      # B = 32 (4-7 clusters): the benchmark's batch
-    (2, True, True, True, True),         # B = 49 (6-7 clusters): a second wave, its last cluster one 1-column group
-    (2, True, True, False, True),        # B = 56 (6-7 clusters)
-    (2, True, False, True, True),        # B = 57 (6-7 clusters)
-    (2, True, False, False, True),       # B = 64 (6-7 clusters): the training step's largest batch
+    # a second wave (8 clusters: from B = 65 on), its last cluster one 1-column group
+    (2, True, True, True, True),         # B = 49 (6-7 clusters; 8: B = 65)
+    (2, True, True, False, True),        # B = 56 (6-7 clusters; 8: B = 72)
+    (2, True, False, True, True),        # B = 57 (6-7 clusters; 8: B = 73)
+    (2, True, False, False, True),       # B = 64 (6-7 clusters; 8: B = 80)
 ]
 CASES = [key_name(lay + (tc,)) for lay in LAYOUTS for tc in T_CLASSES]
 CASE_KEYS = {key_name(lay + (tc,)): lay + (tc,) for lay in LAYOUTS for tc in T_CLASSES}
 
 
 def batch_for(key, max_clusters):
-    """The smallest batch (1 .. 64) whose layout at the key's T has the key on a device with max_clusters co-resident
+    """The smallest batch (1 .. 1024) whose layout at the key's T has the key on a device with max_clusters co-resident
     clusters, or None when no batch of the model reaches it there."""
     T = T_FOR_CLASS[key[5]]
-    for B in BATCHES:
+    for B in ACCEPTED_BATCHES:
         p = plan(T, B, max_clusters)
         if p is not None and variant_key(T, p) == key:
             return B

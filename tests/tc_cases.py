@@ -8,7 +8,7 @@
                         stride-1 conv);
 * plan / variant_key -- hn_conv_tc_plan and the code paths of conv_tc.cu a plan selects;
 * CASES              -- the unit cases of test_tc_kernels.py; test_conv_tc_plan.py checks that they reach every variant
-                        key the model reaches."""
+                        key the model reaches at every batch in ACCEPTED_BATCHES."""
 import ctypes
 
 from horizonnet_b200 import _lib
@@ -16,7 +16,8 @@ from horizonnet_b200._spec import BACKBONES, c_last
 
 SMS = 132                     # H100 SXM
 SM_COUNTS = (132, 114)        # H100 SXM, H100 PCIe
-BATCHES = (1, 2, 3, 8, 16, 32, 64)
+BATCHES = (1, 2, 3, 8, 16, 32, 64)          # the batches the -m gpu tests run the model at
+ACCEPTED_BATCHES = range(1, 1025)           # every max_batch hn_model_create_arch accepts: the host censuses plan them all
 PLAN_FIELDS = ('gemm_kernel', 'BN', 'mode', 'M', 'tw', 'rows_per_tile', 'wsegs', 'rowbox', 'box_rows', 'box_imgs', 'dxr',
                'parity', 'num_kc', 'seg', 'pf', 'n_tiles', 'num_tiles', 'grid')
 
@@ -176,7 +177,7 @@ F32_CASES = [
     case('f32_s22', 2, 32, 64, 128, 128, 3, (2, 2), out_f32=True),
 ]
 
-# The cheapest launch of the model (batch 1 .. 64; input channels cut where the plan stays the same) for each variant key
+# The cheapest launch of the model (batch 1 .. 1024; input channels cut where the plan stays the same) for each variant key
 # the cases above leave out at 132 or 114 SMs, named after the layer.  out_f32 = the training step's raw pass, its data gradients
 # (":dgrad": the transposed conv of train_step.cu) and the LSTM projections, all run here through hn_conv2d impl = 2.
 MODEL_CASES = [
@@ -277,6 +278,60 @@ MODEL_CASES = [
     case('r18.layer4.0.downsample_raw_b1', 1, 32, 64, 256, 512, 1, (2, 2), out_f32=True),
     case('r18.layer4.0.downsample_raw_b16', 9, 32, 64, 64, 512, 1, (2, 2), out_f32=True),
     case('r18.layer4.0.downsample_raw_b8', 5, 32, 64, 64, 512, 1, (2, 2), out_f32=True),
+    # batches between those above and past 64, each named after the first batch that reaches its key; input channels cut
+    # where the key stays.  Past 64 only the small height-reduction convs (ghc2.3, ghc3.2, ghc3.3) change their path:
+    # more tiles than CTAs (multi_tile), and BN 128 once the 64-channel tiles alone would fill the grid.
+    # 132 SMs
+    case('ghc3.2_b33', 33, 4, 32, 256, 512, 3, (2, 1)),
+    case('ghc3.2_raw_b33', 33, 4, 32, 256, 512, 3, (2, 1), out_f32=True),
+    case('ghc3.3_dgrad_b33', 33, 2, 32, 256, 512, 3, (1, 1), out_f32=True),
+    case('ghc3.2_b67', 67, 4, 32, 256, 512, 3, (2, 1)),
+    case('ghc3.2_raw_b67', 67, 4, 32, 256, 512, 3, (2, 1), out_f32=True),
+    case('ghc3.3_dgrad_b67', 67, 2, 32, 256, 512, 3, (1, 1), out_f32=True),
+    case('ghc3.3_b133', 133, 2, 32, 256, 256, 3, (2, 1)),
+    case('ghc3.3_raw_b133', 133, 2, 32, 256, 256, 3, (2, 1), out_f32=True),
+    case('ghc3.3_b217', 217, 2, 32, 256, 256, 3, (2, 1)),
+    case('ghc3.3_raw_b217', 217, 2, 32, 256, 256, 3, (2, 1), out_f32=True),
+    case('ghc3.3_b265', 265, 2, 32, 256, 256, 3, (2, 1)),
+    case('ghc3.3_raw_b265', 265, 2, 32, 256, 256, 3, (2, 1), out_f32=True),
+    case('r18.layer3.0.conv1_b4', 4, 64, 128, 64, 256, 3, (2, 2)),
+    case('r18.layer3.0.conv1_raw_b4', 4, 64, 128, 64, 256, 3, (2, 2), out_f32=True),
+    case('r18.ghc2.1_b17', 17, 16, 64, 64, 128, 3, (2, 1)),
+    case('r18.ghc2.1_raw_b17', 17, 16, 64, 64, 128, 3, (2, 1), out_f32=True),
+    case('r18.ghc2.3_b133', 133, 4, 64, 64, 32, 3, (2, 1)),
+    case('r18.ghc2.3_raw_b133', 133, 4, 64, 64, 32, 3, (2, 1), out_f32=True),
+    case('r18.ghc3.3_dgrad_b133', 133, 2, 32, 64, 128, 3, (1, 1), out_f32=True),
+    case('r18.ghc3.3_dgrad_b219', 219, 2, 32, 64, 128, 3, (1, 1), out_f32=True),
+    case('r18.ghc3.3_dgrad_b265', 265, 2, 32, 64, 128, 3, (1, 1), out_f32=True),
+    case('r18.ghc3.3_b529', 529, 2, 32, 64, 64, 3, (2, 1)),
+    case('r18.ghc3.3_raw_b529', 529, 2, 32, 64, 64, 3, (2, 1), out_f32=True),
+    # 114 SMs
+    case('ghc1.2_b14', 14, 16, 128, 256, 128, 3, (2, 1)),
+    case('ghc1.2_raw_b14', 14, 16, 128, 256, 128, 3, (2, 1), out_f32=True),
+    case('ghc1.3_dgrad_b14', 14, 8, 128, 64, 128, 3, (1, 1), out_f32=True),
+    case('ghc2.1_b7', 7, 16, 64, 256, 512, 3, (2, 1)),
+    case('ghc2.1_raw_b7', 7, 16, 64, 256, 512, 3, (2, 1), out_f32=True),
+    case('ghc2.3_dgrad_b28', 28, 4, 64, 64, 256, 3, (1, 1), out_f32=True),
+    case('ghc3.2_b55', 55, 4, 32, 256, 512, 3, (2, 1)),
+    case('ghc3.2_raw_b55', 55, 4, 32, 256, 512, 3, (2, 1), out_f32=True),
+    case('ghc3.3_dgrad_b55', 55, 2, 32, 256, 512, 3, (1, 1), out_f32=True),
+    case('ghc3.3_b113', 113, 2, 32, 256, 256, 3, (2, 1)),
+    case('ghc3.3_raw_b113', 113, 2, 32, 256, 256, 3, (2, 1), out_f32=True),
+    case('ghc3.3_b229', 229, 2, 32, 256, 256, 3, (2, 1)),
+    case('ghc3.3_raw_b229', 229, 2, 32, 256, 256, 3, (2, 1), out_f32=True),
+    case('layer4.0.conv2_b7', 7, 32, 64, 256, 512, 3, (2, 2)),
+    case('layer4.0.conv2_raw_b7', 7, 32, 64, 256, 512, 3, (2, 2), out_f32=True),
+    case('layer4.1.conv2_b7', 7, 16, 32, 256, 512, 3, (1, 1)),
+    case('layer4.1.conv2_raw_b7', 7, 16, 32, 256, 512, 3, (1, 1), out_f32=True),
+    case('r18.ghc2.1_b28', 28, 16, 64, 64, 128, 3, (2, 1)),
+    case('r18.ghc2.1_raw_b28', 28, 16, 64, 64, 128, 3, (2, 1), out_f32=True),
+    case('r18.ghc2.3_b115', 115, 4, 64, 64, 32, 3, (2, 1)),
+    case('r18.ghc2.3_raw_b115', 115, 4, 64, 64, 32, 3, (2, 1), out_f32=True),
+    case('r18.ghc3.3_dgrad_b115', 115, 2, 32, 64, 128, 3, (1, 1), out_f32=True),
+    case('r18.ghc3.3_dgrad_b229', 229, 2, 32, 64, 128, 3, (1, 1), out_f32=True),
+    case('r18.ghc3.3_b457', 457, 2, 32, 64, 64, 3, (2, 1)),
+    case('r18.ghc3.3_raw_b457', 457, 2, 32, 64, 64, 3, (2, 1), out_f32=True),
+    case('r18.layer4.0.conv2_b7', 7, 16, 32, 256, 512, 3, (1, 1), residual=True),
 ]
 
 ALL_CASES = CASES + F32_CASES + MODEL_CASES

@@ -3,9 +3,9 @@ conv_dgrad_f32), by variant key, and the BatchNorm kernels at the model's channe
 
 CPU (no GPU needed):
 * coverage guard: every variant key (f32_cases.variant_key) that resnet50 or resnet18, with the bi-LSTM or the MLP head,
-  with option tensor_cores on or off, reaches at batch 1 .. 64 on a 132-SM H100 SXM or a 114-SM H100 PCIe is reached by a
-  unit case of f32_cases.CASES planned for the same SM count.  A failure names the missing key and a model launch that
-  reaches it;
+  with option tensor_cores on or off, reaches at any batch the library accepts (tc_cases.ACCEPTED_BATCHES, 1 .. 1024) on a
+  132-SM H100 SXM or a 114-SM H100 PCIe is reached by a unit case of f32_cases.CASES planned for the same SM count.  A
+  failure names the missing key and the first model launch and batch that reach it;
 * every plan of a unit case and of a model launch covers its output once.
 -m gpu:
 * each unit case through hn_conv2d impl 0 (conv) or hn_conv2d_backward (wgrad, dgrad; dgrad also accumulated in place
@@ -35,10 +35,10 @@ def _built():
 
 
 def _model_launches():
-    for backbone in BACKBONES:
-        for use_rnn in (True, False):
-            for tc in (True, False):
-                for B in T.BATCHES:
+    for B in T.ACCEPTED_BATCHES:                          # batch outermost: a failure names the first batch of a key
+        for backbone in BACKBONES:
+            for use_rnn in (True, False):
+                for tc in (True, False):
                     for c in F.model_launches(backbone, use_rnn, B, tc):
                         yield f"{backbone} {'rnn' if use_rnn else 'mlp'} tensor_cores={int(tc)} {c['name']} @ B={B}", c
 

@@ -3,9 +3,9 @@ teacher-forced fp64 replay.
 
 CPU (no GPU needed):
 * census: every key (lstm_cases.variant_key) that the model's recurrence launches (eval forward, training forward, TTA;
-  both layers, T = 256, B = 1 .. 64) or hn_lstm_layer at T = 1, 2, 3 reach on a device with 2 .. 8 co-resident clusters
-  is a unit case of lstm_cases.CASES, and batch_for finds its batch there.  A failure names the missing key and a launch
-  that reaches it;
+  both layers, T = 256, every batch in tc_cases.ACCEPTED_BATCHES, 1 .. 1024) or hn_lstm_layer at T = 1, 2, 3 reach on a
+  device with 2 .. 8 co-resident clusters is a unit case of lstm_cases.CASES, and batch_for finds its batch there.  A
+  failure names the missing key and the first launch and batch that reach it;
 * every plan owns each column once, and takes two groups per cluster exactly when one each would not fit in one wave;
 * hn_lstm_plan rejects T < 1, B < 1 and fewer than 2 co-resident clusters;
 * the bound of gpu_utils.lstm_bound holds for a CPU emulation of the kernel's arithmetic, and fails it with a cross
@@ -40,7 +40,7 @@ def _built():
 def _census(max_clusters):
     """{key: a launch that reaches it} of the model and the ABI's short sequences on max_clusters clusters."""
     keys = {}
-    for B in L.BATCHES:
+    for B in L.ACCEPTED_BATCHES:
         for c in L.model_launches(B) + L.abi_launches(B):
             p = L.plan(c['T'], c['B'], max_clusters)
             assert p is not None, (c, _lib.lib().hn_last_error())
@@ -66,20 +66,24 @@ def test_unit_cases_reach_every_variant_key_of_the_model(max_clusters):
 
 def test_the_census_reaches_the_h100_sxm_layouts():
     """On the 7 clusters of an H100 SXM: the benchmark's batch 32 runs on 4 two-group clusters in one wave, B = 33 .. 39
-    ends on a one-group cluster with a partial group, and B = 49 .. 64 needs a second wave."""
+    ends on a one-group cluster with a partial group, and every batch from 49 (7 groups of 8 columns: 4 cluster pairs,
+    one more than 7 clusters hold) to the largest the library accepts needs a second wave or more."""
     assert L.plan(256, 32, 7) == dict(max_clusters=7, ngroups=4, gpc=2, clusters=4, last_cluster_groups=2,
                                       last_group_cols=8, waves=1)
     for B in range(33, 40):
         k = L.key_dict(L.variant_key(256, L.plan(256, B, 7)))
         assert k['gpc'] == 2 and k['last_cluster_one_group'] and k['partial_group'] and not k['second_wave'], B
-    assert [B for B in L.BATCHES if L.plan(256, B, 7)['waves'] > 1] == list(range(49, 65))
+    plans = {B: L.plan(256, B, 7) for B in L.ACCEPTED_BATCHES}
+    first = min(B for B, p in plans.items() if p['clusters'] > p['max_clusters'])
+    assert first == 49 and plans[first]['clusters'] == 8
+    assert [B for B, p in plans.items() if p['waves'] > 1] == list(range(first, L.ACCEPTED_BATCHES[-1] + 1))
     assert len(L.CASES) == len(set(L.CASES)) == len(L.CASE_KEYS)
 
 
 @pytest.mark.parametrize('max_clusters', L.MAX_CLUSTERS + (9, 16, 132))
 def test_two_groups_per_cluster_exactly_when_one_each_would_not_fit(max_clusters):
     for T in (1, 2, 3, 256):
-        for B in L.BATCHES:
+        for B in L.ACCEPTED_BATCHES:
             p = L.plan(T, B, max_clusters)
             L.check_plan(T, B, p)
             assert (p['gpc'] == 1) == (2 * p['ngroups'] <= max_clusters), (T, B, p)

@@ -2,9 +2,9 @@
 
 CPU (no GPU needed):
 * coverage guard: every variant key (wgrad_cases.variant_key) the training step of resnet50 or resnet18 reaches, with either
-  head, at batch 1 .. 64 on a 132-SM H100 SXM or a 114-SM H100 PCIe, is reached by a unit case of wgrad_cases.CASES planned
-  for the same SM count.  A plan change that sends the model into a new variant fails here until a unit case for it is
-  added;
+  head, at any batch the library accepts (tc_cases.ACCEPTED_BATCHES, 1 .. 1024) on a 132-SM H100 SXM or a 114-SM H100
+  PCIe, is reached by a unit case of wgrad_cases.CASES planned for the same SM count.  A plan change that sends the model
+  into a new variant fails here until a unit case for it is added;
 * every unit case and every model launch has a plan that covers its pixels once (test_wgrad_plan.py's invariants).
 -m gpu:
 * each unit case through hn_conv2d_wgrad_tc against fp64, elementwise, with the bound of gpu_utils.run_wgrad_case; worst
@@ -29,8 +29,8 @@ def _built():
 
 def _model_keys(sms):
     keys = {}
-    for backbone in BACKBONES:
-        for B in T.BATCHES:
+    for B in T.ACCEPTED_BATCHES:                          # batch outermost: a failure names the first batch of a key
+        for backbone in BACKBONES:
             for c in W.model_launches(backbone, B):
                 p = W.plan(c, sms)
                 if p is not None:
@@ -63,7 +63,7 @@ def test_every_weight_gradient_launch_of_the_model_has_a_plan(backbone, sms):
     # conv units the kernel does not take: Cout or Cin not a multiple of 64 (resnet50's ghc0.3; resnet18's narrow
     # height-reduction convs) -- their weight gradients stay on conv_wgrad_f32
     on_tc = {'resnet50': 67 + 5, 'resnet18': 28 + 5}[backbone]                  # conv units + LSTM and MLP rows
-    for B in T.BATCHES:
+    for B in T.ACCEPTED_BATCHES:
         n = 0
         for c in W.model_launches(backbone, B):
             p = W.plan(c, sms)

@@ -145,4 +145,11 @@ CASES = [
     launch('r50.bi_rnn.weight_ih_l1_b1', 1, 1, 256, 128, 128, 1, (1, 1), 'lstm'),
     launch('r50.bi_rnn.weight_ih_l1_b8', 1, 1, 1792, 128, 128, 1, (1, 1), 'lstm'),
     launch('r50.bi_rnn.weight_ih_l1_b8_w1536', 1, 1, 1536, 128, 128, 1, (1, 1), 'lstm'),
+    # batches between those above (none past 64 adds a key)
+    launch('r18.ghc3.3_b31', 31, 2, 32, 128, 64, 3, (2, 1)),
+    launch('r18.ghc3.3_b33', 33, 2, 32, 128, 64, 3, (2, 1)),
+    launch('r18.ghc3.3_b34', 34, 2, 32, 128, 64, 3, (2, 1)),
+    launch('r50.ghc3.3_b47', 31, 2, 32, 128, 128, 3, (2, 1)),
+    launch('r50.ghc3.3_b48', 32, 2, 32, 128, 128, 3, (2, 1)),
+    launch('r50.ghc3.3_b49', 33, 2, 32, 128, 128, 3, (2, 1)),
 ]
